@@ -14,7 +14,12 @@ per-GPU work fixed).  `value` = views of all ranks / max-over-ranks device time,
 `e2e` = same through the public API with the per-view host inputs (camera matrices + uint8 target image in
 pinned memory) copied H2D and the loss read back D2H inside the timed region.
 
-Inputs are larger than L2 (236 MB of parameters are streamed by every view), so no explicit L2 flush is needed.
+Inputs are larger than L2 (236 MB of parameters are streamed by every view, L2 is 50 MB on an H100), so no explicit L2 flush
+is needed.
+
+--dump-outputs DIR writes what the timed path returned in its last timed step: the step's per-view losses and, for a fixed
+seeded sample of DUMP_SAMPLE Gaussians, the accumulated dense gradient of every parameter (plus the per-chunk visibility
+marks), as float32/float64 .npy files, for output-by-output comparison of two builds on the same inputs.
 """
 from __future__ import annotations
 
@@ -37,6 +42,7 @@ import numpy as np  # noqa: E402
 METRIC = "forward+backward views/sec @1080p 1M Gaussians"
 UNIT = "views/s"
 PARAM_KEYS = ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")
+DUMP_SAMPLE = 65536
 
 
 def parse():
@@ -61,6 +67,8 @@ def parse():
     ap.add_argument("--config", default="c2", choices=["c2", "c4"],
                     help="c2 = BASELINE.json configs[1] (1M Gaussians, 1080p: the configuration the metric is quoted on; default); "
                          "c4 = configs[3] (5M Gaussians, 3840x2160, log-scales shifted by -0.5: tile-overflow / sort-bound stress)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's losses and a seeded sample of its accumulated gradients as DIR/<name>.npy")
     ap.add_argument("--allreduce", default="sync", choices=["sync", "overlap"],
                     help="N>1: sync = the step's all-reduce completes before the next step starts (what synchronous training needs; "
                          "headline); overlap = it hides behind the next step's rendering (gradients one step late)")
@@ -77,7 +85,7 @@ def parse():
 # ---------------------------------------------------------------------------------------------------
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md recipe).
+    """nvidia-smi clocks/throttle reasons DURING the timed region.
 
     nvidia-smi needs a few hundred ms to print its first line, longer than a short timed region, so the sampler is started before
     the warm-up steps (the same workload) and every line carries nvidia-smi's own timestamp; stop() keeps the samples whose
@@ -157,6 +165,19 @@ class ClockSampler:
         except Exception:
             pass
         return out
+
+
+def gpu_identity(index: int) -> dict:
+    """The card's name and power limit, stated beside every number this run reports."""
+    import torch
+    out = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(index)],
+                           capture_output=True, text=True, timeout=30)
+        out["power_limit_w"] = float(r.stdout.strip().splitlines()[0])
+    except Exception:
+        pass
+    return out
 
 
 class StageTimer:
@@ -295,7 +316,7 @@ def run_reference(args, rank):
                          "sample": f"{max(1, args.steps)} full-size views, one per step (oracle/, C + OpenMP)"},
         "e2e": {"value": vps, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
     }
-    # informational: the reference's own CUDA kernels (sm_100a build in oracle/_ref) under the same op-level
+    # informational: the reference's own CUDA kernels (sm_90a build in oracle/_ref) under the same op-level
     # orchestration, when a GPU and the prebuilt module are available.
     try:
         line["ref_cuda"] = ref_cuda_views_per_s(args, scene_np)
@@ -306,12 +327,12 @@ def run_reference(args, rank):
 
 def ref_cuda_views_per_s(args, scene_np, iters=24):
     """The GPU-side comparison target (informational keys of the reference line): the reference's OWN CUDA kernels (unmodified
-    sources built for sm_100a, oracle/_ref) against ours under identical orchestration, in two harnesses:
+    sources built for sm_90a, oracle/_ref) against ours under identical orchestration, in two harnesses:
 
       *_cold  : litegs_b200.render Level A (op by op), feedback buffers None -- the reference's first-epoch mode with one blocking
                 size read-back per view (GR/compact.cu:527-549, GR/binning.cu:137-163);
       *_warm  : the reference's own, unmodified Python (litegs.render.render_preprocess + render from the staged package,
-                baseline/_ref) with its pinned feedback buffers filled by a previous pass over the same cameras -- the
+                oracle/_ref/py) with its pinned feedback buffers filled by a previous pass over the same cameras -- the
                 reference's steady-state (best) mode.  `ours_under_reference_python_warm` swaps only the native module."""
     import torch
     if not torch.cuda.is_available():
@@ -365,7 +386,7 @@ def ref_cuda_views_per_s(args, scene_np, iters=24):
     try:
         path = build_ref.reference_python_path()
         if path is None:
-            raise RuntimeError("reference Python package not staged (baseline/_ref)")
+            raise RuntimeError("reference Python package not staged (oracle/_ref/py)")
         from litegs_b200 import shims
         shims.install()
         if path not in sys.path:
@@ -409,16 +430,6 @@ def ref_cuda_views_per_s(args, scene_np, iters=24):
 # ---------------------------------------------------------------------------------------------------
 # ours
 # ---------------------------------------------------------------------------------------------------
-
-# instructions the dominant kernels issue per unit of work, calibrated ONCE per kernel version from an ncu capture
-# (profiles/ncu_raster_r2a_v2_8x16.txt: smsp__inst_executed.sum / work units of that launch) -- the work units themselves are
-# counted in-run, so the issue roofline follows the workload and the clocks of THIS run
-ISSUE_MODEL = {
-    # kernel: (warp instructions per (tile, splat) iteration, description of the unit)
-    "lgs_rasterize_backward": {"8x16": 135.7, "unit": "(tile, splat) iterations = sum over tiles of the deepest consumed list position",
-                               "source": "profiles/ncu_all_kernels_r2g_c2.txt launch 23: 225.07 M warp instructions / 1.659 M iterations"},
-}
-
 
 def run_ours(args, rank, world, local_rank):
     import torch
@@ -501,16 +512,19 @@ def run_ours(args, rank, world, local_rank):
         else:
             a.all_reduce(async_op=False)
 
+    last = {}
+
     def step(serial=False, record=False):
         a = accs[step_no["k"] % len(accs)]
         a.wait()                      # overlap mode: this buffer's previous all-reduce (two steps ago) must have landed
         a.zero_()
         if args.level == "B":
-            run_views(lambda j: cams[j], lambda j, img: (img * w).sum(), serial)
+            losses = run_views(lambda j: cams[j], lambda j, img: (img * w).sum(), serial)
         else:
-            run_views(lambda j: cams[j], lambda j, img: w, serial)
+            losses = run_views(lambda j: cams[j], lambda j, img: w, serial)
         reduce_step(a, record)
         step_no["k"] += 1
+        last.update(losses=losses, acc=a)
 
     def barrier():
         for a in accs:
@@ -539,6 +553,8 @@ def run_ours(args, rank, world, local_rank):
     sampler.mark_end()
     clocks = sampler.stop() if rank == 0 else None
     ms = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        dump_outputs(args.dump_outputs, last["losses"], last["acc"], C_chunks * S)
     comm_ms = sum(a_.elapsed_time(b_) for a_, b_ in comm_events) / max(1, len(comm_events)) if comm_events else 0.0
     # stage attribution / roofline durations: the same steps once more on ONE stream with CUDA events around every
     # C-ABI call (with overlapping streams a kernel's event-to-event time includes the other stream's work).
@@ -766,8 +782,8 @@ def run_ours(args, rank, world, local_rank):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak_gbs = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    peak_gbs = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s"
     summ = timer.summary()
     n_views_rank = vpr * args.steps
     bytes_per = stage_bytes(stats, S, K)
@@ -789,33 +805,13 @@ def run_ours(args, rank, world, local_rank):
             s_["alg_bytes"] = int(b)
             s_["gbs"] = b / (s_["ms_per_view"] / 1000.0) / 1e9
     dom = max(stages.items(), key=lambda kv: kv[1]["ms_per_view"])[0] if stages else None
-    roofline, roofline_issue = None, None
+    roofline = None
     if dom is not None and "gbs" in stages[dom]:
-        traffic, traffic_src = None, None
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json"))).get(dom)
-            if tj and tj.get("tile") == args.tile and tj.get("config", "c2") == args.config:
-                traffic, traffic_src = tj["bytes"], tj.get("source")
-        except Exception:
-            pass
-        # the contract's roofline entry: algorithmic bytes of the dominant kernel over its measured duration against the HBM
-        # peak.  For the raster kernels this fraction is small BY CONSTRUCTION (they are bound by instruction issue: DRAM
-        # throughput 3 % of peak under ncu); `roofline_issue` below is the ceiling that actually bounds them.
+        # algorithmic bytes of the dominant kernel over its measured duration against the HBM peak.  The raster kernels are
+        # not bandwidth-bound, so for them this fraction is small by construction.
         roofline = {"kernel": dom, "bound": "hbm", "achieved": stages[dom]["gbs"], "peak": peak_gbs, "unit": "GB/s",
-                    "frac": stages[dom]["gbs"] / peak_gbs, "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
-                    "alg_bytes_per_launch": stages[dom]["alg_bytes"], "ms_per_launch": stages[dom]["ms_per_view"],
-                    "limiter": "instruction issue, not HBM: see roofline_issue" if dom in ISSUE_MODEL else None}
-        im = ISSUE_MODEL.get(dom)
-        if im is not None and args.tile in im and clocks and clocks.get("sm_mhz"):
-            work = stats["backward_tile_splat_iterations"]
-            inst = im[args.tile] * work
-            sms = torch.cuda.get_device_properties(dev).multi_processor_count
-            peak_ips = sms * 4 * clocks["sm_mhz"] * 1e6                 # one warp instruction per scheduler per cycle, 4 per SM
-            ach = inst / (stages[dom]["ms_per_view"] / 1000.0)
-            roofline_issue = {"kernel": dom, "bound": "sm_issue", "achieved": ach / 1e12, "peak": peak_ips / 1e12,
-                              "unit": "T warp-inst/s", "frac": ach / peak_ips, "work_units_per_launch": work, "unit_of_work": im["unit"],
-                              "warp_inst_per_unit": im[args.tile], "calibration": im["source"], "sm_count": sms,
-                              "sm_mhz_in_run": clocks["sm_mhz"], "ms_per_launch": stages[dom]["ms_per_view"]}
+                    "frac": stages[dom]["gbs"] / peak_gbs, "peak_source": peak_src,
+                    "alg_bytes_per_launch": stages[dom]["alg_bytes"], "ms_per_launch": stages[dom]["ms_per_view"]}
     # whole path = the stages this run actually launched (bytes_per also lists the variants that were not: 32-bit tile keys,
     # the compacted-gradient scatter of level A)
     path_bytes = sum(s_["alg_bytes"] for s_ in stages.values() if "alg_bytes" in s_)
@@ -862,8 +858,8 @@ def run_ours(args, rank, world, local_rank):
                    "backward_kernel": os.environ.get("LGS_BWD", "v2"), "tile_order": os.environ.get("LGS_TILE_ORDER", "1") != "0",
                    "gpu_driven_sizing": bool(pipeline.SYNC_FREE and args.level == "B"), "cuda_graphs": bool(pipeline.GRAPHS_ENABLED and pipeline.SYNC_FREE and args.level == "B" and n_streams > 1),
                    "stage_timing": "serialized pass of the same steps on one stream (CUDA events around every C-ABI call)"},
-        "clocks": clocks, "e2e": e2e, "gpu_launches": int(gpu_launches),
-        "roofline": roofline, "roofline_issue": roofline_issue, "path_roofline": path, "workload_stats": stats, "stages": stages,
+        "gpu": gpu_identity(local_rank), "clocks": clocks, "e2e": e2e, "gpu_launches": int(gpu_launches),
+        "roofline": roofline, "path_roofline": path, "workload_stats": stats, "stages": stages,
     }
     if comm is not None:
         line["comm"] = comm
@@ -875,6 +871,23 @@ def run_ours(args, rank, world, local_rank):
         except Exception as e:
             line["cpu_baseline"] = {"unavailable": str(e)[:200]}
     emit_line(line)
+
+
+def dump_outputs(out_dir, losses, acc, n_gaussians):
+    """The last timed step's results as out_dir/<name>.npy: per-view losses (float64), the per-chunk visibility marks and,
+    for DUMP_SAMPLE Gaussians drawn with a fixed seed (the same ones for the same --gaussians), every parameter's
+    accumulated gradient rows (float32)."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    idx = np.sort(np.random.default_rng(0).choice(n_gaussians, min(DUMP_SAMPLE, n_gaussians), replace=False))
+    pos = torch.from_numpy(idx).to(acc.buf.device)
+    np.save(os.path.join(out_dir, "losses.npy"), np.array([float(x) for x in losses], np.float64))
+    np.save(os.path.join(out_dir, "gaussian_sample_index.npy"), idx.astype(np.float64))
+    for k, g in acc.grads().items():
+        if k == "_touched":
+            np.save(os.path.join(out_dir, "chunk_touched.npy"), g.float().cpu().numpy())
+        else:
+            np.save(os.path.join(out_dir, f"grad_{k}.npy"), g.reshape(-1, n_gaussians)[:, pos].float().cpu().numpy())
 
 
 _REAL_STDOUT = None

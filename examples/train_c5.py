@@ -5,7 +5,7 @@
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 \
         examples/train_c5.py --data /tmp/c5 --trainer ours --iters 7000          # this repository's data-parallel loop (N GPUs)
 
---trainer reference imports the reference package (the mounted tree, or the byte copy staged under baseline/_ref by
+--trainer reference imports the reference package (the LiteGS checkout, or the byte copy staged under oracle/_ref/py by
 oracle/build_ref.py) and calls ``litegs.training.start`` exactly as ``example_train.py:26`` does, with ``litegs_fused`` /
 ``fused_ssim`` resolving to this repository and ``plyfile`` / ``torchmetrics`` / ``matplotlib`` / ``simple_knn`` to the stand-ins of
 ``litegs_b200/shims``.  The reference is single-GPU (SURVEY fact 3), so the multi-GPU half of C5 is --trainer ours: views of a
@@ -48,7 +48,7 @@ def run_reference(data, iters, out_dir, target_primitives):
     from litegs_b200 import shims
     path = build_ref.reference_python_path()
     if path is None:
-        sys.exit("reference Python package not available (neither /root/reference nor baseline/_ref)")
+        sys.exit("reference Python package not available (no LiteGS checkout found and none staged under oracle/_ref/py: see oracle/build_ref.py)")
     shims.install()
     sys.path.insert(1, path)
     import litegs

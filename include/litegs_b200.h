@@ -1,5 +1,5 @@
 /*
- * litegs_b200.h -- C ABI of liblitegs_b200.so, the B200-native (sm_100a) replacement for the hot path of
+ * litegs_b200.h -- C ABI of liblitegs_b200.so, the H100-native (sm_90a) replacement for the hot path of
  * MooreThreads/LiteGS' `litegs_fused` extension (reference: litegs/submodules/gaussian_raster/, "GR/").
  *
  * The reference binds this path through a pybind11 module on at::Tensor (GR/ext_cuda.cpp:9-35); its
@@ -143,7 +143,7 @@ int lgs_tile_range_u16(const unsigned short* table_tile_id, int V, int table_len
  * cub::DeviceRadixSort::SortPairs (GR/binning.cu:204-221) for the tile sort.  keys_in/vals_in are not modified.
  * lgs_set_sort_impl: 1 = own histogram/scan/scatter passes (default), 0 = cub::DeviceRadixSort; env LGS_SORT=lgs|cub. */
 int lgs_set_sort_impl(int impl);
-/* form of the own radix sort: 0 = histogram / row-scan / scatter passes (default, measured faster), 1 = onesweep (global
+/* form of the own radix sort: 0 = histogram / row-scan / scatter passes (default), 1 = onesweep (global
  * histograms in one read + decoupled look-back per pass); env LGS_RS=passes|onesweep */
 int lgs_set_radix_form(int onesweep);
 int lgs_sort_pairs_u16_workspace_bytes(int n, size_t* bytes);
@@ -223,16 +223,16 @@ int lgs_rasterize_backward(const int* sorted_points, const int* start_index, con
                            int tile_w, int enable_statistic, float* packed_grad, float* d_ndc, float* d_cov2d_inv,
                            float* d_color, float* d_opacity, float* err_sum, float* err_square_sum, void* stream);
 
-/* staging selector for the raster kernels: 0 = cp.async / LDGSTS (default, measured faster), 1 = cp.async.bulk + mbarrier */
+/* staging selector for the raster kernels: 0 = cp.async / LDGSTS (default), 1 = cp.async.bulk + mbarrier */
 int lgs_set_staging(int bulk);
 /* warp reduction of the per-(tile,splat) gradient in the backward: 1 = deferred through shared memory (default),
  * 0 = register butterfly */
 int lgs_set_backward_reduce(int deferred);
 /* tiles (warps) per CTA of the raster kernels: 1, 2 or 4 (default 4, env LGS_WPB) */
 int lgs_set_warps_per_block(int wpb);
-/* forward blend on packed pixel pairs (fma.rn.f32x2): 1 on, 0 = scalar predicated body.  env LGS_FWD_PAIRS=0|1 */
+/* forward blend on pixel pairs (two scalar chains side by side): 1 on, 0 = scalar predicated body.  env LGS_FWD_PAIRS=0|1 */
 int lgs_set_forward_pairs(int on);
-/* backward kernel: 2 = packed-pair (fma.rn.f32x2), branch-free pixel body (default); 1 = scalar kernel.  env LGS_BWD=v1|v2 */
+/* backward kernel: 2 = pixel pairs, branch-free pixel body (default); 1 = scalar kernel.  env LGS_BWD=v1|v2 */
 int lgs_set_backward_kernel(int version);
 /* 1 = deterministic backward: per-(tile, splat) sums accumulated as 64-bit fixed point with integer atomics (associative, so
  * two runs give bit-identical gradients; scratch from the stream-ordered allocator); 0 = fp32 RED atomics (default, faster).

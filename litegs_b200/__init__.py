@@ -1,4 +1,4 @@
-"""litegs_b200 -- a B200-native (sm_100a) differentiable 3D Gaussian Splatting render path behind MooreThreads/LiteGS's
+"""litegs_b200 -- an H100-native (sm_90a) differentiable 3D Gaussian Splatting render path behind MooreThreads/LiteGS's
 operator surface.
 
     fused       the 26 entry points of the reference's ``litegs_fused`` pybind module, on the C ABI (include/litegs_b200.h)

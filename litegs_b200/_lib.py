@@ -98,7 +98,7 @@ def load() -> ctypes.CDLL:
         return _lib
     if not os.path.exists(LIB_PATH):
         raise LiteGSB200Error(
-            f"{LIB_PATH} not found: build it with `python -m litegs_b200.build` (nvcc, sm_100a). "
+            f"{LIB_PATH} not found: build it with `python -m litegs_b200.build` (nvcc, sm_90a). "
             "litegs_b200 has no CPU or PyTorch fallback.")
     lib = ctypes.CDLL(LIB_PATH)
     for name, argtypes in SIGNATURES.items():

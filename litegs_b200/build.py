@@ -1,4 +1,4 @@
-"""Builds liblitegs_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Builds liblitegs_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
 One translation unit per .cu, compiled in parallel, linked into a single C-ABI shared library that
 depends on nothing but cudart.  ``python -m litegs_b200.build`` or ``__graft_entry__.build()``.
@@ -15,9 +15,9 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_obj")
 LIB = os.path.join(HERE, "liblitegs_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-# $CXX in this image is a gcc without libgomp; the system one is a safe host compiler for nvcc.
+# the system g++ is preferred as nvcc's host compiler: a $CXX set by the environment may lack libgomp.
 HOST_CXX = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "-ccbin", HOST_CXX, "--expt-relaxed-constexpr"]
 
 
@@ -54,7 +54,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as ex:
         objs = list(ex.map(lambda s: _compile(s, verbose), _sources()))
     if force or not os.path.exists(LIB) or any(os.path.getmtime(o) > os.path.getmtime(LIB) for o in objs):
-        cmd = [NVCC, "-shared", "-ccbin", HOST_CXX, "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB, *objs,
+        cmd = [NVCC, "-shared", "-ccbin", HOST_CXX, "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB, *objs,
                "-cudart", "shared"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:

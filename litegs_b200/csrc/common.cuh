@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for the litegs_b200 CUDA library (sm_100a only).
+// common.cuh -- shared helpers for the litegs_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

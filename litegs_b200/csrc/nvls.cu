@@ -3,7 +3,7 @@
 // sum of its slice from all replicas with multimem.ld_reduce and pushes it back to all replicas with multimem.st -- "two-shot"
 // all-reduce with the reduction done inside the switch, 16 bytes per instruction.  Per GPU and direction the links carry the
 // buffer once (+1/world), the NVLS algorithm NCCL uses; what the own kernel removes is the protocol / channel overhead of the
-// library call (236 MB at 8 GPUs: 0.68 ms through ncclAllReduce).
+// library call.
 //
 // The buffer must be symmetric memory mapped for multicast (torch.distributed._symmetric_memory: empty + rendezvous ->
 // multicast_ptr); the caller brackets the launch with cross-GPU barriers on the same stream (all replicas complete before the

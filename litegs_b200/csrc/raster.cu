@@ -1,7 +1,7 @@
 // raster.cu -- per-tile front-to-back alpha compositing and the matching back-to-front backward.
 //                                                                 replaces GR/raster.cu (all of it)
 //
-// Design (B200 / sm_100a, no tensor-core work: there is no dense contraction here):
+// Design (H100 / sm_90a, no tensor-core work: there is no dense contraction here):
 //  * one warp owns one tile (8x16, 12x16, 16x16 or 8x8 pixels); a lane owns a column strip of
 //    PPT = TH*TW/32 pixels, so the splat's quadratic form is evaluated with dx fixed per lane and two
 //    FMAs per pixel; transmittance, colour and the contributor count live in registers;
@@ -18,8 +18,7 @@
 //    matrix (default: 9 conflict-free STS per splat, every 3 splats 27 lanes each add up one row with
 //    8 LDS.128) or a 9-shuffle transposing butterfly -- and leave the SM exactly once, as one
 //    RED.ADD.F32 per value touching a single 48-byte record.
-//  * backward v2 (default): the per-pixel math runs on PAIRS of pixels with packed fp32 (fma/mul/add.rn.f32x2 ->
-//    FFMA2/FMUL2/FADD2: one issue slot per two lanes of work), the "does this splat touch this pixel" test zeroes the
+//  * backward v2 (default): the per-pixel math runs on PAIRS of pixels (add2/mul2/fma2), the "does this splat touch this pixel" test zeroes the
 //    Gaussian weight instead of branching around the body (every lane executes straight-line code), the 9 values that
 //    leave the warp are RAW moments (sum dx*s0, sum s1, sum dx^2*s0, sum dx*s1, sum s2, colour, sum s0) whose conic
 //    factors are applied once per splat by the consumer (unpack / project_backward) instead of once per (tile, splat, lane),
@@ -45,6 +44,12 @@ __device__ __forceinline__ float fast_rcp(float x)
     asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
+
+// Pixel-pair arithmetic.  sm_90 has no packed fp32 instructions, so each is two scalar single-rounded ops (FADD/FMUL/FFMA),
+// the same per-lane results a packed f32x2 instruction gives; the pair layout keeps the two pixels' chains side by side.
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
 
 // One pixel of the front-to-back blend as straight predicated code (no branches, no selects):
 //   act = Ts > TS_MIN ; n += act ; ok = act && a >= A_MIN ; if ok { w = a*Ts ; C += c*w ; Ts -= (255/256) w }
@@ -209,7 +214,7 @@ __global__ void pack_kernel(const float* __restrict__ ndc, const float* __restri
 }
 
 // ---- forward ---------------------------------------------------------------------------------------
-// PAIRS: blend the lane's pixels two at a time with packed fp32 (A/B switch, lgs_set_forward_pairs / env LGS_FWD_PAIRS).
+// PAIRS: blend the lane's pixels two at a time (add2/mul2/fma2; A/B switch, lgs_set_forward_pairs / env LGS_FWD_PAIRS).
 template <int TH, int TW, bool STAT, bool BULK, bool PAIRS = false>
 __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_forward_kernel(
     const int* __restrict__ sorted, const int* __restrict__ start_index, const SplatRec* __restrict__ recs,
@@ -271,8 +276,8 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_forward_kernel(
                 if ((k & 3) == 0) {
                     // tile-wide early out, tested every 4th splat: a saturated pixel blends nothing and counts
                     // nothing, so running up to 3 splats past the point where the last pixel saturates is exact.
-                    // (Skipping individual saturated pixel ROWS with warp-uniform branches was measured 35-65 % SLOWER:
-                    //  the branches serialise the 8 independent pixel chains the scheduler otherwise interleaves.)
+                    // (Individual saturated pixel ROWS are not skipped with warp-uniform branches: the branches would
+                    //  serialise the independent pixel chains the scheduler otherwise interleaves.)
                     float tmax = Ts[0];
 #pragma unroll
                     for (int j = 1; j < PPT; j++) tmax = fmaxf(tmax, Ts[j]);
@@ -288,7 +293,7 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_forward_kernel(
                 const float os = q2.y;
                 int fcount = 0; float wsum = 0.f;
                 if (PAIRS && !STAT) {
-                    // packed-pair form (fma/mul/add.rn.f32x2): the two pixels of a pair share every instruction of the chain;
+                    // pair form (add2/mul2/fma2): the two pixels of a pair run the same chain side by side;
                     // a pixel that is saturated or below the alpha threshold blends with weight 0, which is an exact no-op
                     const float2 dy02 = make_float2(dy0, dy0), c22 = make_float2(c2, c2), lin2 = make_float2(lin, lin),
                                  base2 = make_float2(base, base), os2 = make_float2(os, os);
@@ -296,19 +301,19 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_forward_kernel(
                                  nki2 = make_float2(-KI, -KI);
 #pragma unroll
                     for (int p = 0; p < PPT / 2; p++) {
-                        const float2 dy = __fadd2_rn(dy02, make_float2(-(float)(2 * p), -(float)(2 * p + 1)));
-                        const float2 pw = __ffma2_rn(dy, __ffma2_rn(c22, dy, lin2), base2);
-                        const float2 t = __fmul2_rn(os2, make_float2(fast_ex2(pw.x), fast_ex2(pw.y)));
+                        const float2 dy = add2(dy02, make_float2(-(float)(2 * p), -(float)(2 * p + 1)));
+                        const float2 pw = fma2(dy, fma2(c22, dy, lin2), base2);
+                        const float2 t = mul2(os2, make_float2(fast_ex2(pw.x), fast_ex2(pw.y)));
                         const float a0 = __saturatef(t.x), a1 = __saturatef(t.y);      // min(alpha, 255/256) * 256/255
                         const bool act0 = Ts[2 * p] > TS_MIN, act1 = Ts[2 * p + 1] > TS_MIN;
                         if (act0) nf[2 * p] += 1.0f;
                         if (act1) nf[2 * p + 1] += 1.0f;
                         const float2 aw = make_float2((act0 && a0 >= A_MIN_S) ? a0 : 0.0f, (act1 && a1 >= A_MIN_S) ? a1 : 0.0f);
-                        const float2 w = __fmul2_rn(aw, make_float2(Ts[2 * p], Ts[2 * p + 1]));
-                        const float2 r2 = __ffma2_rn(cr2, w, make_float2(Cr[2 * p], Cr[2 * p + 1]));
-                        const float2 g2 = __ffma2_rn(cg2, w, make_float2(Cg[2 * p], Cg[2 * p + 1]));
-                        const float2 b2_ = __ffma2_rn(cb2, w, make_float2(Cb[2 * p], Cb[2 * p + 1]));
-                        const float2 tn = __ffma2_rn(nki2, w, make_float2(Ts[2 * p], Ts[2 * p + 1]));
+                        const float2 w = mul2(aw, make_float2(Ts[2 * p], Ts[2 * p + 1]));
+                        const float2 r2 = fma2(cr2, w, make_float2(Cr[2 * p], Cr[2 * p + 1]));
+                        const float2 g2 = fma2(cg2, w, make_float2(Cg[2 * p], Cg[2 * p + 1]));
+                        const float2 b2_ = fma2(cb2, w, make_float2(Cb[2 * p], Cb[2 * p + 1]));
+                        const float2 tn = fma2(nki2, w, make_float2(Ts[2 * p], Ts[2 * p + 1]));
                         Cr[2 * p] = r2.x; Cr[2 * p + 1] = r2.y; Cg[2 * p] = g2.x; Cg[2 * p + 1] = g2.y;
                         Cb[2 * p] = b2_.x; Cb[2 * p + 1] = b2_.y; Ts[2 * p] = tn.x; Ts[2 * p + 1] = tn.y;
                     }
@@ -574,16 +579,15 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_kernel(
     st.drain();
 }
 
-// ---- backward v2: packed fp32 pairs, branch-free pixel body ----------------------------------------------------------
+// ---- backward v2: pixel pairs, branch-free pixel body ----------------------------------------------------------------
 // Same tiling, staging, chunk walk and shared-memory transposed reduction as raster_backward_kernel<.., DEFER=true>, with
-//  * a lane's PPT pixels handled as PPT/2 PAIRS held in float2 registers; every add/mul/fma of the per-pixel chain is one
-//    packed instruction for the pair (FADD2/FMUL2/FFMA2: half the issue slots of the scalar chain, which is what bounds
-//    this kernel -- profiles/ncu_raster_r1b_8x16_cpasync.txt: issue slots busy 79 %, DRAM 1.5 %);
+//  * a lane's PPT pixels handled as PPT/2 PAIRS held in float2 registers (add2/mul2/fma2), the two chains of a pair
+//    independent and interleaved;
 //  * no branch around the pixel body: a pixel the splat does not reach (alpha below 1/256, or the pixel had already
 //    stopped before this list position) gets its Gaussian weight G forced to 0, which makes every term of the chain an
 //    exact no-op (a = 0, 1/(1-a) = 1, T and S unchanged, all gradient terms +0);
 //  * d opacity = sum(G dalpha) = sum(dpw) / o, so the ninth reduced value is the s0 moment itself;
-//  * the transposed row sums of the flush use packed adds on the LDS.128 pairs.
+//  * the transposed row sums of the flush add the LDS.128 halves pairwise.
 // STAT adds the densification error term in one of two forms (err_mode): 1 = the reference's lane-running recurrence
 // (GR/raster.cu:779-784: after each executed pixel PAIR the lane's running sum of G dalpha over its even rows and over its
 // odd rows is squared and added), 0 = sum over pixels of (G dalpha)^2.
@@ -657,17 +661,17 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
         if (lane < pend * NV) {
             const float4* r4 = reinterpret_cast<const float4*>(&s_acc[warp][lane][0]);
             const float4 x0 = r4[0], x1 = r4[1], x2 = r4[2], x3 = r4[3], x4 = r4[4], x5 = r4[5], x6 = r4[6], x7 = r4[7];
-            float2 p0 = __fadd2_rn(make_float2(x0.x, x0.y), make_float2(x0.z, x0.w));
-            float2 p1 = __fadd2_rn(make_float2(x1.x, x1.y), make_float2(x1.z, x1.w));
-            float2 p2 = __fadd2_rn(make_float2(x2.x, x2.y), make_float2(x2.z, x2.w));
-            float2 p3 = __fadd2_rn(make_float2(x3.x, x3.y), make_float2(x3.z, x3.w));
-            float2 p4 = __fadd2_rn(make_float2(x4.x, x4.y), make_float2(x4.z, x4.w));
-            float2 p5 = __fadd2_rn(make_float2(x5.x, x5.y), make_float2(x5.z, x5.w));
-            float2 p6 = __fadd2_rn(make_float2(x6.x, x6.y), make_float2(x6.z, x6.w));
-            float2 p7 = __fadd2_rn(make_float2(x7.x, x7.y), make_float2(x7.z, x7.w));
-            p0 = __fadd2_rn(p0, p1); p2 = __fadd2_rn(p2, p3); p4 = __fadd2_rn(p4, p5); p6 = __fadd2_rn(p6, p7);
-            p0 = __fadd2_rn(p0, p2); p4 = __fadd2_rn(p4, p6);
-            p0 = __fadd2_rn(p0, p4);
+            float2 p0 = add2(make_float2(x0.x, x0.y), make_float2(x0.z, x0.w));
+            float2 p1 = add2(make_float2(x1.x, x1.y), make_float2(x1.z, x1.w));
+            float2 p2 = add2(make_float2(x2.x, x2.y), make_float2(x2.z, x2.w));
+            float2 p3 = add2(make_float2(x3.x, x3.y), make_float2(x3.z, x3.w));
+            float2 p4 = add2(make_float2(x4.x, x4.y), make_float2(x4.z, x4.w));
+            float2 p5 = add2(make_float2(x5.x, x5.y), make_float2(x5.z, x5.w));
+            float2 p6 = add2(make_float2(x6.x, x6.y), make_float2(x6.z, x6.w));
+            float2 p7 = add2(make_float2(x7.x, x7.y), make_float2(x7.z, x7.w));
+            p0 = add2(p0, p1); p2 = add2(p2, p3); p4 = add2(p4, p5); p6 = add2(p6, p7);
+            p0 = add2(p0, p2); p4 = add2(p4, p6);
+            p0 = add2(p0, p4);
             const float sum = p0.x + p0.y;
             const int sp = lane / NV, v = lane - sp * NV;
             const int pid = s_pid[warp][sp];
@@ -716,42 +720,42 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
             bool any = false;
 #pragma unroll
             for (int p = 0; p < NP; p++) {
-                const float2 dy = __fadd2_rn(dy02, make_float2(-(float)(2 * p), -(float)(2 * p + 1)));
-                const float2 pw = __ffma2_rn(dy, __ffma2_rn(c22, dy, lin2), base2);      // same two roundings as the forward's fmaf chain
+                const float2 dy = add2(dy02, make_float2(-(float)(2 * p), -(float)(2 * p + 1)));
+                const float2 pw = fma2(dy, fma2(c22, dy, lin2), base2);      // same two roundings as the forward's fmaf chain
                 float2 G = make_float2(fast_ex2(pw.x), fast_ex2(pw.y));
                 // contribution test = the forward's expression bit for bit (os * G >= A_MIN_S), and the pixel must still have
                 // been active at list position k
-                const float2 tt = __fmul2_rn(os2, G);
+                const float2 tt = mul2(os2, G);
                 const bool ok0 = (tt.x >= A_MIN_S) && (k < nl[2 * p]);
                 const bool ok1 = (tt.y >= A_MIN_S) && (k < nl[2 * p + 1]);
                 any |= ok0 | ok1;
                 G.x = ok0 ? G.x : 0.0f;
                 G.y = ok1 ? G.y : 0.0f;
-                const float2 at = __fmul2_rn(o2, G);
+                const float2 at = mul2(o2, G);
                 const float2 a = make_float2(fminf(at.x, ALPHA_MAX), fminf(at.y, ALPHA_MAX));
-                const float2 om = __ffma2_rn(a, bc2(-1.0f), bc2(1.0f));                  // 1 - a
+                const float2 om = fma2(a, bc2(-1.0f), bc2(1.0f));                  // 1 - a
                 const float2 rc = make_float2(fast_rcp(om.x), fast_rcp(om.y));
-                const float2 Tn = __fmul2_rn(T[p], rc);                                  // transmittance in front of this splat
+                const float2 Tn = mul2(T[p], rc);                                  // transmittance in front of this splat
                 T[p] = Tn;                                                               // (rc = 1 exactly where G was zeroed)
-                const float2 w = __fmul2_rn(a, Tn);
-                const float2 cgd = __ffma2_rn(cr2, g0[p], __ffma2_rn(cg2, g1[p], __fmul2_rn(cb2, g2[p])));
-                const float2 diff = __ffma2_rn(S[p], bc2(-1.0f), cgd);                   // (c - R) . g
-                float2 da = __fmul2_rn(Tn, diff);
-                if (TRANS) da = __ffma2_rn(ngt[p], rc, da);
-                S[p] = __ffma2_rn(a, diff, S[p]);
-                const float2 dpw = __fmul2_rn(at, da);      // passes through the 255/256 clamp (GR/raster.cu:776-778)
-                const float2 td = __fmul2_rn(dpw, dy);
+                const float2 w = mul2(a, Tn);
+                const float2 cgd = fma2(cr2, g0[p], fma2(cg2, g1[p], mul2(cb2, g2[p])));
+                const float2 diff = fma2(S[p], bc2(-1.0f), cgd);                   // (c - R) . g
+                float2 da = mul2(Tn, diff);
+                if (TRANS) da = fma2(ngt[p], rc, da);
+                S[p] = fma2(a, diff, S[p]);
+                const float2 dpw = mul2(at, da);      // passes through the 255/256 clamp (GR/raster.cu:776-778)
+                const float2 td = mul2(dpw, dy);
                 if (p == 0) {
-                    dr = __fmul2_rn(w, g0[p]); dg = __fmul2_rn(w, g1[p]); db = __fmul2_rn(w, g2[p]);
-                    s0 = dpw; s1 = td; s2 = __fmul2_rn(td, dy);
+                    dr = mul2(w, g0[p]); dg = mul2(w, g1[p]); db = mul2(w, g2[p]);
+                    s0 = dpw; s1 = td; s2 = mul2(td, dy);
                 } else {
-                    dr = __ffma2_rn(w, g0[p], dr); dg = __ffma2_rn(w, g1[p], dg); db = __ffma2_rn(w, g2[p], db);
-                    s0 = __fadd2_rn(s0, dpw);
-                    s1 = __fadd2_rn(s1, td);
-                    s2 = __ffma2_rn(td, dy, s2);
+                    dr = fma2(w, g0[p], dr); dg = fma2(w, g1[p], dg); db = fma2(w, g2[p], db);
+                    s0 = add2(s0, dpw);
+                    s1 = add2(s1, td);
+                    s2 = fma2(td, dy, s2);
                 }
                 if (STAT) {
-                    const float2 go = __fmul2_rn(G, da);
+                    const float2 go = mul2(G, da);
                     if (err_mode == 1) {
                         if (__any_sync(FULL_MASK, ok0 | ok1)) {      // the reference skips a pair no lane of the warp reaches
                             runx += go.x; runy += go.y;
@@ -871,7 +875,7 @@ static int g_use_bulk = -1;
 static bool use_bulk()
 {
     if (g_use_bulk < 0) {
-        // "cpasync" (default: measured 12-20 % faster on B200 for this 48-byte-per-lane gather, profiles/sweep_r1.txt)
+        // "cpasync" (default: three 16-byte cp.async per lane for this 48-byte-per-lane gather)
         // | "bulk" (cp.async.bulk + mbarrier)
         const char* e = getenv("LGS_STAGING");
         g_use_bulk = (e && e[0] == 'b') ? 1 : 0;
@@ -892,7 +896,7 @@ static bool use_deferred_reduce()
 }
 extern "C" int lgs_set_backward_reduce(int deferred) { g_defer = deferred ? 1 : 0; return LGS_OK; }
 
-// forward blend: 1 = packed pixel pairs, 0 = scalar predicated PTX body.  env LGS_FWD_PAIRS=0|1
+// forward blend: 1 = pixel pairs, 0 = scalar predicated PTX body.  env LGS_FWD_PAIRS=0|1
 static int g_fwd_pairs = -1;
 static bool forward_pairs()
 {
@@ -904,7 +908,7 @@ static bool forward_pairs()
 }
 extern "C" int lgs_set_forward_pairs(int on) { g_fwd_pairs = on ? 1 : 0; return LGS_OK; }
 
-// backward kernel: 2 = packed-pair kernel (default), 1 = the scalar kernel (kept as A/B and for the TMA staging variant).
+// backward kernel: 2 = pixel-pair kernel (default), 1 = the scalar kernel (kept as A/B and for the TMA staging variant).
 // env LGS_BWD=v1|v2
 static int g_bwd = -1;
 static int backward_version()
@@ -923,7 +927,7 @@ extern "C" int lgs_set_backward_kernel(int version)
 }
 
 // densification error statistic (enable_statistic): 1 = the reference's lane-running recurrence (GR/raster.cu:779-784,
-// default), 0 = sum over pixels of (G dalpha)^2.  Only the packed-pair kernel implements mode 1.
+// default), 0 = sum over pixels of (G dalpha)^2.  Only the pixel-pair kernel implements mode 1.
 static int g_err_mode = 1;
 extern "C" int lgs_set_err_square_mode(int mode)
 {

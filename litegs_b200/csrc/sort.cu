@@ -9,8 +9,7 @@
 //     orders the tile in shared memory and writes it out as one coalesced run per digit.  Digit width is
 //     chosen per call so that ceil(bits / passes) bits are sorted per pass: 14 tile bits = 2 x 7,
 //     16 = 2 x 8, 24 depth bits = 3 x 8.  Blocks are 256 threads x 8 or 16 keys, so a 1M-key depth sort
-//     still launches 490 blocks (cub's onesweep launches 109 blocks of 384 x 23 keys on the same input and
-//     is latency bound at 18 us per pass -- profiles/ncu_sort_r1.txt).
+//     still launches 490 blocks (cub's onesweep launches 109 blocks of 384 x 23 keys on the same input).
 //   * "cub": cub::DeviceRadixSort::SortPairs (onesweep), kept as the cross-check and fallback.
 // Both are stable and sort exactly the bits [begin_bit, end_bit); results are bit-identical.
 #include <cub/device/device_radix_sort.cuh>
@@ -39,9 +38,9 @@ int sort_impl()
     return g_sort_impl;
 }
 
-// Automatic choice when nothing is forced: the own passes win up to 7-bit digits (1080p: 14 tile bits = 2 x 7, 163 vs 186 us for
-// 10.9 M pairs), cub's onesweep wins when the tile ids need 8-bit digits on tens of millions of pairs (4K: 16 bits, 71.7 M pairs:
-// 0.90 vs 1.26 ms) -- profiles/microbench/dev_count_bench.py.
+// Automatic choice when nothing is forced: the own passes up to 7-bit digits (1080p: 14 tile bits = 2 x 7), cub's onesweep when
+// the tile ids need 8-bit digits on more than 8 M pairs (4K: 16 bits, 71.7 M pairs) -- profiles/microbench/dev_count_bench.py
+// times both.
 int sort_impl_for(int n, int bits, unsigned bias)
 {
     int impl = sort_impl();
@@ -133,7 +132,7 @@ __global__ void __launch_bounds__(RS_THREADS) rs_scan_rows_kernel(int* __restric
 // of match slots, one __syncwarp later item j reads the count of its digit, the group sizes of that digit in the items before it
 // and its own group's mask -- all independent loads -- and the highest lane of every group publishes the group size with one
 // ATOMS.ADD.  The three warp barriers and the dependent ATOMS -> LDS -> STS chain of a round are paid once per NS keys instead of
-// once per key (the kernel was latency bound: 0.57 eligible warps per scheduler, profiles/ncu_all_kernels_r2_c2.txt launch 16).
+// once per key (the per-key form is latency bound).
 template <typename KeyT, int IPT, int NS>
 __global__ void __launch_bounds__(RS_THREADS, IPT == 16 ? 3 : 4) rs_scatter_kernel(const KeyT* __restrict__ kin, const unsigned* __restrict__ vin,
                                                                 KeyT* __restrict__ kout, unsigned* __restrict__ vout, int n, int shift,
@@ -185,8 +184,7 @@ __global__ void __launch_bounds__(RS_THREADS, IPT == 16 ? 3 : 4) rs_scatter_kern
 #pragma unroll
     for (int i0 = 0; i0 < IPT; i0 += NS) {
         // lanes of this warp holding the same digit: OR the lane bits into the digit's slot (one ATOMS; MATCH.ANY
-        // issues about once per 64 cycles per SM on sm_100 and alone bounded this kernel, eight ballots cost ~32
-        // issue slots)
+        // issues at a low rate and alone bounded this kernel, eight ballots cost ~32 issue slots)
         unsigned d[NS];
 #pragma unroll
         for (int q = 0; q < NS; q++) {
@@ -249,7 +247,7 @@ __global__ void __launch_bounds__(RS_THREADS, IPT == 16 ? 3 : 4) rs_scatter_kern
 // per pass that ranks a tile, obtains the number of same-digit keys in all EARLIER tiles by decoupled look-back (each tile
 // publishes its per-digit counts, then its inclusive prefix, in one 32-bit word per digit: 2 flag bits + 30-bit count) and
 // scatters.  Against the histogram / row-scan / scatter passes above this removes, per pass, one full read of the keys and two
-// latency-bound launches (the row scan alone is 6-10 us of a 13 us ... 60 us pass, profiles/ncu_all_kernels_r2_c2.txt).
+// latency-bound launches.
 // The ranking and the shared-memory reorder are the ones of rs_scatter_kernel.  Tiles take their index from an atomic ticket, so a
 // tile's predecessors have always started: the look-back cannot dead-lock whatever order the hardware dispatches CTAs in.
 constexpr unsigned LB_AGG = 1u << 30, LB_INC = 2u << 30, LB_MASK = (1u << 30) - 1u;
@@ -465,7 +463,7 @@ int rs_sort(const KeyT* keys_in, KeyT* keys_out, const unsigned* vals_in, unsign
         rs_scan_rows_kernel<<<nbins, RS_THREADS, 0, st>>>(table, p.nblocks, totals);
         LGS_CHECK_LAUNCH("rs_scan_rows_kernel");
         // keys ranked per round: as many as the match slots fit in the value staging buffer they alias (env LGS_RS_RANK caps it: A/B)
-        static const int rank_cap = getenv("LGS_RS_RANK") ? atoi(getenv("LGS_RS_RANK")) : 2;   // measured: 172 / 166 / 172 us at 1 / 2 / 4 (profiles/rank_ab_r2.txt)
+        static const int rank_cap = getenv("LGS_RS_RANK") ? atoi(getenv("LGS_RS_RANK")) : 2;
         int ns = 1;
         while (ns < 4 && ns * 2 <= rank_cap && ns * 2 * RS_WARPS * nbins <= p.tile) ns *= 2;
 #define RS_SCATTER(IPT_, NS_) rs_scatter_kernel<KeyT, IPT_, NS_><<<p.nblocks, RS_THREADS, 0, st>>>(ksrc, vsrc, kdst, vdst, n, bit, nbins, \
@@ -481,9 +479,8 @@ int rs_sort(const KeyT* keys_in, KeyT* keys_out, const unsigned* vals_in, unsign
 }
 
 // 0 = histogram / row-scan / scatter passes (default), 1 = onesweep form.  env LGS_RS=passes|onesweep
-// Measured on B200 (profiles/microbench/dev_count_bench.py): 10.9 M tile pairs on 14 bits 169 us (passes) vs 232 us (onesweep),
-// 1 M depth keys on 24 bits 64.6 vs 66.7 us: with one thread per digit walking back one predecessor per dependent load, the
-// look-back of the ~900 concurrently resident tiles costs more than the histogram read and the row scan it saves.
+// With one thread per digit walking back one predecessor per dependent load, the look-back of the concurrently resident tiles
+// costs more than the histogram read and the row scan it saves (profiles/microbench/dev_count_bench.py times both forms).
 int g_rs_onesweep = -1;
 bool rs_use_onesweep()
 {

@@ -5,8 +5,7 @@
 // Same maths as the reference (11-tap sigma-1.5 Gaussian, zero padding, separable, per channel; the partial derivatives
 // dm/dmu1, dm/dsigma1^2, dm/dsigma12 are saved by the forward and filtered again by the backward), different schedule.
 // The reference stages a 26x26 window per 16x16 tile and keeps a 5-channel intermediate image in shared memory; that costs
-// ~130 shared-memory accesses and ~440 issued instructions per output and caps occupancy at 25 % on B200 (first version of
-// this file, profiles/ncu_ssim_r1_tiled_first_version.txt).  Here a CTA is a band of 128 columns x 32 rows and every thread streams DOWN
+// ~130 shared-memory accesses and ~440 issued instructions per output.  Here a CTA is a band of 128 columns x 32 rows and every thread streams DOWN
 // one column:
 //   * vertical pass in registers, straight from global memory (coalesced across the warp, 11 rows of loads in flight):
 //     each incoming row is scattered into the 11 pending output rows of a register ring (statically indexed: the row loop

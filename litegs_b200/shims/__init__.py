@@ -11,7 +11,7 @@ top of ``litegs_fused`` / ``fused_ssim`` from this repository.  Each shim implem
   simple_knn     simple_knn._C.distCUDA2(points[N,3]) -> mean squared distance to the 3 nearest neighbours
 
 ``install()`` appends this directory to ``sys.path`` -- AFTER site-packages, so a real installation of any of the four
-always wins -- and makes the repository root importable so that ``litegs_fused`` and ``fused_ssim`` resolve to the B200
+always wins -- and makes the repository root importable so that ``litegs_fused`` and ``fused_ssim`` resolve to this
 implementation.  Nothing in ``litegs_b200`` itself imports these shims."""
 from __future__ import annotations
 

@@ -1,5 +1,5 @@
 """Host mirror of the reference's ``fused_ssim`` package (fused_ssim/fused_ssim/__init__.py:1-90 above the pybind module
-fused_ssim/ext.cpp:4-9) on the B200 kernels of csrc/ssim.cu.
+fused_ssim/ext.cpp:4-9) on the kernels of csrc/ssim.cu.
 
 Same names, argument order and semantics:
 

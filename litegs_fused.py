@@ -1,4 +1,4 @@
-"""Drop-in module: ``import litegs_fused`` resolves to the B200-native implementation.
+"""Drop-in module: ``import litegs_fused`` resolves to the H100-native implementation.
 
 The reference imports its CUDA extension by this name (litegs/utils/wrapper.py:8-12).  With this repository
 root on ``sys.path`` -- ahead of any installed ``litegs_fused`` -- the reference's wrapper.py, render/__init__.py,

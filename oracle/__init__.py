@@ -10,7 +10,7 @@ module (``GR/ext_cuda.cpp:9-35``) so that parity tests read like calls into the 
 
 Parity pinning: the reference ships no CPU path and no golden vectors for this path (SURVEY.md 8c).
 The oracle is pinned against the reference's own CUDA kernels (``oracle/build_ref.py`` builds them
-into ``oracle/_ref``; ``tests/golden/make_golden.py`` runs them on a B200 and writes fixtures).
+into ``oracle/_ref``; ``tests/golden/make_golden.py`` runs them on an H100 and writes fixtures).
 """
 from __future__ import annotations
 

@@ -1,10 +1,12 @@
-"""Recipe that compiles the UNMODIFIED reference extension (litegs/submodules/gaussian_raster) for sm_100a.
+"""Recipe that compiles the UNMODIFIED reference extension (litegs/submodules/gaussian_raster) for sm_90a (H100).
 
-TEST INFRASTRUCTURE ONLY.  Sources are compiled where they lie under /root/reference (nothing is
-copied into this repository); the only outputs are ``oracle/_ref/litegs_fused_ref.so`` and ``oracle/_ref/fused_ssim_cuda_ref.so`` (git-ignored,
-NOT gpurun-ignored, so it travels to the GPU box).  It is the "reference itself run here" that pins the
-CPU oracle (tests/test_gpu_vs_reference.py, tests/golden/make_golden.py) and the CUDA baseline that
-``bench.py`` times next to ours ("ref_cuda").  Flags are the reference's own: -O3 --use_fast_math
+TEST INFRASTRUCTURE ONLY.  The reference checkout is the one the environment variable LITEGS_REFERENCE names, else a LiteGS
+checkout next to this repository (``../reference`` or ``../LiteGS``).  Sources are compiled where they lie (nothing is copied
+into this repository); the outputs are ``oracle/_ref/litegs_fused_ref.so``, ``oracle/_ref/fused_ssim_cuda_ref.so`` and the
+staged Python package under ``oracle/_ref/py`` (all git-ignored; a machine that runs the tests without the checkout needs
+only a copy of ``oracle/_ref``).  They are the "reference itself"
+whose outputs tests/golden/make_golden*.py store as the fixtures that pin the CPU oracle and our kernels, and the CUDA
+baseline that ``bench.py --impl reference`` times next to ours ("ref_cuda").  Flags are the reference's own: -O3 --use_fast_math
 (GR/setup.py:33-36) plus the arch.  The reference's build system (setup.py / CMake) is not run.
 """
 from __future__ import annotations
@@ -15,12 +17,31 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 OUT = os.path.join(HERE, "_ref")
-REF_GR = "/root/reference/litegs/submodules/gaussian_raster"
+
+
+def _find_reference() -> str:
+    """$LITEGS_REFERENCE, else a LiteGS checkout beside the repository; "" when there is none."""
+    env = os.environ.get("LITEGS_REFERENCE", "")
+    if env:
+        return env
+    repo = os.path.dirname(HERE)
+    for name in ("reference", "LiteGS"):
+        cand = os.path.join(os.path.dirname(repo), name)
+        if os.path.isdir(os.path.join(cand, "litegs", "submodules", "gaussian_raster")):
+            return cand
+    return ""
+
+
+REF_ROOT = _find_reference()
+REF_GR = os.path.join(REF_ROOT, "litegs", "submodules", "gaussian_raster") if REF_ROOT else ""
 NAME = "litegs_fused_ref"
 SOURCES = ["binning.cu", "compact.cu", "cuda_errchk.cpp", "ext_cuda.cpp", "raster.cu", "transform.cu"]
 
 
-REF_SSIM = "/root/reference/litegs/submodules/fused_ssim"
+REF_SSIM = os.path.join(REF_ROOT, "litegs", "submodules", "fused_ssim") if REF_ROOT else ""
+NOT_FOUND = ("[build_ref] no LiteGS checkout found (set LITEGS_REFERENCE, or place it at ../reference or ../LiteGS beside this "
+             "repository): nothing is built or staged from it; what oracle/_ref already holds is used, and the tests that need the "
+             "reference's own Python package skip without it")
 SSIM_NAME = "fused_ssim_cuda_ref"
 SSIM_SOURCES = ["ssim.cu", "ext.cpp"]
 
@@ -38,12 +59,12 @@ def build(quiet: bool = False):
     """Build oracle/_ref/litegs_fused_ref.so if the reference tree is present; returns the path or None."""
     if so_path() is not None:
         return so_path()
-    if not os.path.isdir(REF_GR):
+    if not REF_GR or not os.path.isdir(REF_GR):
         if not quiet:
-            print("[build_ref] /root/reference not present: nothing to build")
+            print(NOT_FOUND)
         return None
     os.makedirs(OUT, exist_ok=True)
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0a")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     os.environ["CXX"] = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else os.environ.get("CXX", "g++")
     os.environ["CC"] = "/usr/bin/gcc" if os.path.exists("/usr/bin/gcc") else os.environ.get("CC", "gcc")
     from torch.utils import cpp_extension
@@ -56,7 +77,7 @@ def build(quiet: bool = False):
         name=NAME,
         sources=[os.path.join(REF_GR, s) for s in SOURCES],
         extra_cflags=["-O3"],
-        extra_cuda_cflags=["-O3", "--use_fast_math", "-gencode", "arch=compute_100a,code=sm_100a"],
+        extra_cuda_cflags=["-O3", "--use_fast_math", "-gencode", "arch=compute_90a,code=sm_90a"],
         build_directory=OUT,
         verbose=not quiet,
         is_python_module=True,
@@ -69,13 +90,13 @@ def build_ssim(quiet: bool = False):
     nvcc flags (fused_ssim/setup.py:33: --maxrregcount=32 --use_fast_math) plus the arch; returns the path or None."""
     if so_path(SSIM_NAME) is not None:
         return so_path(SSIM_NAME)
-    if not os.path.isdir(REF_SSIM):
+    if not REF_SSIM or not os.path.isdir(REF_SSIM):
         if not quiet:
-            print("[build_ref] /root/reference not present: nothing to build")
+            print(NOT_FOUND)
         return None
     out = os.path.join(OUT, "ssim_build")
     os.makedirs(out, exist_ok=True)
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0a")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     os.environ["CXX"] = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else os.environ.get("CXX", "g++")
     os.environ["CC"] = "/usr/bin/gcc" if os.path.exists("/usr/bin/gcc") else os.environ.get("CC", "gcc")
     from torch.utils import cpp_extension
@@ -83,7 +104,7 @@ def build_ssim(quiet: bool = False):
         name=SSIM_NAME,
         sources=[os.path.join(REF_SSIM, s) for s in SSIM_SOURCES],
         extra_cflags=["-O3"],
-        extra_cuda_cflags=["-O3", "--maxrregcount=32", "--use_fast_math", "-gencode", "arch=compute_100a,code=sm_100a"],
+        extra_cuda_cflags=["-O3", "--maxrregcount=32", "--use_fast_math", "-gencode", "arch=compute_90a,code=sm_90a"],
         build_directory=out,
         verbose=not quiet,
         is_python_module=True,
@@ -95,23 +116,21 @@ def build_ssim(quiet: bool = False):
     return so_path(SSIM_NAME)
 
 
-REF_ROOT = "/root/reference"
-PY_OUT = os.path.join(os.path.dirname(HERE), "baseline", "_ref")
+PY_OUT = os.path.join(OUT, "py")
 
 
 def stage_python(quiet: bool = False):
     """Stage the UNMODIFIED reference Python package (``litegs/`` without its native submodules, plus the example scripts)
-    under ``baseline/_ref`` (the location the bench contract reserves for an unmodified reference install) -- git-ignored,
-    NOT gpurun-ignored -- so that the drop-in test
+    under ``oracle/_ref/py`` (git-ignored) so that the drop-in test
     (tests/test_gpu_dropin.py) and the ``ref_cuda`` bench leg can import the reference's own ``wrapper.py`` /
-    ``render/__init__.py`` / ``training/trainer.py`` on the GPU box, where /root/reference does not exist.  Files are byte
+    ``render/__init__.py`` / ``training/trainer.py`` on a machine the reference checkout is not copied to.  Files are byte
     copies (checked by the test against a manifest of SHA-256 digests written here); nothing is copied into tracked paths."""
     import hashlib
     import json
     import shutil
-    if not os.path.isdir(os.path.join(REF_ROOT, "litegs")):
+    if not REF_ROOT or not os.path.isdir(os.path.join(REF_ROOT, "litegs")):
         if not quiet:
-            print("[build_ref] /root/reference not present: nothing to stage")
+            print(NOT_FOUND)
         return PY_OUT if os.path.isdir(PY_OUT) else None
     os.makedirs(PY_OUT, exist_ok=True)
     manifest = {}
@@ -134,9 +153,9 @@ def stage_python(quiet: bool = False):
 
 
 def reference_python_path():
-    """Directory to put on sys.path to import the reference's ``litegs`` package: the mounted tree if present, else the
+    """Directory to put on sys.path to import the reference's ``litegs`` package: the checkout if present, else the
     staged copy, else None."""
-    if os.path.isdir(os.path.join(REF_ROOT, "litegs")):
+    if REF_ROOT and os.path.isdir(os.path.join(REF_ROOT, "litegs")):
         return REF_ROOT
     return PY_OUT if os.path.isdir(os.path.join(PY_OUT, "litegs")) else None
 
@@ -153,7 +172,7 @@ def _load(name: str):
 
 
 def load():
-    """Import the prebuilt reference module (needs torch; used on the GPU box). Returns None if absent."""
+    """Import the prebuilt reference module (needs torch). Returns None if absent."""
     return _load(NAME)
 
 

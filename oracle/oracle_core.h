@@ -5,13 +5,13 @@
  * and once with REAL=double (finite-difference / gradcheck tier).  It is NOT part of the
  * product: nothing under litegs_b200/ may include, link or call it.
  *
- * Every function cites the reference file:line (relative to /root/reference/litegs/submodules/
+ * Every function cites the reference file:line (relative to the reference's litegs/submodules/
  * gaussian_raster/, abbreviated GR/) whose arithmetic it restates.  Layouts are the reference's:
  * SoA with the point index innermost, row-vector matrices.
  *
  * PARITY PINNING: the reference ships no CPU path, no golden vectors and no test for this path
  * (SURVEY.md section 8c).  The restatement is pinned against the reference's own CUDA kernels run on
- * a B200 (oracle/build_ref.py -> oracle/_ref, fixtures under tests/golden/) -- see DESIGN.md.
+ * an H100 (oracle/build_ref.py -> oracle/_ref, fixtures under tests/golden/) -- see DESIGN.md.
  */
 
 #ifndef REAL

@@ -1,4 +1,4 @@
-"""Timing of the SURVEY 8(f) "next" rows on a B200, beside the unmodified reference kernels where they exist:
+"""Timing of the SURVEY 8(f) "next" rows beside the unmodified reference kernels where they exist:
 
   * fused L1+SSIM loss forward+backward at 1920x1080x3 (what trainer.py:145 runs per iteration): ours through the
     reference-shaped autograd surface, ours through l1_ssim_loss_and_grad (no loss map), the reference's fused_ssim_cuda
@@ -7,7 +7,7 @@
     reference's litegs_fused.adamUpdate).
 
 Prints one JSON object; CUDA events, 5 warm-up + 50 timed repetitions, inputs (25-236 MB) streamed from HBM each time.
-usage: python profiles/microbench/next_rows_bench.py > profiles/next_rows_r1.json"""
+usage: python profiles/microbench/next_rows_bench.py > next_rows.json"""
 import json
 import sys
 

@@ -1,6 +1,6 @@
 """One forward+backward view of the bench workload between cudaProfilerStart/Stop, for `ncu --profile-from-start off`:
 
-    ncu --set full --clock-control none --import-source on --profile-from-start off -o gpurun_out/prof_all_r2 python profiles/one_view.py [c2|c4]
+    ncu --set full --clock-control none --import-source on --profile-from-start off -o prof_all python profiles/one_view.py [c2|c4]
 
 Synchronising path, no CUDA graphs, one stream: every kernel of the view appears once, in order."""
 import os

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""Opcode histogram (SASS, sm_100a) of the hot kernels in liblitegs_b200.so -- static evidence next to the ncu captures:
-which pipes a kernel's instruction stream leans on, and that the Blackwell-specific forms are really in the binary
+"""Opcode histogram (SASS, sm_90a) of the hot kernels in liblitegs_b200.so -- static evidence next to ncu captures:
+which pipes a kernel's instruction stream leans on, and that the Hopper forms it relies on are really in the binary
 (LDGSTS = cp.async, UBLKCP = cp.async.bulk / TMA 1-D, REDG = fire-and-forget RED, REDUX, MUFU.EX2/RCP).
-usage: python profiles/sass_mix.py > profiles/sass_mix_r2.txt"""
+usage: python profiles/sass_mix.py > sass_mix.txt"""
 import collections
 import re
 import subprocess
@@ -48,7 +48,7 @@ def main():
         print(f"\n== {title}: {total} instructions")
         print("   " + "  ".join(f"{k} {v}" for k, v in ops.most_common(22)))
         # the forms that prove what the kernel is built on, wherever they rank
-        marks = ("FFMA2", "FMUL2", "FADD2", "LDGSTS", "UBLKCP", "SYNCS", "REDG", "RED", "REDUX", "ATOMS", "ATOMG", "MUFU.EX2", "MUFU.RCP",
+        marks = ("LDGSTS", "UBLKCP", "SYNCS", "REDG", "RED", "REDUX", "ATOMS", "ATOMG", "MUFU.EX2", "MUFU.RCP",
                  "MATCH", "SHFL", "VOTE", "LDGMC", "STGMC", "MULTIMEM")
         seen = [f"{k} {ops[k]}" for k in marks if ops.get(k)]
         if seen:

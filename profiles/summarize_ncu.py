@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Turns an `ncu --set full` report into the short text summary committed under profiles/.
-usage: python profiles/summarize_ncu.py gpurun_out/prof.ncu-rep > profiles/<name>.txt"""
+"""Turns an `ncu --set full` report into a short text summary.
+usage: python profiles/summarize_ncu.py prof.ncu-rep > <name>.txt"""
 import csv
 import io
 import subprocess

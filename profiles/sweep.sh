@@ -1,16 +1,17 @@
 #!/bin/bash
-# A/B sweeps on the C2 workload; prints views/s and per-stage ms/view.  Usage: gpurun -- 'bash profiles/sweep.sh [tiles|switches|streams]'
+# A/B sweeps on the C2 workload; prints views/s and per-stage ms/view.  Usage: bash profiles/sweep.sh [tiles|switches|streams]
+# (scratch output goes to $SWEEP_DIR, default a fresh temporary directory)
 # Switches (all default to the faster setting; each keeps the other implementation selectable for cross-checks):
 #   LGS_SORT=lgs|cub            own radix sort | cub::DeviceRadixSort          LGS_TILE_RANGE=search|scan   lower_bound per tile | streaming
 #   LGS_STAGING=cpasync|bulk    3 x cp.async | cp.async.bulk + mbarrier         LGS_BWD_REDUCE=smem|butterfly  backward warp reduction
 #   LGS_VIEWS_AUTOGRAD=0|1      render_views direct | through the autograd Function     LGS_WPB=4|2|1  tiles per CTA
-mkdir -p gpurun_out
+SWEEP_DIR=${SWEEP_DIR:-$(mktemp -d)}
 run() {  # label, env..., -- bench args
   local label="$1"; shift
-  env "$@" timeout 300 python bench.py --steps 20 --warmup 3 --no-e2e --no-cpu-baseline $EXTRA > gpurun_out/sw.json 2>gpurun_out/sw.err || { echo "FAIL $label"; tail -3 gpurun_out/sw.err; return; }
-  python - "$label" <<'PY'
+  env "$@" timeout 300 python bench.py --steps 20 --warmup 3 --no-e2e --no-cpu-baseline $EXTRA > "$SWEEP_DIR/sw.json" 2>"$SWEEP_DIR/sw.err" || { echo "FAIL $label"; tail -3 "$SWEEP_DIR/sw.err"; return; }
+  python - "$label" "$SWEEP_DIR/sw.json" <<'PY'
 import json,sys
-d=json.load(open('gpurun_out/sw.json')); s=d['stages']
+d=json.load(open(sys.argv[2])); s=d['stages']
 print(f"{sys.argv[1]:34s} views/s {d['value']:7.1f} ms/view {d['path_roofline']['ms_per_view']:.3f} D {d['workload_stats']['D']}  " +
       " ".join(f"{k[4:].replace('rasterize_','r').replace('_packed','').replace('sort_pairs_','sort')}={v['ms_per_view']:.3f}" for k,v in s.items()))
 PY

@@ -1,15 +1,15 @@
-"""Generates the golden fixtures that pin the CPU oracle to the REFERENCE ITSELF.
+"""Generates the golden fixtures that pin the CPU oracle and our kernels to the REFERENCE ITSELF.
 
-Runs the unmodified reference kernels (oracle/_ref/litegs_fused_ref*.so, built from /root/reference by
-oracle/build_ref.py with the reference's own flags, for sm_100a) on a B200 over a small seeded scene and stores
-every output of the hot path as float32/int32 arrays:
+Runs the unmodified reference kernels (oracle/_ref/litegs_fused_ref*.so, built by oracle/build_ref.py with the
+reference's own flags, for sm_90a) on an H100 over a small seeded scene and stores every output of the hot path that
+the tests compare as float32/int32 arrays:
 
-    /usr/local/graft/bin/gpurun -- 'python tests/golden/make_golden.py gpurun_out/golden'
-    cp gpurun_out/golden/*.npz tests/golden/        (then commit)
+    python tests/golden/make_golden.py OUTDIR        # then copy OUTDIR/*.npz into tests/golden/
 
 Inputs are NOT stored: tests regenerate them from the seed with litegs_b200.scene (numpy PCG64 streams are
-stable), plus the seeded upstream gradients below.  tests/test_golden.py compares the oracle (CPU, no GPU
-needed) against these fixtures; tests/test_gpu_vs_reference.py does the live comparison on the GPU box.
+stable), plus the seeded upstream gradients below.  Arrays of more than SAMPLE_ABOVE elements are stored as the values at
+seeded flat positions (``<name>`` + ``<name>__index``), which keeps every fixture under 1 MB.  tests/test_golden.py
+compares the oracle (CPU) against these fixtures, tests/test_gpu_vs_reference.py our kernels (GPU).
 """
 import os
 import sys
@@ -25,6 +25,16 @@ CASES = {
     "c_small_8x16": (2000, (96, 128), (8, 16), 2, 1, 3),
 }
 PARAM_KEYS = ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")
+SAMPLE_ABOVE = 65536
+NOT_STORED = ("left_up", "right_down", "final_T")          # outputs no test compares
+
+
+def matched(ref, got, k):
+    """(stored reference values, ours at the same positions) for output k."""
+    got = np.asarray(got[k])
+    if f"{k}__index" in ref:
+        return ref[k], got.reshape(-1)[ref[f"{k}__index"]]
+    return ref[k], got
 
 
 def case_inputs(name):
@@ -112,17 +122,28 @@ def run_backend(mod, name, torch, dev):
 def main():
     import torch
     from oracle import build_ref
-    outdir = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "gpurun_out", "golden")
+    outdir = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "tests", "golden")
     os.makedirs(outdir, exist_ok=True)
     ref = build_ref.load()
     if ref is None:
-        sys.exit("oracle/_ref is not built: run `python -m oracle.build_ref` where /root/reference is mounted")
+        sys.exit("oracle/_ref is not built: see oracle/build_ref.py")
     dev = torch.device("cuda:0")
     for name in CASES:
         out = run_backend(ref, name, torch, dev)
         torch.cuda.synchronize()
-        np.savez_compressed(os.path.join(outdir, f"{name}.npz"), **out)
-        print(name, {k: v.shape for k, v in list(out.items())[:4]}, "...", len(out), "arrays")
+        store = {}
+        rng = np.random.default_rng(11)
+        for k, v in out.items():
+            if k in NOT_STORED:
+                continue
+            if v.size > SAMPLE_ABOVE:
+                idx = np.sort(rng.choice(v.size, SAMPLE_ABOVE // 2, replace=False))
+                store[k], store[f"{k}__index"] = v.reshape(-1)[idx], idx
+            else:
+                store[k] = v
+        path = os.path.join(outdir, f"{name}.npz")
+        np.savez_compressed(path, **store)
+        print("wrote", path, os.path.getsize(path), "bytes")
 
 
 if __name__ == "__main__":

@@ -1,5 +1,5 @@
 """The bench contract on the CPU arm: `bench.py --impl reference` prints exactly ONE stdout line, valid JSON, with the
-keys the driver reads (metric, value, unit, n_gpus, steps, warmup, ms_per_step, higher_is_better, scaling, vs_baseline,
+keys a consumer of the line reads (metric, value, unit, n_gpus, steps, warmup, ms_per_step, higher_is_better, scaling, vs_baseline,
 dtype, data, config.workload, impl, cpu_baseline, e2e).  Runs the oracle on a scene small enough for a few seconds."""
 import json
 import os

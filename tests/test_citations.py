@@ -1,13 +1,12 @@
 """Every reference citation of the form `<file>:<line>[-<line>]` in the C ABI header, the kernels, the host mirror, the
-oracle and the design documents must resolve against the mounted reference tree: the file exists and has at least that many lines.  Skipped
-where /root/reference is absent (the GPU box)."""
+oracle and the design documents must resolve against the reference tree: the file exists and has at least that many lines
+(tests/golden/reference_line_counts.json, written by tests/golden/make_golden_reference_cpu.py)."""
+import json
 import os
 import re
 
-import pytest
-
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+COUNTS = os.path.join(ROOT, "tests", "golden", "reference_line_counts.json")
 PREFIXES = {"GR/": "litegs/submodules/gaussian_raster/", "fused_ssim/": "litegs/submodules/fused_ssim/", "litegs/": "litegs/"}
 BARE = {"wrapper.py": "litegs/utils/wrapper.py", "optimizer.py": "litegs/training/optimizer.py", "trainer.py": "litegs/training/trainer.py",
         "data.py": "litegs/data.py", "densify.py": "litegs/training/densify.py", "statistic_helper.py": "litegs/utils/statistic_helper.py",
@@ -36,22 +35,18 @@ def _resolve(name):
     return [BARE[name]]
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="/root/reference not mounted")
 def test_reference_citations_resolve():
-    lines_of = {}
+    lines_of = json.load(open(COUNTS))
     bad, n = [], 0
     for src in _sources():
         text = open(src, errors="replace").read()
         for m in CITE.finditer(text):
             name, a, b = m.group(1), int(m.group(2)), int(m.group(3) or m.group(2))
-            paths = [os.path.join(REF, c) for c in _resolve(name)]
-            path = next((p for p in paths if os.path.exists(p)), None)
+            path = next((c for c in _resolve(name) if c in lines_of), None)
             n += 1
             if path is None:
                 bad.append((os.path.relpath(src, ROOT), m.group(0), "no such file"))
                 continue
-            if path not in lines_of:
-                lines_of[path] = sum(1 for _ in open(path, errors="replace"))
             if not (1 <= a <= b <= lines_of[path]):
                 bad.append((os.path.relpath(src, ROOT), m.group(0), f"file has {lines_of[path]} lines"))
     assert n > 150, n

@@ -1,8 +1,8 @@
 """Multi-GPU numeric check of the data path's only collective (VERDICT "What's weak" 5): on a box with >= 2 GPUs, the NCCL
 all-reduced gradient buffer of a sharded view batch equals the single-rank sum of the same views (tests/dist_nccl_check.py,
 one process per GPU under torch.distributed.run).  Skipped on a single-GPU box; the host-side logic has its own world-size-2
-gloo test on CPU (tests/test_dist_gloo.py).  `gpurun --gpus 2 -- python -m pytest tests/test_gpu_dist.py -m gpu -s` runs it;
-the output of such a run is kept under profiles/nccl_check_r2.txt."""
+gloo test on CPU (tests/test_dist_gloo.py).  `python -m pytest tests/test_gpu_dist.py -m gpu -s` on a
+multi-GPU machine runs it."""
 import json
 import os
 import subprocess

@@ -1,6 +1,6 @@
 """The drop-in, exercised (VERDICT "What's weak" 2): the reference's OWN, UNMODIFIED Python -- ``litegs/utils/wrapper.py``,
 ``litegs/render/__init__.py``, ``litegs/utils/statistic_helper.py``, ``litegs/training/trainer.py`` -- imported from the staged
-byte copy under ``baseline/_ref`` (``oracle/build_ref.py:stage_python``; /root/reference itself does not exist on the GPU box)
+LiteGS checkout or its byte copy that ``__graft_entry__.build()`` stages under ``oracle/_ref/py`` (``oracle/build_ref.py:stage_python``)
 and run on top of THIS repository's ``litegs_fused`` / ``fused_ssim`` modules and the dependency stand-ins of
 ``litegs_b200/shims``:
 
@@ -34,7 +34,7 @@ def litegs_ref(cuda):
     from oracle import build_ref
     path = build_ref.reference_python_path()
     if path is None:
-        pytest.skip("reference Python package not staged (run __graft_entry__.build() where /root/reference is mounted)")
+        pytest.skip("reference Python package not available: no LiteGS checkout was found when oracle/_ref was built (oracle/build_ref.py)")
     man = os.path.join(path, "MANIFEST.json")
     if os.path.exists(man):                       # staged copy: every file is byte-identical to what was staged
         for rel, digest in json.load(open(man)).items():

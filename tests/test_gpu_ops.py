@@ -1,4 +1,4 @@
-"""GPU parity tests (B200): every op of the C ABI, through the litegs_fused-shaped host mirror, against
+"""GPU parity tests (H100): every op of the C ABI, through the litegs_fused-shaped host mirror, against
 the CPU oracle on identical seeded inputs.  Integer/index outputs must be bit-exact; fp32 outputs within
 1e-4 relative (BASELINE.json north_star); pixels the oracle flags as sitting on a step-function
 threshold (SURVEY Appendix B) are masked and counted."""
