@@ -141,7 +141,9 @@ int lgs_tile_range_u16(const unsigned short* table_tile_id, int V, int table_len
 /* building blocks of the fused pipeline, on the caller's stream and workspace.  Stable LSD radix sort of (key, value)
  * pairs on the bits [begin_bit, end_bit): replaces torch.sort (wrapper.py:739) for the depth order and
  * cub::DeviceRadixSort::SortPairs (GR/binning.cu:204-221) for the tile sort.  keys_in/vals_in are not modified.
- * lgs_set_sort_impl: 1 = own histogram/scan/scatter passes (default), 0 = cub::DeviceRadixSort; env LGS_SORT=lgs|cub. */
+ * lgs_set_sort_impl: 1 = own histogram/scan/scatter passes (default), 0 = cub::DeviceRadixSort; env LGS_SORT=lgs|cub.
+ * Either value forces that sort for every later call; -1 returns to the unforced state of a fresh process (LGS_SORT is
+ * read again, and without it the tile sort of more than 14 key bits on more than 8 << 20 pairs takes cub's onesweep). */
 int lgs_set_sort_impl(int impl);
 /* form of the own radix sort: 0 = histogram / row-scan / scatter passes (default), 1 = onesweep (global
  * histograms in one read + decoupled look-back per pass); env LGS_RS=passes|onesweep */

@@ -576,12 +576,13 @@ int sort_pairs(const char* who, const KeyT* keys_in, KeyT* keys_out, const unsig
 
 }  // namespace
 
-// 0 = cub::DeviceRadixSort, 1 = the histogram/scan/scatter passes above (default; env LGS_SORT=cub|lgs)
+// 0 = cub::DeviceRadixSort, 1 = the histogram/scan/scatter passes above (default; env LGS_SORT=cub|lgs); both force the choice.
+// -1 = unforced again: LGS_SORT is read on the next sort and, without it, sort_impl_for chooses per call.
 extern "C" int lgs_set_sort_impl(int impl)
 {
-    LGS_REQUIRE(impl == 0 || impl == 1, "set_sort_impl: %d is not 0 (cub) or 1 (lgs)", impl);
+    LGS_REQUIRE(impl == -1 || impl == 0 || impl == 1, "set_sort_impl: %d is not -1 (unforced), 0 (cub) or 1 (lgs)", impl);
     g_sort_impl = impl;
-    g_sort_forced = true;
+    g_sort_forced = impl >= 0;
     return LGS_OK;
 }
 

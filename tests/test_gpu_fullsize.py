@@ -12,6 +12,7 @@ import torch
 
 from litegs_b200 import fused, pipeline, render, scene
 from litegs_b200.arguments import PipelineParams
+from tests.util import differing_tiles
 
 pytestmark = pytest.mark.gpu
 KEYS = ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")
@@ -103,29 +104,6 @@ def test_c2_level_a_equals_level_b(cuda):
         assert float((a - b).abs().max()) / (float(a.abs().max()) + 1e-30) < 2e-4, k
 
 
-def _differing_tiles(ranges_a, pid_a, ranges_b, pid_b):
-    """Tiles (0-based) whose depth-ordered splat lists differ between two binnings, and the number of differing pairs."""
-    ntile = ranges_a.shape[1] - 2
-
-    def segs(r, n):
-        r = r[0].astype(np.int64)
-        start = r[1:ntile + 1].copy()
-        nxt = np.full(ntile + 1, n, np.int64)                 # end of tile t = next populated start after t
-        s2 = np.where(r[1:ntile + 2] >= 0, r[1:ntile + 2], np.iinfo(np.int64).max)
-        nxt = np.minimum.accumulate(s2[::-1])[::-1]
-        end = np.where(start >= 0, np.minimum(nxt[1:], n), -1)
-        return start, end
-    sa, ea = segs(ranges_a, pid_a.shape[1]); sb, eb = segs(ranges_b, pid_b.shape[1])
-    bad, npairs = [], 0
-    for t in range(ntile):
-        la = pid_a[0, sa[t]:ea[t]] if sa[t] >= 0 else pid_a[0, :0]
-        lb = pid_b[0, sb[t]:eb[t]] if sb[t] >= 0 else pid_b[0, :0]
-        if la.shape != lb.shape or not np.array_equal(la, lb):
-            bad.append(t)
-            npairs += len(set(la.tolist()) ^ set(lb.tolist()))
-    return np.array(bad, np.int64), npairs
-
-
 def test_c2_one_view_matches_oracle(cuda):
     """BASELINE.json configs[1] (the configuration the headline number is quoted on): ONE full-size view -- 1M Gaussians,
     1920x1080, sh_degree 3, 8x16 tiles -- fused pipeline vs the CPU oracle: per-tile lists (identical except for a handful of
@@ -151,7 +129,7 @@ def test_c2_one_view_matches_oracle(cuda):
         _, st, _ = pipeline.render_view_forward({k: P[k].detach() for k in KEYS}, A[0], A[1], C["frustumplane"], C["view"], C["proj"], deg,
                                                 (H, W), tile)
     D = o0["sorted_pid"].shape[1]
-    bad, npairs = _differing_tiles(st.ranges.cpu().numpy(), st.sorted_pid.cpu().numpy(), o0["ranges"], o0["sorted_pid"])
+    bad, npairs = differing_tiles(st.ranges.cpu().numpy(), st.sorted_pid.cpu().numpy(), o0["ranges"], o0["sorted_pid"])
     print(f"C2 view: D = {D} pairs (ours {st.n_pairs}), {len(bad)} tiles / {npairs} pairs differ from the oracle's lists, "
           f"{frag.mean() * 100:.2f} % fragile pixels")
     assert abs(st.n_pairs - D) <= 1e-5 * D and npairs <= 1e-5 * D, (st.n_pairs, D, npairs)
@@ -197,7 +175,7 @@ def test_c4_crop_tile_lists_match_oracle(cuda):
     C = {k: torch.from_numpy(v).to(cuda) for k, v in cam.items()}
     _, st, _ = pipeline.render_view_forward(P, A[0], A[1], C["frustumplane"], C["view"], C["proj"], 3, (H, W), tile)
     D = pid.shape[1]
-    bad, npairs = _differing_tiles(st.ranges.cpu().numpy(), st.sorted_pid.cpu().numpy(), ranges, pid)
+    bad, npairs = differing_tiles(st.ranges.cpu().numpy(), st.sorted_pid.cpu().numpy(), ranges, pid)
     print(f"C4 crop: D = {D} pairs (ours {st.n_pairs}), {len(bad)} tiles / {npairs} pairs differ")
     assert abs(st.n_pairs - D) <= 1e-5 * D + 1 and npairs <= 1e-5 * D + 1, (st.n_pairs, D, npairs)
 

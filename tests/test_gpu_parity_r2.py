@@ -319,17 +319,17 @@ def test_raster_specific_tiles(cuda, proj, bwd):
 
 def test_tile_order_is_a_descending_permutation(cuda):
     rng = np.random.default_rng(0)
-    ntile = 16200
-    work = np.minimum(rng.exponential(300, size=(2, ntile)), 9000).astype(np.int32)
-    work[:, ::7] = 0
-    order = torch.empty((2, ntile), dtype=torch.int32, device=cuda)
-    w = T(work, cuda)
-    _lib.call("lgs_tile_order", w.data_ptr(), 2, ntile, order.data_ptr(), torch.cuda.current_stream().cuda_stream)
-    od = order.cpu().numpy()
-    for b in range(2):
-        assert np.array_equal(np.sort(od[b]), np.arange(1, ntile + 1))            # a permutation of the 1-based tile ids
-        wb = np.minimum(work[b][od[b] - 1] >> 2, 1023)
-        assert (np.diff(wb) <= 0).all()                                           # non-increasing in the bucketed work
+    for ntile in (16200, 64800, 129600):                     # 1080p at 8x16 tiles, 4K at 8x16 and at 8x8
+        work = np.minimum(rng.exponential(300, size=(2, ntile)), 9000).astype(np.int32)
+        work[:, ::7] = 0
+        order = torch.empty((2, ntile), dtype=torch.int32, device=cuda)
+        w = T(work, cuda)
+        _lib.call("lgs_tile_order", w.data_ptr(), 2, ntile, order.data_ptr(), torch.cuda.current_stream().cuda_stream)
+        od = order.cpu().numpy()
+        for b in range(2):
+            assert np.array_equal(np.sort(od[b]), np.arange(1, ntile + 1)), ntile    # a permutation of the 1-based tile ids
+            wb = np.minimum(work[b][od[b] - 1] >> 2, 1023)
+            assert (np.diff(wb) <= 0).all(), ntile                                # non-increasing in the bucketed work
 
 
 def test_fused_pipeline_tile_order_changes_nothing(cuda):
