@@ -2,6 +2,7 @@
 
     python examples/train_colmap.py --make /tmp/synth_colmap          # writes a synthetic dataset first (renders of a hidden scene)
     python examples/train_colmap.py --data /path/to/colmap --iters 2000
+    python examples/train_colmap.py --make /tmp/noisy --pose-noise 1 0.02 --refine-poses     # learn the camera poses too
 
 Reads ``sparse/0/{cameras,images,points3D}.bin`` and ``images/*`` (litegs_b200.colmap; same files and conventions as the
 reference's ``litegs/io_manager/colmap.py`` + ``litegs/data.py``), initialises Gaussians from the SfM points the way
@@ -22,9 +23,13 @@ from litegs_b200.arguments import PipelineParams  # noqa: E402
 from litegs_b200.dist import PARAM_ORDER  # noqa: E402
 
 
-def make_dataset(root, n_gaussians=60_000, n_views=24, hw=(270, 480), n_points=20_000, seed=0, dev=None, log_scale_range=(0.01, 0.04)):
+def make_dataset(root, n_gaussians=60_000, n_views=24, hw=(270, 480), n_points=20_000, seed=0, dev=None, log_scale_range=(0.01, 0.04),
+                 pose_noise=None):
     """A hidden scene rendered from the lattice cameras -> COLMAP model + PNGs.  The 'SfM points' are a subsample of the
-    hidden Gaussians' centres with their band-0 colours (what a real reconstruction would roughly deliver)."""
+    hidden Gaussians' centres with their band-0 colours (what a real reconstruction would roughly deliver).
+
+    pose_noise = (degrees, fraction): the poses written to the model are off by a rotation of that many degrees about a random
+    axis and a translation of that fraction of the camera's distance, as noisy SfM poses are; the images stay exact."""
     dev = dev or torch.device("cuda:0")
     H, W = hw
     pp = PipelineParams(tile_size=(8, 16), sparse_grad=True)
@@ -44,6 +49,21 @@ def make_dataset(root, n_gaussians=60_000, n_views=24, hw=(270, 480), n_points=2
     sel = rng.choice(xyz.shape[0], size=min(n_points, xyz.shape[0]), replace=False)
     rgb = np.clip((truth["sh_0"].reshape(3, -1).T[sel] * colmap.SH_C0 + 0.5) * 255.0, 0, 255).astype(np.uint8)
     colmap.write_synthetic_dataset(root, xyz[sel].astype(np.float64), rgb, n_views, W, H, render_fn=render_fn)
+    if pose_noise is not None:
+        deg, frac = pose_noise
+        cams, images, pts = colmap.read_model(root)
+        for k, im in images.items():
+            axis = rng.normal(size=3)
+            axis /= np.linalg.norm(axis)
+            a = np.radians(deg)
+            c, s_ = np.cos(a), np.sin(a)
+            K = np.array([[0, -axis[2], axis[1]], [axis[2], 0, -axis[0]], [-axis[1], axis[0], 0]])
+            dR = np.eye(3) + s_ * K + (1 - c) * K @ K
+            d = rng.normal(size=3)
+            t = np.asarray(im.tvec, np.float64)
+            t = t + frac * np.linalg.norm(t) * d / np.linalg.norm(d)
+            images[k] = im._replace(qvec=colmap.rotmat_to_qvec(dR @ colmap.qvec_to_rotmat(im.qvec)), tvec=t)
+        colmap.write_model(root, cams, images, pts)
     return root
 
 
@@ -64,21 +84,58 @@ def load_dataset(root, image_dir="images", dev=None):
     return frames, np.stack([p.xyz for p in P]), np.stack([p.rgb for p in P])
 
 
-def train(root, iters=300, views_per_step=8, log=print):
+def train(root, iters=300, views_per_step=8, log=print, refine_poses=False):
     from litegs_b200 import fused
+    if refine_poses and int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        raise ValueError("--refine-poses runs on one GPU: multi-GPU pose refinement is not supported")
     keep = fused.CONFIG["true_sigmoid_grad"]
     fused.CONFIG["true_sigmoid_grad"] = True               # our own loops train with the true sigmoid derivative (SURVEY Q15)
     try:
-        return _train(root, iters, views_per_step, log)
+        return _train(root, iters, views_per_step, log, refine_poses)
     finally:
         fused.CONFIG["true_sigmoid_grad"] = keep
 
 
-def _train(root, iters, views_per_step, log):
+class _Poses:
+    """Learnable extrinsics f32[n_frames,7] (qw qx qy qz tx ty tz, initialised from the COLMAP poses) with their own Adam.  Each
+    view's camera comes from create_viewproj_forward; render_views' camera gradients are mapped back through
+    create_viewproj_backward.  The field of view stays fixed, as in the reference (trainer.py:161-162)."""
+    Z_NEAR, Z_FAR = 0.01, 5000.0
+
+    def __init__(self, frames, hw, dev, lr=1e-4):
+        self.hw = hw
+        H, W = hw
+        ext, recp = [], None
+        for cam, _, _ in frames:
+            q, t, intr = colmap.camera_to_colmap({k: v.cpu().numpy() for k, v in cam.items()}, W, H)
+            ext.append(np.concatenate([q, t]))
+            recp = intr[0] / (W * 0.5)
+        self.extr = torch.tensor(np.stack(ext), dtype=torch.float32, device=dev).requires_grad_(True)
+        self.recp = torch.tensor([recp], dtype=torch.float32, device=dev)
+        self.opt = torch.optim.Adam([self.extr], lr=lr)
+
+    def cameras(self, idx):
+        from litegs_b200 import fused
+        v, p, _, planes = fused.create_viewproj_forward(self.extr.detach()[idx], self.recp, *self.hw, self.Z_NEAR, self.Z_FAR)
+        return [dict(view=v[i:i + 1], proj=p[i:i + 1], frustumplane=planes[i:i + 1]) for i in range(len(idx))]
+
+    def step(self, idx, camera_grads):
+        from litegs_b200 import fused
+        ix = torch.tensor(idx, dtype=torch.int64, device=self.extr.device)
+        g, _ = fused.create_viewproj_backward(camera_grads[:, 0], camera_grads[:, 1], torch.zeros_like(camera_grads[:, 0]),
+                                              self.extr.detach()[ix], self.recp, *self.hw, self.Z_NEAR, self.Z_FAR)
+        self.extr.grad = torch.zeros_like(self.extr).index_add_(0, ix, g)
+        self.opt.step()
+
+
+def _train(root, iters, views_per_step, log, refine_poses=False):
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", 0)))
     torch.cuda.set_device(dev)
     frames, xyz, rgb = load_dataset(root, dev=dev)
     H, W = frames[0][2]
+    poses = _Poses(frames, (H, W), dev) if refine_poses else None
+    extr0 = poses.extr.detach().clone() if poses else None
+    cgrads = torch.empty((views_per_step, 2, 4, 4), dtype=torch.float32, device=dev) if poses else None
     g = colmap.gaussians_from_points(xyz, rgb, sh_degree=3)
     P = {k: torch.from_numpy(g[k]).to(dev) for k in PARAM_ORDER}
     pp = PipelineParams(tile_size=(8, 16), sparse_grad=True)
@@ -92,11 +149,15 @@ def _train(root, iters, views_per_step, log):
         # positions and shapes move, so the chunk AABBs used for culling are refreshed from the parameters now and then
         if it % 50 == 0:
             A = list(scene.cluster_aabb_torch(P["xyz"], P["scale"], P["rot"]))
-        losses = render.render_views(views_per_step, lambda i: frames[idx[i]][0], None, A[0], A[1], P["xyz"], P["scale"], P["rot"],
+        cams = poses.cameras(idx) if poses else [frames[j][0] for j in idx]
+        losses = render.render_views(views_per_step, lambda i: cams[i], None, A[0], A[1], P["xyz"], P["scale"], P["rot"],
                                      P["sh_0"], P["sh_rest"], P["opacity"], 3, (H, W), pp, acc.grads(),
                                      loss_and_grad_fn=lambda i, img: ssim.l1_ssim_loss_and_grad(img.contiguous(), frames[idx[i]][1], 0.2,
-                                                                                              upstream=1.0 / views_per_step))
+                                                                                              upstream=1.0 / views_per_step),
+                                     camera_grads=cgrads)
         opt.step(acc)
+        if poses:
+            poses.step(idx, cgrads)
         sched.step()
         hist.append(float(torch.stack(losses).mean()))
         if it % 50 == 0 or it == iters - 1:
@@ -105,13 +166,17 @@ def _train(root, iters, views_per_step, log):
     dt = time.perf_counter() - t0
     with torch.no_grad():
         mse = []
-        for cam, gt, _ in frames[:8]:
+        for j, (cam, gt, _) in enumerate(frames[:8]):
+            cam = poses.cameras([j])[0] if poses else cam
             img = render.render_view(A[0], A[1], cam["frustumplane"], cam["view"], cam["proj"], P["xyz"], P["scale"], P["rot"], P["sh_0"],
                                      P["sh_rest"], P["opacity"], 3, (H, W), pp)[0]
             mse.append(float(((img - gt) ** 2).mean()))
     psnr = -10.0 * np.log10(np.mean(mse))
     log(f"{iters} iterations x {views_per_step} views in {dt:.1f} s ({iters * views_per_step / dt:.0f} views/s incl. loss + optimizer); "
         f"{xyz.shape[0]} Gaussians, PSNR over 8 training views {psnr:.2f} dB")
+    if poses:
+        moved = (poses.extr.detach() - extr0).abs()
+        log(f"poses refined: mean |change| of the quaternions {float(moved[:, :4].mean()):.2e}, of the translations {float(moved[:, 4:].mean()):.2e}")
     return hist, psnr
 
 
@@ -120,11 +185,14 @@ if __name__ == "__main__":
     ap.add_argument("--make", default=None, help="write a synthetic COLMAP dataset to this directory first and train on it")
     ap.add_argument("--data", default=None)
     ap.add_argument("--iters", type=int, default=300)
+    ap.add_argument("--refine-poses", action="store_true", help="also optimise the camera extrinsics (one GPU)")
+    ap.add_argument("--pose-noise", type=float, nargs=2, default=None, metavar=("DEG", "FRAC"),
+                    help="with --make: perturb the written poses by DEG degrees and FRAC of the camera distance")
     a = ap.parse_args()
     root = a.data
     if a.make:
-        root = make_dataset(a.make)
+        root = make_dataset(a.make, pose_noise=a.pose_noise)
     if root is None:
         ap.error("give --data or --make")
-    h, _ = train(root, a.iters)
+    h, _ = train(root, a.iters, refine_poses=a.refine_poses)
     assert h[-1] < h[0]

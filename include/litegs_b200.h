@@ -274,13 +274,30 @@ int lgs_emit_pairs_u16(const float* packed_params, const int* offset, const unsi
  * createTransformMatrix_backward + mvp_transform_backward + activate_backward (wrapper.py:481-524,588-592,404-407,
  * 190-193,278-285,820-845).  zero_outputs: 0 = assign compacted [..,A,S] outputs, 1 = clear them first,
  * 2 = ACCUMULATE into dense [..,C,S] gradient tensors at the source chunk (multi-view / data-parallel path).
- * touched (f32[C], may be NULL) receives 1 at every visible chunk: the marks lgs_adam_step_dense consumes. */
+ * touched (f32[C], may be NULL) receives 1 at every visible chunk: the marks lgs_adam_step_dense consumes.
+ * cam_partials (f32[A,32]) and d_cam (f32[32]), both NULL or both given: d_cam receives the gradient of the view matrix
+ * (d_cam[0..15], row-vector [k*4+j]) and of the projection matrix (d_cam[16..31]) through the NDC mean and the V3x3 factor of
+ * the 2D covariance, with J and the SH direction held constant (the convention of the position gradient, DESIGN.md section 1).
+ * The reference's operators return no view-matrix gradient (wrapper.py:285,407,845); this one is new.  Summed in a fixed
+ * order (bit-reproducible), no host synchronisation; needs S % 32 == 0. */
 int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
                          const float* view_matrix, const float* proj_matrix, const float* position, const float* scale,
                          const float* rotation, const float* opacity, int C, int S, int A, int rest_dim, int img_h,
                          int img_w, int true_sigmoid_grad, const float* packed_grad, const float* grad_inv_scaler,
                          int zero_outputs, float* g_position, float* g_scale, float* g_rotation, float* g_sh_base,
-                         float* g_sh_rest, float* g_opacity, float* touched, void* stream);
+                         float* g_sh_rest, float* g_opacity, float* touched, float* cam_partials, float* d_cam, void* stream);
+
+/* create_viewproj_forward, GR/compact.cu:17-141: view_params f32[V,7] (qw qx qy qz tx ty tz), recp_tan_half_fov_x f32[1] ->
+ * view, proj, viewproj f32[V,4,4] (row-vector convention) and frustumplane f32[V,6,4].  One thread per view. */
+int lgs_create_viewproj_forward(const float* view_params, const float* recp_tan_half_fov_x, int V, int img_h, int img_w,
+                                float z_near, float z_far, float* view_matrix, float* proj_matrix, float* viewproj_matrix,
+                                float* frustumplane, void* stream);
+/* create_viewproj_backward, GR/compact.cu:143-316, with the reference's arithmetic (DESIGN.md section 7): the fov gradient scales
+ * d proj[1][1] by the integer quotient img_w / img_h, and the quaternion gradient is the true one times |q|.  grad_recp f32[1] is
+ * the sum over views in a fixed order (the reference's is a race for V > 1).  Outputs are assigned, not accumulated. */
+int lgs_create_viewproj_backward(const float* view_matrix_grad, const float* proj_matrix_grad, const float* viewproj_matrix_grad,
+                                 const float* view_params, const float* recp_tan_half_fov_x, int V, int img_h, int img_w,
+                                 float z_near, float z_far, float* grad_view_params, float* grad_recp_tan_half_fov_x, void* stream);
 
 /* ---- optimiser / statistics (next rows, SURVEY 8f) ------------------------------------------------------ */
 

@@ -509,6 +509,51 @@ def gpu_driven_pipeline_sparse_op(A, B, visible_chunk_ids, visible_count, op_nam
 
 
 # ---------------------------------------------------------------------------------------------------
+# learnable cameras
+# ---------------------------------------------------------------------------------------------------
+
+def create_viewproj_forward(view_params, recp_tan_half_fov_x, img_h, img_w, z_near, z_far):
+    """GR/compact.cu:123-141: view_params f32[V,7] (qw qx qy qz tx ty tz), recp_tan_half_fov_x f32[1] ->
+    [view f32[V,4,4], proj f32[V,4,4], viewproj f32[V,4,4], frustumplane f32[V,6,4]] (row-vector convention)."""
+    vp = _f32c(view_params, "view_params"); rf = _f32c(recp_tan_half_fov_x.reshape(-1), "recp_tan_half_fov_x")
+    if vp.dim() != 2 or vp.shape[1] != 7:
+        raise RuntimeError(f"view_params must be [V,7], got {tuple(vp.shape)}")
+    V = vp.shape[0]
+    dev = vp.device
+    with torch.cuda.device(dev):
+        view = torch.empty((V, 4, 4), dtype=_F32, device=dev)
+        proj = torch.empty((V, 4, 4), dtype=_F32, device=dev)
+        viewproj = torch.empty((V, 4, 4), dtype=_F32, device=dev)
+        planes = torch.empty((V, 6, 4), dtype=_F32, device=dev)
+        _lib.call("lgs_create_viewproj_forward", _ptr(vp), _ptr(rf), V, int(img_h), int(img_w), float(z_near), float(z_far),
+                  _ptr(view), _ptr(proj), _ptr(viewproj), _ptr(planes), _stream(dev))
+    return [view, proj, viewproj, planes]
+
+
+def create_viewproj_backward(view_matrix_grad, proj_matrix_grad, viewproj_matrix_grad, view_params, recp_tan_half_fov_x,
+                             img_h, img_w, z_near, z_far):
+    """GR/compact.cu:289-316 -> [grad_view_params f32[V,7], grad_recp_tan_half_fov_x f32[1]].
+
+    The reference's arithmetic, quirks included (DESIGN.md section 7): the quaternion gradient is the true one times |q|, and the
+    fov gradient scales d proj[1][1] by the integer quotient img_w // img_h.  The fov gradient is summed over the views in a
+    fixed order (the reference's is a race for more than one view)."""
+    vp = _f32c(view_params, "view_params"); rf = _f32c(recp_tan_half_fov_x.reshape(-1), "recp_tan_half_fov_x")
+    V = vp.shape[0]
+    gv = _f32c(view_matrix_grad, "view_matrix_grad"); gp = _f32c(proj_matrix_grad, "proj_matrix_grad")
+    gvp = _f32c(viewproj_matrix_grad, "viewproj_matrix_grad")
+    for name, g in (("view_matrix_grad", gv), ("proj_matrix_grad", gp), ("viewproj_matrix_grad", gvp)):
+        if g.numel() != V * 16:
+            raise RuntimeError(f"{name} must be [V,4,4] with V = {V}, got {tuple(g.shape)}")
+    dev = vp.device
+    with torch.cuda.device(dev):
+        g_params = torch.empty((V, 7), dtype=_F32, device=dev)
+        g_recp = torch.zeros_like(rf)         # only [0] is a parameter of the camera (GR/compact.cu:54); the rest stays zero
+        _lib.call("lgs_create_viewproj_backward", _ptr(gv), _ptr(gp), _ptr(gvp), _ptr(vp), _ptr(rf), V, int(img_h), int(img_w),
+                  float(z_near), float(z_far), _ptr(g_params), _ptr(g_recp), _stream(dev))
+    return [g_params, g_recp.reshape(recp_tan_half_fov_x.shape)]
+
+
+# ---------------------------------------------------------------------------------------------------
 # entry points outside the hot path (SURVEY 8b: optional / dead in the reference)
 # ---------------------------------------------------------------------------------------------------
 
@@ -519,8 +564,6 @@ def _out_of_scope(name, why):
     return fn
 
 
-create_viewproj_forward = _out_of_scope("create_viewproj_forward", "learnable_viewproj is off by default (arguments.py:91)")
-create_viewproj_backward = _out_of_scope("create_viewproj_backward", "learnable_viewproj is off by default (arguments.py:91)")
 world2ndc_forward = _out_of_scope("world2ndc_forward", "only reachable through the unused World2NdcFunc (wrapper.py:287)")
 world2ndc_backword = _out_of_scope("world2ndc_backword", "only reachable through the unused World2NdcFunc (wrapper.py:287)")
 

@@ -189,14 +189,18 @@ def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_exte
 
 def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_trans: Optional[torch.Tensor] = None,
                          enable_statistic: bool = False, specific_tiles: Optional[torch.Tensor] = None,
-                         accumulate_into: Optional[dict] = None, clamped_img: Optional[torch.Tensor] = None):
+                         accumulate_into: Optional[dict] = None, clamped_img: Optional[torch.Tensor] = None,
+                         camera_grad: Optional[torch.Tensor] = None):
     """Backward of one view: d_img f32[1,3,Hp,Wp] (padded) -> compacted parameter gradients
     (xyz[3,A,S], scale[3,A,S], rot[4,A,S], sh_0[1,3,A,S], sh_rest[R,3,A,S], opacity[1,A,S]) with
     A = state.n_chunks_visible, plus packed_grad (whose slot 9 carries the statistics term).
 
     accumulate_into: dict of DENSE contiguous gradient tensors shaped like the parameters; when given, this
     view's gradients are added into them by the kernel itself and no compacted tensors are produced
-    (returns (None, packed_grad)).  An optional "_touched" entry (f32[C]) receives 1 at every visible chunk."""
+    (returns (None, packed_grad)).  An optional "_touched" entry (f32[C]) receives 1 at every visible chunk.
+
+    camera_grad: optional contiguous f32[2,4,4] CUDA tensor that receives (d view_matrix, d proj_matrix) of this view, with
+    J and the SH view direction held constant (DESIGN.md section 1).  It is assigned, not accumulated."""
     xyz = params["xyz"]
     dev = xyz.device
     C, S = xyz.shape[-2:]
@@ -210,8 +214,13 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
     d_img = d_img if d_img.is_contiguous() else d_img.contiguous()
     if d_trans is not None:
         d_trans = d_trans if d_trans.is_contiguous() else d_trans.contiguous()
+    if camera_grad is not None and not (camera_grad.is_cuda and camera_grad.dtype == _F32 and camera_grad.is_contiguous()
+                                        and tuple(camera_grad.shape) == (2, 4, 4)):
+        raise RuntimeError("camera_grad must be a contiguous float32 CUDA tensor of shape [2,4,4]")
     with _on(dev):
         st = _stream(dev)
+        cam_partials = None if camera_grad is None else torch.empty((max(A, 1), 32), dtype=_F32, device=dev)
+        cam_args = (_ptr(cam_partials), _ptr(camera_grad))
         pg = torch.empty((1, Nmax, 12), dtype=_F32, device=dev)
         if specific_tiles is None:
             specific_tiles = state.tile_order          # every tile, longest lists first (None = index order)
@@ -231,7 +240,9 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
                           _ptr(state.view), _ptr(state.proj), _ptr(xyz), _ptr(params["scale"]), _ptr(params["rot"]),
                           _ptr(params["opacity"]), C, S, A, R, H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(pg), None, 2,
                           _ptr(d["xyz"]), _ptr(d["scale"]), _ptr(d["rot"]), _ptr(d["sh_0"]), _ptr(d["sh_rest"]), _ptr(d["opacity"]),
-                          _ptr(d.get("_touched")), st)   # "_touched": chunk marks for the fused optimizer step
+                          _ptr(d.get("_touched")), *cam_args, st)   # "_touched": chunk marks for the fused optimizer step
+            elif camera_grad is not None:
+                camera_grad.zero_()
             return None, pg
         g_pos = torch.empty((3, A, S), dtype=_F32, device=dev)
         g_sc = torch.empty((3, A, S), dtype=_F32, device=dev)
@@ -244,7 +255,9 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
             _lib.call("lgs_project_backward", state.sh_degree, _ptr(state.chunk_ids), ctypes.c_void_p(state.counters.data_ptr()),
                       _ptr(state.view), _ptr(state.proj), _ptr(xyz), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["opacity"]),
                       C, S, A, R, H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(pg), None, 0, _ptr(g_pos), _ptr(g_sc), _ptr(g_rot),
-                      _ptr(g_s0), _ptr(g_sr), _ptr(g_op), None, st)
+                      _ptr(g_s0), _ptr(g_sr), _ptr(g_op), None, *cam_args, st)
+        elif camera_grad is not None:
+            camera_grad.zero_()
     return [g_pos, g_sc, g_rot, g_s0, g_sr, g_op], pg
 
 
@@ -301,6 +314,7 @@ class ViewWorkspace:
         self.pg = e((1, N, 12), _F32)
         self.d_img = e((1, 3, self.Hp, self.Wp), _F32)
         self.cam_view, self.cam_proj, self.cam_planes = e((1, 4, 4), _F32), e((1, 4, 4), _F32), e((1, 6, 4), _F32)
+        self.cam_partials, self.d_cam = e((C, 32), _F32), e((2, 4, 4), _F32)     # camera gradient: per-chunk rows, their sum
         nb = max(_query_bytes("lgs_sort_pairs_u32_workspace_bytes", _round_up(N, 1 << 16)),
                  _query_bytes("lgs_scan_gathered_workspace_bytes", _round_up(N, 1 << 16)),
                  _query_bytes(f"lgs_sort_pairs_{'u16' if self.u16 else 'u32'}_workspace_bytes", _round_up(D, 1 << 18)))
@@ -346,7 +360,7 @@ class ViewWorkspace:
         if order:
             _lib.call("lgs_tile_order", _ptr(self.work), 1, self.ntile, _ptr(self.tile_order), st)
 
-    def _backward_kernels(self, params, sh_degree, accumulate_into, use_clamp):
+    def _backward_kernels(self, params, sh_degree, accumulate_into, use_clamp, camera_grad):
         st = _stream(self.dev)
         H, W = self.hw
         th, tw = self.tile
@@ -361,7 +375,8 @@ class ViewWorkspace:
         _lib.call("lgs_project_backward", int(sh_degree), _ptr(self.chunk_ids), ctypes.c_void_p(self.counters.data_ptr()), _ptr(self.cam_view),
                   _ptr(self.cam_proj), _ptr(params["xyz"]), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["opacity"]), C, S, C, R,
                   H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(self.pg), None, 2, _ptr(d["xyz"]), _ptr(d["scale"]), _ptr(d["rot"]),
-                  _ptr(d["sh_0"]), _ptr(d["sh_rest"]), _ptr(d["opacity"]), _ptr(d.get("_touched")), st)
+                  _ptr(d["sh_0"]), _ptr(d["sh_rest"]), _ptr(d["opacity"]), _ptr(d.get("_touched")),
+                  _ptr(self.cam_partials) if camera_grad else None, _ptr(self.d_cam) if camera_grad else None, st)
 
     def _run(self, kind, sig, fn):
         """Eager the first time a pointer signature is seen, captured into a CUDA graph the second time, replayed afterwards."""
@@ -395,8 +410,11 @@ class ViewWorkspace:
         self.views_done += 1
         return self.img
 
-    def backward(self, params, d_img, sh_degree, accumulate_into, use_clamp=True):
-        """d_img f32[1,3,H,W] or [1,3,Hp,Wp]: gradient of the loss w.r.t. the (clamped) image."""
+    def backward(self, params, d_img, sh_degree, accumulate_into, use_clamp=True, camera_grad=None):
+        """d_img f32[1,3,H,W] or [1,3,Hp,Wp]: gradient of the loss w.r.t. the (clamped) image.  camera_grad (optional f32[2,4,4]
+        CUDA tensor) receives (d view_matrix, d proj_matrix) of this view, copied on the stream after the backward."""
+        if camera_grad is not None and not (camera_grad.is_cuda and camera_grad.dtype == _F32 and tuple(camera_grad.shape) == (2, 4, 4)):
+            raise RuntimeError("camera_grad must be a float32 CUDA tensor of shape [2,4,4]")
         H, W = self.hw
         if d_img.shape[-2:] == (self.Hp, self.Wp):
             self.d_img.copy_(d_img, non_blocking=True)
@@ -407,8 +425,11 @@ class ViewWorkspace:
         sig = (tuple(params[k].data_ptr() for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")),
                tuple(accumulate_into[k].data_ptr() for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")),
                0 if accumulate_into.get("_touched") is None else accumulate_into["_touched"].data_ptr(), int(sh_degree), bool(use_clamp),
-               bool(CONFIG["tile_order"]))
-        self._run("bwd", sig, lambda: self._backward_kernels(params, sh_degree, accumulate_into, use_clamp))
+               bool(CONFIG["tile_order"]), camera_grad is not None)
+        cam = camera_grad is not None
+        self._run("bwd", sig, lambda: self._backward_kernels(params, sh_degree, accumulate_into, use_clamp, cam))
+        if cam:
+            camera_grad.copy_(self.d_cam, non_blocking=True)
 
     # -- feedback --------------------------------------------------------------------------------------------------
     def post_flags(self):

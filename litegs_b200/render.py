@@ -155,14 +155,22 @@ class _RenderViewFn(torch.autograd.Function):
         if g_img is None:
             g_img = torch.zeros((1, 3, *state.T.shape[-2:]), dtype=torch.float32, device=xyz.device)
         # ... and the backward kernel applies that clamp's gradient mask from the saved image
+        # camera gradient only when the view or projection matrix asks for one: otherwise the kernel without it runs
+        cam = None
+        if ctx.needs_input_grad[9] or ctx.needs_input_grad[10]:
+            cam = torch.empty((2, 4, 4), dtype=torch.float32, device=xyz.device)
         grads, pg = pipeline.render_view_backward(params, state, g_img, g_T if (ctx.trans and g_T is not None) else None,
                                                   enable_statistic=ctx.stat,
-                                                  accumulate_into=ctx.accumulate_into, clamped_img=img_out)
+                                                  accumulate_into=ctx.accumulate_into, clamped_img=img_out, camera_grad=cam)
         if ctx.stat:
             _feed_statistics(state, ctx.stats, pg, state.tile)
+        g_view = g_proj = None
+        if cam is not None:
+            g_view = cam[0].reshape(state.view.shape) if ctx.needs_input_grad[9] else None
+            g_proj = cam[1].reshape(state.proj.shape) if ctx.needs_input_grad[10] else None
         if grads is None:          # gradients went straight into the caller's dense buffers
             ctx.state = None
-            return (None,) * 19
+            return (None,) * 9 + (g_view, g_proj) + (None,) * 8
         C, S = xyz.shape[-2:]
         ids = state.chunk_ids[: state.n_chunks_visible]
         out = []
@@ -170,7 +178,7 @@ class _RenderViewFn(torch.autograd.Function):
             ct = CompactedTensor((*g.shape[:-2], C, S), ids, g)
             out.append(ct if ctx.sparse else ct.to_dense())
         ctx.state = None
-        return (*out, None, None, None, None, None, None, None, None, None, None, None, None, None)
+        return (*out, None, None, None, g_view, g_proj, None, None, None, None, None, None, None, None)
 
 
 def render_view(cluster_origin, cluster_extend, frustumplane, view_matrix, proj_matrix,
@@ -214,7 +222,7 @@ def _streams(dev, n):
 
 def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_extend,
                  xyz, scale, rot, sh_0, sh_rest, opacity, actived_sh_degree: int, output_shape, pp,
-                 accumulate_into: dict, n_streams: int = 4, loss_and_grad_fn=None):
+                 accumulate_into: dict, n_streams: int = 4, loss_and_grad_fn=None, camera_grads=None):
     """Forward + backward of a batch of views with the gradients summed into ``accumulate_into`` (dense tensors shaped
     like the parameters, e.g. ``GradAccumulator.grads()``).  This is the per-rank body of a data-parallel step.
 
@@ -228,8 +236,15 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
 
     ``loss_and_grad_fn(i, img) -> (loss, d_img)`` (with ``loss_fn=None``) skips autograd altogether: the pipeline's forward
     and backward are called directly (no autograd Function, no engine hop: ~0.1 ms less host time per view), the image
-    handed to the function is the kernel's clamp(0,1) output and its gradient goes straight to the raster backward."""
+    handed to the function is the kernel's clamp(0,1) output and its gradient goes straight to the raster backward.
+
+    ``camera_grads`` (optional contiguous f32[n_views,2,4,4] CUDA tensor): slot i receives (d view_matrix, d proj_matrix) of view i
+    (pipeline.render_view_backward), on every path; it is complete when this function returns (the current stream waits)."""
     dev = xyz.device
+    if camera_grads is not None and not (camera_grads.is_cuda and camera_grads.dtype == torch.float32 and camera_grads.is_contiguous()
+                                         and tuple(camera_grads.shape) == (n_views, 2, 4, 4)):
+        raise RuntimeError(f"camera_grads must be a contiguous float32 CUDA tensor of shape [{n_views},2,4,4]")
+    slot = (lambda i: None) if camera_grads is None else (lambda i: camera_grads[i])
     losses = []
     H, W = int(output_shape[0]), int(output_shape[1])
     th, tw = int(pp.tile_size[0]), int(pp.tile_size[1])
@@ -258,14 +273,17 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
         if wait_ev is not None:
             torch.cuda.current_stream(dev).wait_event(wait_ev)
         _, pg_ = pipeline.render_view_backward(params, state, d_img, None, enable_statistic=stat, accumulate_into=accumulate_into,
-                                               clamped_img=img_p)
+                                               clamped_img=img_p, camera_grad=slot(i))
         if stat:
             _feed_statistics(state, stats, pg_, (th, tw))
         losses.append(loss.detach())
 
     def one_autograd(i, wait_ev):
         cam = camera_fn(i)
-        img = render_view(cluster_origin, cluster_extend, cam["frustumplane"], cam["view"], cam["proj"], xyz, scale, rot, sh_0, sh_rest,
+        view, proj = cam["view"], cam["proj"]
+        if camera_grads is not None:              # leaves of this call: their .grad is view i's camera gradient
+            view, proj = view.detach().requires_grad_(True), proj.detach().requires_grad_(True)
+        img = render_view(cluster_origin, cluster_extend, cam["frustumplane"], view, proj, xyz, scale, rot, sh_0, sh_rest,
                           opacity, actived_sh_degree, output_shape, pp, accumulate_into=accumulate_into)[0]
         loss = loss_fn(i, img)
         if wait_ev is not None:          # the previous view's accumulate (other stream) must have landed
@@ -275,6 +293,8 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
             img.backward(d_img)
         else:
             loss.backward()
+        if camera_grads is not None:
+            camera_grads[i, 0].copy_(view.grad.reshape(4, 4)); camera_grads[i, 1].copy_(proj.grad.reshape(4, 4))
         losses.append(loss.detach())
 
     # GPU-driven path (default): one preallocated ViewWorkspace per stream slot, no host synchronisation inside the batch, the
@@ -301,7 +321,7 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
                 (d_img,) = torch.autograd.grad(loss, leaf)
         if wait_ev is not None:
             torch.cuda.current_stream(dev).wait_event(wait_ev)
-        ws.backward(params, d_img, int(actived_sh_degree), accumulate_into, use_clamp=True)
+        ws.backward(params, d_img, int(actived_sh_degree), accumulate_into, use_clamp=True, camera_grad=slot(i))
         losses.append(loss.detach())
 
     def one_probe(i, wait_ev):

@@ -209,6 +209,28 @@ class GaussiansRasterFunc(torch.autograd.Function):
         return None, None, d_ndc, d_cov, d_color, d_opacity, None, None, None, None, None, None, None
 
 
+class CreateViewProj(torch.autograd.Function):
+    """Learnable cameras (wrapper.py:772-791): view_params f32[V,7], recp_tan_half_fov_x f32[1] -> view, proj, viewproj,
+    frustumplane.  The Level A operators above return no view-matrix gradient, as the reference's do; the camera gradient
+    comes from render.render_view (Level B)."""
+
+    @staticmethod
+    def forward(ctx, view_params, proj_params, img_h: int, img_w: int, z_near: float, z_far: float):
+        view_matrix, proj_matrix, viewproj_matrix, frustumplane = litegs_fused.create_viewproj_forward(view_params, proj_params, img_h, img_w,
+                                                                                                      z_near, z_far)
+        ctx.save_for_backward(view_params, proj_params)
+        ctx.geom = (img_h, img_w, z_near, z_far)
+        ctx.mark_non_differentiable(frustumplane)
+        return view_matrix, proj_matrix, viewproj_matrix, frustumplane
+
+    @staticmethod
+    def backward(ctx, view_matrix_grad, proj_matrix_grad, viewproj_matrix_grad, frustumplane_grad):
+        view_params, proj_params = ctx.saved_tensors
+        g_view, g_proj = litegs_fused.create_viewproj_backward(view_matrix_grad, proj_matrix_grad, viewproj_matrix_grad, view_params,
+                                                               proj_params, *ctx.geom)
+        return g_view, g_proj, None, None, None, None
+
+
 class CullCompactActivateWithSparseGrad(torch.autograd.Function):
     """Gather visible chunks, activate, SH->RGB; gradients come back chunk-compacted
     (wrapper.py:793-845).  With b_sparse_grad=False they are scattered into dense tensors (the
