@@ -29,6 +29,8 @@ def main():
     ap.add_argument("--width", type=int, default=960)
     ap.add_argument("--height", type=int, default=540)
     ap.add_argument("--sh-degree", type=int, default=3)
+    ap.add_argument("--antialiased", action="store_true",
+                    help="opacity compensation of the 2D filter (for models trained in that mode, or renders at another resolution)")
     a = ap.parse_args()
     path = a.ply
     if a.make:
@@ -58,7 +60,7 @@ def main():
         for cam, hw, _ in cams:
             c = {k: torch.from_numpy(v).to(dev) for k, v in cam.items()}
             img, _, _ = pipeline.render_view_forward(P, A[0], A[1], c["frustumplane"], c["view"], c["proj"], a.sh_degree, hw, (8, 16),
-                                                     clamp_zero=True)
+                                                     clamp_zero=True, antialiased=a.antialiased)
             imgs.append(img[0, :, : hw[0], : hw[1]])
     torch.cuda.synchronize()
     dt = time.perf_counter() - t0

@@ -84,14 +84,14 @@ def load_dataset(root, image_dir="images", dev=None):
     return frames, np.stack([p.xyz for p in P]), np.stack([p.rgb for p in P])
 
 
-def train(root, iters=300, views_per_step=8, log=print, refine_poses=False):
+def train(root, iters=300, views_per_step=8, log=print, refine_poses=False, antialiased=False):
     from litegs_b200 import fused
     if refine_poses and int(os.environ.get("WORLD_SIZE", "1")) > 1:
         raise ValueError("--refine-poses runs on one GPU: multi-GPU pose refinement is not supported")
     keep = fused.CONFIG["true_sigmoid_grad"]
     fused.CONFIG["true_sigmoid_grad"] = True               # our own loops train with the true sigmoid derivative (SURVEY Q15)
     try:
-        return _train(root, iters, views_per_step, log, refine_poses)
+        return _train(root, iters, views_per_step, log, refine_poses, antialiased)
     finally:
         fused.CONFIG["true_sigmoid_grad"] = keep
 
@@ -128,7 +128,7 @@ class _Poses:
         self.opt.step()
 
 
-def _train(root, iters, views_per_step, log, refine_poses=False):
+def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=False):
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", 0)))
     torch.cuda.set_device(dev)
     frames, xyz, rgb = load_dataset(root, dev=dev)
@@ -138,7 +138,7 @@ def _train(root, iters, views_per_step, log, refine_poses=False):
     cgrads = torch.empty((views_per_step, 2, 4, 4), dtype=torch.float32, device=dev) if poses else None
     g = colmap.gaussians_from_points(xyz, rgb, sh_degree=3)
     P = {k: torch.from_numpy(g[k]).to(dev) for k in PARAM_ORDER}
-    pp = PipelineParams(tile_size=(8, 16), sparse_grad=True)
+    pp = PipelineParams(tile_size=(8, 16), sparse_grad=True, antialiased=antialiased)
     acc = lgs_dist.GradAccumulator(P)
     extent = float(np.linalg.norm(xyz.max(0) - xyz.min(0)) * 0.5)
     opt, sched = optimizer.get_optimizer(P, spatial_lr_scale=extent)
@@ -186,6 +186,7 @@ if __name__ == "__main__":
     ap.add_argument("--data", default=None)
     ap.add_argument("--iters", type=int, default=300)
     ap.add_argument("--refine-poses", action="store_true", help="also optimise the camera extrinsics (one GPU)")
+    ap.add_argument("--antialiased", action="store_true", help="train (and evaluate) in the antialiased mode")
     ap.add_argument("--pose-noise", type=float, nargs=2, default=None, metavar=("DEG", "FRAC"),
                     help="with --make: perturb the written poses by DEG degrees and FRAC of the camera distance")
     a = ap.parse_args()
@@ -194,5 +195,5 @@ if __name__ == "__main__":
         root = make_dataset(a.make, pose_noise=a.pose_noise)
     if root is None:
         ap.error("give --data or --make")
-    h, _ = train(root, a.iters, refine_poses=a.refine_poses)
+    h, _ = train(root, a.iters, refine_poses=a.refine_poses, antialiased=a.antialiased)
     assert h[-1] < h[0]

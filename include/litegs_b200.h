@@ -254,12 +254,15 @@ int lgs_set_err_square_mode(int mode);
  * depth_key u32 (float bits of view z, 0xFFFFFFFF when invisible), iota u32 (slot index), tile_count i32,
  * totals i32[3] = { number of (tile,splat) pairs, ~min and max of the depth keys of the splats that have pairs }
  * (so the depth sort can be limited to the bits in which those keys differ; splats without pairs may land anywhere
- * in the order, they emit nothing). */
+ * in the order, they emit nothing).
+ * antialiased != 0: antialiased mode, ours (the reference has none).  The record's opacity is sigmoid(opacity) * rho with
+ * rho = sqrt(det(M^T M) / det(M^T M + 0.3 I)), the opacity compensation of the 2D low-pass filter (DESIGN.md section 1);
+ * the visibility test, the tile walk and the rasteriser all see that opacity.  0 = the reference's behaviour. */
 int lgs_project_forward(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
                         const float* view_matrix, const float* proj_matrix, const float* position, const float* scale,
                         const float* rotation, const float* sh_base, const float* sh_rest, const float* opacity, int C,
                         int S, int A, int img_h, int img_w, int tile_h, int tile_w, float* packed_params,
-                        unsigned* depth_key, unsigned* iota, int* tile_count, int* totals, void* stream);
+                        unsigned* depth_key, unsigned* iota, int* tile_count, int* totals, int antialiased, void* stream);
 
 /* duplicate_with_keys (GR/binning.cu:33-110) reading the packed record: offset = inclusive scan of the depth-ordered
  * counts, order = depth-sorted slot ids; keys/vals i32[cap] must be zero-initialised by the caller. */
@@ -279,13 +282,16 @@ int lgs_emit_pairs_u16(const float* packed_params, const int* offset, const unsi
  * (d_cam[0..15], row-vector [k*4+j]) and of the projection matrix (d_cam[16..31]) through the NDC mean and the V3x3 factor of
  * the 2D covariance, with J and the SH direction held constant (the convention of the position gradient, DESIGN.md section 1).
  * The reference's operators return no view-matrix gradient (wrapper.py:285,407,845); this one is new.  Summed in a fixed
- * order (bit-reproducible), no host synchronisation; needs S % 32 == 0. */
+ * order (bit-reproducible), no host synchronisation; needs S % 32 == 0.
+ * antialiased: must equal the value the forward of this view was given (ours, no reference counterpart).  The record
+ * gradient is then taken at the compensated opacity and the gradient of rho flows into scale, rotation and the camera. */
 int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
                          const float* view_matrix, const float* proj_matrix, const float* position, const float* scale,
                          const float* rotation, const float* opacity, int C, int S, int A, int rest_dim, int img_h,
                          int img_w, int true_sigmoid_grad, const float* packed_grad, const float* grad_inv_scaler,
                          int zero_outputs, float* g_position, float* g_scale, float* g_rotation, float* g_sh_base,
-                         float* g_sh_rest, float* g_opacity, float* touched, float* cam_partials, float* d_cam, void* stream);
+                         float* g_sh_rest, float* g_opacity, float* touched, float* cam_partials, float* d_cam, int antialiased,
+                         void* stream);
 
 /* create_viewproj_forward, GR/compact.cu:17-141: view_params f32[V,7] (qw qx qy qz tx ty tz), recp_tan_half_fov_x f32[1] ->
  * view, proj, viewproj f32[V,4,4] (row-vector convention) and frustumplane f32[V,6,4].  One thread per view. */

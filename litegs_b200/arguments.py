@@ -11,3 +11,6 @@ class PipelineParams:
     enable_transmitance: bool = False
     enable_depth: bool = False
     input_color_type: str = "sh"
+    # ours, not the reference's: antialiased mode of the fused path (DESIGN.md section 1).  Readers use
+    # getattr(pp, "antialiased", False), so the reference's own PipelineParams keeps working.
+    antialiased: bool = False

@@ -107,8 +107,32 @@ __device__ __forceinline__ void project_chain(const float* __restrict__ Vm, cons
     t.inv[0] = c11 * dr; t.inv[1] = -c01 * dr; t.inv[2] = c00 * dr;
 }
 
+// Antialiased mode (DESIGN.md section 1): the opacity compensation of the 2D low-pass filter,
+// rho = sqrt(det(M^T M) / det(M^T M + 0.3 I)).  Every step is one correctly rounded op in a fixed order, so that the
+// opacity the tile decision sees is the oracle's bit for bit.
+struct AAFactor {
+    float a00, a01, a11;            // M^T M (unfiltered 2D covariance)
+    float c00, c11;                 // diagonal of the filtered covariance
+    float det_o, det_b, r2, rho;
+};
+
+__device__ __forceinline__ void antialias_factor(const float* M, AAFactor& f)
+{
+    f.a00 = __fadd_rn(__fadd_rn(__fmul_rn(M[0], M[0]), __fmul_rn(M[2], M[2])), __fmul_rn(M[4], M[4]));
+    f.a01 = __fadd_rn(__fadd_rn(__fmul_rn(M[0], M[1]), __fmul_rn(M[2], M[3])), __fmul_rn(M[4], M[5]));
+    f.a11 = __fadd_rn(__fadd_rn(__fmul_rn(M[1], M[1]), __fmul_rn(M[3], M[3])), __fmul_rn(M[5], M[5]));
+    f.c00 = __fadd_rn(f.a00, 0.3f);
+    f.c11 = __fadd_rn(f.a11, 0.3f);
+    const float a01sq = __fmul_rn(f.a01, f.a01);
+    f.det_o = __fsub_rn(__fmul_rn(f.a00, f.a11), a01sq);
+    f.det_b = __fsub_rn(__fmul_rn(f.c00, f.c11), a01sq);
+    f.r2 = __fdiv_rn(f.det_o, f.det_b);
+    f.rho = __fsqrt_rn(fmaxf(f.r2, 0.0f));
+}
+
 // grid = allocated chunks (all M: chunks >= *visible_num write an invisible record), block = chunk size
-template <int DEG, int TH, int TW>
+// AA: the record's opacity is sigma(o_raw) * rho (antialiased mode); everything downstream reads it from the record.
+template <int DEG, int TH, int TW, bool AA>
 __global__ void project_forward_kernel(
     const int64_t* __restrict__ chunk_ids, const int* __restrict__ visible_num, const float* __restrict__ view,
     const float* __restrict__ proj, const float* __restrict__ pos, const float* __restrict__ scale,
@@ -130,6 +154,11 @@ __global__ void project_forward_kernel(
         float q[4] = { rot[src], rot[CS + src], rot[2 * CS + src], rot[3 * CS + src] };
         ProjIntermediates t;
         project_chain(view, proj, p, sr_, q, opac[src], H, W, t);
+        if constexpr (AA) {
+            AAFactor f;
+            antialias_factor(t.M, f);
+            t.o = __fmul_rn(t.o, f.rho);
+        }
         // colour (GR/compact.cu:573-653), no clamp on this path (SURVEY Q13)
         constexpr int K = (DEG + 1) * (DEG + 1);
         float b[16];
@@ -188,7 +217,7 @@ extern "C" int lgs_project_forward(int sh_degree, const int64_t* visible_chunk_i
                                    const float* scale, const float* rotation, const float* sh_base, const float* sh_rest,
                                    const float* opacity, int C, int S, int A, int img_h, int img_w, int tile_h, int tile_w,
                                    float* packed_params, unsigned* depth_key, unsigned* iota, int* tile_count, int* totals,
-                                   void* stream)
+                                   int antialiased, void* stream)
 {
     LGS_REQUIRE(sh_degree >= 0 && sh_degree <= 3, "project_forward: sh_degree %d not in 0..3", sh_degree);
     LGS_REQUIRE(lgs_tile_ok(tile_h, tile_w), "project_forward: tile %dx%d not one of 8x16, 12x16, 16x16, 8x8", tile_h, tile_w);
@@ -197,10 +226,16 @@ extern "C" int lgs_project_forward(int sh_degree, const int64_t* visible_chunk_i
     LGS_CUDA(cudaMemsetAsync(totals, 0, 3 * sizeof(int), st));
     if (A == 0) return LGS_OK;
     int gx = (img_w + tile_w - 1) / tile_w, gy = (img_h + tile_h - 1) / tile_h;
-#define PF(D) project_forward_kernel<D, TH, TW><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num, view_matrix, proj_matrix, position, \
-        scale, rotation, sh_base, sh_rest, opacity, C, S, img_h, img_w, gx, gy, (SplatRec*)packed_params, depth_key, iota, tile_count, totals)
-    LGS_DISPATCH_TILE(tile_h, tile_w,
-        switch (sh_degree) { case 0: PF(0); break; case 1: PF(1); break; case 2: PF(2); break; default: PF(3); })
+#define PF(D, AA) project_forward_kernel<D, TH, TW, AA><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num, view_matrix, proj_matrix, \
+        position, scale, rotation, sh_base, sh_rest, opacity, C, S, img_h, img_w, gx, gy, (SplatRec*)packed_params, depth_key, iota,    \
+        tile_count, totals)
+    if (antialiased) {
+        LGS_DISPATCH_TILE(tile_h, tile_w,
+            switch (sh_degree) { case 0: PF(0, true); break; case 1: PF(1, true); break; case 2: PF(2, true); break; default: PF(3, true); })
+    } else {
+        LGS_DISPATCH_TILE(tile_h, tile_w,
+            switch (sh_degree) { case 0: PF(0, false); break; case 1: PF(1, false); break; case 2: PF(2, false); break; default: PF(3, false); })
+    }
 #undef PF
     LGS_CHECK_LAUNCH("project_forward_kernel");
     return LGS_OK;
@@ -388,7 +423,9 @@ __device__ __forceinline__ float warp_sum32_transposed(float* v)
 // CAM: also the camera gradient (DESIGN.md section 1, "Camera gradient").  Each thread forms its contribution to
 // d_view[16] and d_proj[16]; the block sums them in a fixed order and writes one row of cam_partials f32[A,32] per
 // chunk (chunks at or past the visible count write zeros); camera_grad_sum_kernel folds the rows.
-template <int DEG, bool CAM>
+// AA: antialiased mode.  The record gradient is taken at o_eff = sigma(o_raw) * rho; d o = d o_eff * rho, and the rho path
+// adds d det(M^T M) and d det(M^T M + 0.3 I) to d cov2d before dM = 2 M G, so ds, dq and the camera path all see it.
+template <int DEG, bool CAM, bool AA>
 __global__ void project_backward_kernel(
     const int64_t* __restrict__ chunk_ids, const int* __restrict__ visible_num, const float* __restrict__ view,
     const float* __restrict__ proj, const float* __restrict__ pos, const float* __restrict__ scale,
@@ -429,19 +466,39 @@ __global__ void project_backward_kernel(
         const float o_raw = opac[src];
         ProjIntermediates t;
         project_chain(view, proj, p, sr_, q, o_raw, H, W, t);
+        AAFactor f;
+        float o_rec = t.o;                                  // the record's opacity
+        if constexpr (AA) {
+            antialias_factor(t.M, f);
+            o_rec = __fmul_rn(t.o, f.rho);
+        }
         // raw moments -> record gradient (GR/raster.cu:826-841), then unpack (GR/raster.cu:870-884)
         LgsRasterGrad rgd;
-        lgs_finish_raster_grad(ga, gb, gc, t.inv[0], t.inv[1], t.inv[2], t.o, rgd);
+        lgs_finish_raster_grad(ga, gb, gc, t.inv[0], t.inv[1], t.inv[2], o_rec, rgd);
         const float d_ndcx = rgd.dmx * 0.5f * W * sc, d_ndcy = rgd.dmy * 0.5f * H * sc;
         const float dA = rgd.dA * sc, dBh = rgd.dB * 0.5f * sc, dC = rgd.dC * sc;
         const float dcol[3] = { gb.y * sc, gb.z * sc, gb.w * sc };
-        const float d_o = rgd.dop * sc;
+        float d_o = rgd.dop * sc;
         // inverse backward: dCov = -(inv . dInv . inv) (GR/transform.cu:1446-1450), NaN -> 0
         const float iA = t.inv[0], iB = t.inv[1], iC = t.inv[2];
         float t00 = iA * dA + iB * dBh, t01 = iA * dBh + iB * dC, t10 = iB * dA + iC * dBh, t11 = iB * dBh + iC * dC;
         float G[4];
         G[0] = nan_to_num0(-(t00 * iA + t01 * iB)); G[1] = nan_to_num0(-(t00 * iB + t01 * iC));
         G[2] = nan_to_num0(-(t10 * iA + t11 * iB)); G[3] = nan_to_num0(-(t10 * iB + t11 * iC));
+        if constexpr (AA) {
+            // o_eff = o sqrt(r2), r2 = det_o / det_b; rho = 0 means an invisible record, which gets no gradient
+            if (f.rho > 0.0f) {
+                const float d_r2 = d_o * t.o / (2.0f * f.rho);
+                const float d_det_o = d_r2 / f.det_b;
+                const float d_det_b = -d_r2 * f.r2 / f.det_b;
+                const float d_a01_half = -f.a01 * (d_det_o + d_det_b);
+                G[0] += d_det_o * f.a11 + d_det_b * f.c11;
+                G[3] += d_det_o * f.a00 + d_det_b * f.c00;
+                G[1] += d_a01_half;
+                G[2] += d_a01_half;
+            }
+            d_o = d_o * f.rho;
+        }
         // cov2d backward: dT = 2 M G (VJ)^T (GR/transform.cu:861-880)
         float dT[9];
         float dM[CAM ? 6 : 1];
@@ -597,7 +654,7 @@ extern "C" int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_
                                     int rest_dim, int img_h, int img_w, int true_sigmoid_grad, const float* packed_grad,
                                     const float* grad_inv_scaler, int zero_outputs, float* g_position, float* g_scale,
                                     float* g_rotation, float* g_sh_base, float* g_sh_rest, float* g_opacity, float* touched,
-                                    float* cam_partials, float* d_cam, void* stream)
+                                    float* cam_partials, float* d_cam, int antialiased, void* stream)
 {
     LGS_REQUIRE(sh_degree >= 0 && sh_degree <= 3, "project_backward: sh_degree %d not in 0..3", sh_degree);
     LGS_REQUIRE(rest_dim >= (sh_degree + 1) * (sh_degree + 1) - 1, "project_backward: sh_rest has %d rows, degree %d needs %d", rest_dim,
@@ -621,14 +678,16 @@ extern "C" int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_
         LGS_CUDA(cudaMemsetAsync(g_sh_rest, 0, sizeof(float) * (size_t)rest_dim * 3 * AS, st));
         LGS_CUDA(cudaMemsetAsync(g_opacity, 0, sizeof(float) * AS, st));
     }
-#define PB(D, K) project_backward_kernel<D, K><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num, view_matrix, proj_matrix, position, \
-        scale, rotation, opacity, C, S, A, rest_dim, img_h, img_w, true_sigmoid_grad, accumulate, packed_grad, grad_inv_scaler, g_position, \
-        g_scale, g_rotation, g_sh_base, g_sh_rest, g_opacity, touched, cam_partials)
-    if (cam) {
-        switch (sh_degree) { case 0: PB(0, true); break; case 1: PB(1, true); break; case 2: PB(2, true); break; default: PB(3, true); }
+#define PB(D, K, AA) project_backward_kernel<D, K, AA><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num, view_matrix, proj_matrix, \
+        position, scale, rotation, opacity, C, S, A, rest_dim, img_h, img_w, true_sigmoid_grad, accumulate, packed_grad, grad_inv_scaler,  \
+        g_position, g_scale, g_rotation, g_sh_base, g_sh_rest, g_opacity, touched, cam_partials)
+#define PB_DEG(K, AA) switch (sh_degree) { case 0: PB(0, K, AA); break; case 1: PB(1, K, AA); break; case 2: PB(2, K, AA); break; default: PB(3, K, AA); }
+    if (antialiased) {
+        if (cam) { PB_DEG(true, true) } else { PB_DEG(false, true) }
     } else {
-        switch (sh_degree) { case 0: PB(0, false); break; case 1: PB(1, false); break; case 2: PB(2, false); break; default: PB(3, false); }
+        if (cam) { PB_DEG(true, false) } else { PB_DEG(false, false) }
     }
+#undef PB_DEG
 #undef PB
     LGS_CHECK_LAUNCH("project_backward_kernel");
     if (cam) {

@@ -62,6 +62,7 @@ class ViewState:
     T: torch.Tensor                  # f32[1,1,Hp,Wp]
     last: torch.Tensor               # i16[1,1,Hp,Wp] (unsigned 16-bit counts)
     tile_order: Optional[torch.Tensor] = None   # i32[1,tiles]: tile ids, heaviest backward work first
+    antialiased: bool = False        # antialiased mode (DESIGN.md section 1): the backward must use the forward's setting
 
 
 class _Pinned:
@@ -78,10 +79,14 @@ class _Pinned:
 
 def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_extend: torch.Tensor, frustumplane: torch.Tensor,
                         view_matrix: torch.Tensor, proj_matrix: torch.Tensor, sh_degree: int, hw: tuple, tile: tuple,
-                        enable_statistic: bool = False, specific_tiles: Optional[torch.Tensor] = None, clamp_zero: bool = False):
+                        enable_statistic: bool = False, specific_tiles: Optional[torch.Tensor] = None, clamp_zero: bool = False,
+                        antialiased: bool = False):
     """Forward of one view.  params: xyz[3,C,S] scale[3,C,S] rot[4,C,S] sh_0[1,3,C,S] sh_rest[R,3,C,S]
     opacity[1,C,S] (raw, clustered; float32 CUDA, contiguous).  Returns (img f32[1,3,Hp,Wp] padded to whole
-    tiles, ViewState, (fragment_count, fragment_weight) or None)."""
+    tiles, ViewState, (fragment_count, fragment_weight) or None).
+
+    antialiased: scale each splat's opacity by the compensation of the 2D low-pass filter (DESIGN.md section 1), so that its
+    integrated alpha does not depend on the resolution.  The state remembers it for the backward."""
     xyz = params["xyz"]
     dev = xyz.device
     C, S = xyz.shape[-2:]
@@ -112,7 +117,7 @@ def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_exte
         _lib.call("lgs_project_forward", int(sh_degree), _ptr(ids), ctypes.c_void_p(counters.data_ptr()), _ptr(view_matrix),
                   _ptr(proj_matrix), _ptr(xyz), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["sh_0"]),
                   _ptr(params["sh_rest"]), _ptr(params["opacity"]), C, S, M, H, W, th, tw, _ptr(packed), _ptr(dkey), _ptr(iota),
-                  _ptr(tcount), ctypes.c_void_p(counters.data_ptr() + 4), st)
+                  _ptr(tcount), ctypes.c_void_p(counters.data_ptr() + 4), int(bool(antialiased)), st)
         pinned = _Pinned.get(dev)
         pinned.copy_(counters, non_blocking=True)
         torch.cuda.current_stream(dev).synchronize()
@@ -183,7 +188,7 @@ def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_exte
             _lib.call("lgs_tile_order", _ptr(work), 1, ntile, _ptr(order), st)
     state = ViewState(sh_degree=int(sh_degree), hw=(H, W), tile=(th, tw), n_chunks_visible=nvis, n_pairs=D, chunk_ids=ids,
                       counters=counters, view=view_matrix, proj=proj_matrix, packed=packed, tile_count=tcount,
-                      sorted_pid=sorted_pid, ranges=ranges, T=T, last=last, tile_order=order)
+                      sorted_pid=sorted_pid, ranges=ranges, T=T, last=last, tile_order=order, antialiased=bool(antialiased))
     return img, state, stats
 
 
@@ -240,7 +245,7 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
                           _ptr(state.view), _ptr(state.proj), _ptr(xyz), _ptr(params["scale"]), _ptr(params["rot"]),
                           _ptr(params["opacity"]), C, S, A, R, H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(pg), None, 2,
                           _ptr(d["xyz"]), _ptr(d["scale"]), _ptr(d["rot"]), _ptr(d["sh_0"]), _ptr(d["sh_rest"]), _ptr(d["opacity"]),
-                          _ptr(d.get("_touched")), *cam_args, st)   # "_touched": chunk marks for the fused optimizer step
+                          _ptr(d.get("_touched")), *cam_args, int(state.antialiased), st)   # "_touched": chunk marks for the fused optimizer step
             elif camera_grad is not None:
                 camera_grad.zero_()
             return None, pg
@@ -255,7 +260,7 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
             _lib.call("lgs_project_backward", state.sh_degree, _ptr(state.chunk_ids), ctypes.c_void_p(state.counters.data_ptr()),
                       _ptr(state.view), _ptr(state.proj), _ptr(xyz), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["opacity"]),
                       C, S, A, R, H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(pg), None, 0, _ptr(g_pos), _ptr(g_sc), _ptr(g_rot),
-                      _ptr(g_s0), _ptr(g_sr), _ptr(g_op), None, *cam_args, st)
+                      _ptr(g_s0), _ptr(g_sr), _ptr(g_op), None, *cam_args, int(state.antialiased), st)
         elif camera_grad is not None:
             camera_grad.zero_()
     return [g_pos, g_sc, g_rot, g_s0, g_sr, g_op], pg
@@ -327,7 +332,7 @@ class ViewWorkspace:
         self.views_done = 0
 
     # -- enqueue ---------------------------------------------------------------------------------------------------
-    def _forward_kernels(self, params, cluster_origin, cluster_extend, sh_degree, clamp_zero):
+    def _forward_kernels(self, params, cluster_origin, cluster_extend, sh_degree, clamp_zero, antialiased):
         dev, st = self.dev, _stream(self.dev)
         H, W = self.hw
         th, tw = self.tile
@@ -339,7 +344,7 @@ class ViewWorkspace:
         _lib.call("lgs_project_forward", int(sh_degree), _ptr(self.chunk_ids), ctypes.c_void_p(cnt), _ptr(self.cam_view), _ptr(self.cam_proj),
                   _ptr(params["xyz"]), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["sh_0"]), _ptr(params["sh_rest"]),
                   _ptr(params["opacity"]), C, S, C, H, W, th, tw, _ptr(self.packed), _ptr(self.dkey), _ptr(self.iota), _ptr(self.tcount),
-                  ctypes.c_void_p(cnt + 4), st)
+                  ctypes.c_void_p(cnt + 4), int(antialiased), st)
         _lib.call("lgs_view_params", ctypes.c_void_p(cnt), S, D, self.planned_bits, ctypes.c_void_p(vp), _ptr(self.sticky), st)
         n_dev, d_dev, bias_dev = ctypes.c_void_p(vp), ctypes.c_void_p(vp + 4), ctypes.c_void_p(vp + 8)
         wsz = ctypes.c_size_t(self.ws_bytes)
@@ -360,7 +365,7 @@ class ViewWorkspace:
         if order:
             _lib.call("lgs_tile_order", _ptr(self.work), 1, self.ntile, _ptr(self.tile_order), st)
 
-    def _backward_kernels(self, params, sh_degree, accumulate_into, use_clamp, camera_grad):
+    def _backward_kernels(self, params, sh_degree, accumulate_into, use_clamp, camera_grad, antialiased):
         st = _stream(self.dev)
         H, W = self.hw
         th, tw = self.tile
@@ -376,7 +381,7 @@ class ViewWorkspace:
                   _ptr(self.cam_proj), _ptr(params["xyz"]), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["opacity"]), C, S, C, R,
                   H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(self.pg), None, 2, _ptr(d["xyz"]), _ptr(d["scale"]), _ptr(d["rot"]),
                   _ptr(d["sh_0"]), _ptr(d["sh_rest"]), _ptr(d["opacity"]), _ptr(d.get("_touched")),
-                  _ptr(self.cam_partials) if camera_grad else None, _ptr(self.d_cam) if camera_grad else None, st)
+                  _ptr(self.cam_partials) if camera_grad else None, _ptr(self.d_cam) if camera_grad else None, int(antialiased), st)
 
     def _run(self, kind, sig, fn):
         """Eager the first time a pointer signature is seen, captured into a CUDA graph the second time, replayed afterwards."""
@@ -399,20 +404,22 @@ class ViewWorkspace:
         self._graphs[key] = g
         g.replay()
 
-    def forward(self, params, cluster_origin, cluster_extend, cam, sh_degree, clamp_zero=True):
-        """cam: dict(view, proj, frustumplane) of device tensors.  Returns the padded image (a view of the workspace)."""
+    def forward(self, params, cluster_origin, cluster_extend, cam, sh_degree, clamp_zero=True, antialiased=False):
+        """cam: dict(view, proj, frustumplane) of device tensors.  Returns the padded image (a view of the workspace).
+        antialiased: antialiased mode (DESIGN.md section 1); the backward of this view must be given the same value."""
         self.cam_view.copy_(cam["view"], non_blocking=True)
         self.cam_proj.copy_(cam["proj"], non_blocking=True)
         self.cam_planes.copy_(cam["frustumplane"], non_blocking=True)
         sig = (tuple(params[k].data_ptr() for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")), cluster_origin.data_ptr(),
-               cluster_extend.data_ptr(), int(sh_degree), bool(clamp_zero), bool(CONFIG["tile_order"]))
-        self._run("fwd", sig, lambda: self._forward_kernels(params, cluster_origin, cluster_extend, sh_degree, clamp_zero))
+               cluster_extend.data_ptr(), int(sh_degree), bool(clamp_zero), bool(CONFIG["tile_order"]), bool(antialiased))
+        self._run("fwd", sig, lambda: self._forward_kernels(params, cluster_origin, cluster_extend, sh_degree, clamp_zero, antialiased))
         self.views_done += 1
         return self.img
 
-    def backward(self, params, d_img, sh_degree, accumulate_into, use_clamp=True, camera_grad=None):
+    def backward(self, params, d_img, sh_degree, accumulate_into, use_clamp=True, camera_grad=None, antialiased=False):
         """d_img f32[1,3,H,W] or [1,3,Hp,Wp]: gradient of the loss w.r.t. the (clamped) image.  camera_grad (optional f32[2,4,4]
-        CUDA tensor) receives (d view_matrix, d proj_matrix) of this view, copied on the stream after the backward."""
+        CUDA tensor) receives (d view_matrix, d proj_matrix) of this view, copied on the stream after the backward.
+        antialiased: the value the forward of this view was given."""
         if camera_grad is not None and not (camera_grad.is_cuda and camera_grad.dtype == _F32 and tuple(camera_grad.shape) == (2, 4, 4)):
             raise RuntimeError("camera_grad must be a float32 CUDA tensor of shape [2,4,4]")
         H, W = self.hw
@@ -425,9 +432,9 @@ class ViewWorkspace:
         sig = (tuple(params[k].data_ptr() for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")),
                tuple(accumulate_into[k].data_ptr() for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")),
                0 if accumulate_into.get("_touched") is None else accumulate_into["_touched"].data_ptr(), int(sh_degree), bool(use_clamp),
-               bool(CONFIG["tile_order"]), camera_grad is not None)
+               bool(CONFIG["tile_order"]), bool(antialiased), camera_grad is not None)
         cam = camera_grad is not None
-        self._run("bwd", sig, lambda: self._backward_kernels(params, sh_degree, accumulate_into, use_clamp, cam))
+        self._run("bwd", sig, lambda: self._backward_kernels(params, sh_degree, accumulate_into, use_clamp, cam, antialiased))
         if cam:
             camera_grad.copy_(self.d_cam, non_blocking=True)
 
@@ -463,14 +470,15 @@ class CapacityExceeded(RuntimeError):
         self.pairs, self.pair_capacity, self.depth_bits, self.planned_depth_bits = pairs, pair_capacity, depth_bits, planned_depth_bits
 
 
-def probe_view_sizes(params, cluster_origin, cluster_extend, cams, sh_degree, hw, tile):
+def probe_view_sizes(params, cluster_origin, cluster_extend, cams, sh_degree, hw, tile, antialiased=False):
     """One synchronising forward per camera (the cold path) -> (max pairs, max depth-key bits): the first-epoch sizing step of
-    the reference's feedback protocol, used to dimension a ViewWorkspace."""
+    the reference's feedback protocol, used to dimension a ViewWorkspace.  antialiased: size for that mode (it has fewer pairs)."""
     max_pairs, max_bits = 0, 1
     p = {k: params[k].detach() for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")}
     with torch.no_grad():
         for cam in cams:
-            _, st, _ = render_view_forward(p, cluster_origin, cluster_extend, cam["frustumplane"], cam["view"], cam["proj"], sh_degree, hw, tile)
+            _, st, _ = render_view_forward(p, cluster_origin, cluster_extend, cam["frustumplane"], cam["view"], cam["proj"], sh_degree, hw, tile,
+                                           antialiased=antialiased)
             max_pairs = max(max_pairs, st.n_pairs)
             c = st.counters.cpu()
             kmin, kmax = ~int(c[2]) & 0xFFFFFFFF, int(c[3]) & 0xFFFFFFFF

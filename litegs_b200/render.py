@@ -69,7 +69,10 @@ def render(view_matrix, proj_matrix, xyz, scale, rot, color, opacity,
            valid_length, feedback_binning_allocate_size, idx_tensor,
            actived_sh_degree: int, output_shape, pp):
     """Projection -> binning -> rasterisation; returns (img, transmittance, depth, normal, primitive_visible)
-    as render/__init__.py:50-94."""
+    as render/__init__.py:50-94.  The antialiased mode exists on the fused path only (render_view, render_views)."""
+    if getattr(pp, "antialiased", False):
+        raise RuntimeError("pp.antialiased is set, but the op-by-op render() has no antialiased mode and would draw every splat "
+                           "without its opacity compensation; render through render_view or render_views instead")
     nvtx.range_push("Proj")
     view_pos, ndc_pos = wrapper.MVPTransform.apply(xyz, view_matrix, proj_matrix, valid_length)
     transform_matrix = wrapper.CreateTransformMatrix.call_fused(scale, rot, valid_length)
@@ -130,13 +133,14 @@ def _feed_statistics(state, stats, packed_grad, tile):
 class _RenderViewFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, xyz, scale, rot, sh_0, sh_rest, opacity, cluster_origin, cluster_extend, frustumplane,
-                view_matrix, proj_matrix, sh_degree, H, W, th, tw, sparse_grad, enable_transmitance, accumulate_into):
+                view_matrix, proj_matrix, sh_degree, H, W, th, tw, sparse_grad, enable_transmitance, accumulate_into, antialiased):
         params = dict(xyz=xyz, scale=scale, rot=rot, sh_0=sh_0, sh_rest=sh_rest, opacity=opacity)
         stat = bool(StatisticsHelperInst.bStart)
         ctx.set_materialize_grads(False)       # an unused transmittance output must not cost a zero-filled gradient image
         # the kernel writes clamp(c,0,1) directly (render/__init__.py:87 does it as a separate pass) ...
         img, state, stats = pipeline.render_view_forward(params, cluster_origin, cluster_extend, frustumplane, view_matrix,
-                                                         proj_matrix, sh_degree, (H, W), (th, tw), enable_statistic=stat, clamp_zero=True)
+                                                         proj_matrix, sh_degree, (H, W), (th, tw), enable_statistic=stat, clamp_zero=True,
+                                                         antialiased=antialiased)
         ctx.state = state
         ctx.stats = stats
         ctx.stat = stat
@@ -170,7 +174,7 @@ class _RenderViewFn(torch.autograd.Function):
             g_proj = cam[1].reshape(state.proj.shape) if ctx.needs_input_grad[10] else None
         if grads is None:          # gradients went straight into the caller's dense buffers
             ctx.state = None
-            return (None,) * 9 + (g_view, g_proj) + (None,) * 8
+            return (None,) * 9 + (g_view, g_proj) + (None,) * 9
         C, S = xyz.shape[-2:]
         ids = state.chunk_ids[: state.n_chunks_visible]
         out = []
@@ -178,7 +182,7 @@ class _RenderViewFn(torch.autograd.Function):
             ct = CompactedTensor((*g.shape[:-2], C, S), ids, g)
             out.append(ct if ctx.sparse else ct.to_dense())
         ctx.state = None
-        return (*out, None, None, None, g_view, g_proj, None, None, None, None, None, None, None, None)
+        return (*out, None, None, None, g_view, g_proj, None, None, None, None, None, None, None, None, None)
 
 
 def render_view(cluster_origin, cluster_extend, frustumplane, view_matrix, proj_matrix,
@@ -190,14 +194,14 @@ def render_view(cluster_origin, cluster_extend, frustumplane, view_matrix, proj_
     None, depth=None, normal=None, last_contributor [1,1,Hp,Wp]).  Gradients reach the six parameter tensors as CompactedTensor (pp.sparse_grad) or dense
     tensors -- or, with ``accumulate_into`` (dict of dense gradient tensors, e.g. ``GradAccumulator.grads()``), are
     ADDED into those buffers by the backward kernel itself and ``param.grad`` stays untouched (multi-view batches,
-    data-parallel training)."""
+    data-parallel training).  ``pp.antialiased`` (absent = False) selects the antialiased mode (DESIGN.md section 1)."""
     if not pp.cluster_size:
         raise RuntimeError("render_view needs the clustered layout (cluster_size > 0); use render_preprocess + render otherwise")
     H, W = int(output_shape[0]), int(output_shape[1])
     th, tw = int(pp.tile_size[0]), int(pp.tile_size[1])
     img, T, last = _RenderViewFn.apply(xyz, scale, rot, sh_0, sh_rest, opacity, cluster_origin, cluster_extend, frustumplane,
                                        view_matrix, proj_matrix, int(actived_sh_degree), H, W, th, tw, pp.sparse_grad,
-                                       pp.enable_transmitance, accumulate_into)
+                                       pp.enable_transmitance, accumulate_into, bool(getattr(pp, "antialiased", False)))
     img = img[..., :H, :W]          # already clamped to [0,1] by the kernel
     trans = T[..., :H, :W] if pp.enable_transmitance else None
     return img, trans, None, None, last
@@ -248,6 +252,7 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
     losses = []
     H, W = int(output_shape[0]), int(output_shape[1])
     th, tw = int(pp.tile_size[0]), int(pp.tile_size[1])
+    aa = bool(getattr(pp, "antialiased", False))
     direct = loss_and_grad_fn is not None or _DIRECT_VIEWS
     if direct:
         params = dict(xyz=xyz.detach(), scale=scale.detach(), rot=rot.detach(), sh_0=sh_0.detach(), sh_rest=sh_rest.detach(),
@@ -258,7 +263,7 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
         cam = camera_fn(i)
         img_p, state, stats = pipeline.render_view_forward(params, cluster_origin, cluster_extend, cam["frustumplane"], cam["view"],
                                                            cam["proj"], int(actived_sh_degree), (H, W), (th, tw), enable_statistic=stat,
-                                                           clamp_zero=True)
+                                                           clamp_zero=True, antialiased=aa)
         if loss_and_grad_fn is not None:
             loss, d_img = loss_and_grad_fn(i, img_p[..., :H, :W])
         else:                          # autograd only through the user's loss, never through the render kernels
@@ -302,14 +307,14 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
     # path and measures the capacities (the reference's cold first epoch); statistics runs keep the synchronising path.
     slots = None
     if direct and pipeline.SYNC_FREE and not stat:
-        slots = _view_slots(params, (H, W), (th, tw), max(1, n_streams))
+        slots = _view_slots(params, (H, W), (th, tw), max(1, n_streams), aa)
         if slots.big:
             slots = None
     probe = {"pairs": 0, "bits": 1} if (slots is not None and slots.ws is None) else None
 
     def one_ws(i, wait_ev, ws):
         cam = camera_fn(i)
-        img_p = ws.forward(params, cluster_origin, cluster_extend, cam, int(actived_sh_degree), clamp_zero=True)
+        img_p = ws.forward(params, cluster_origin, cluster_extend, cam, int(actived_sh_degree), clamp_zero=True, antialiased=aa)
         if loss_and_grad_fn is not None:
             loss, d_img = loss_and_grad_fn(i, img_p[..., :H, :W])
         else:
@@ -321,7 +326,7 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
                 (d_img,) = torch.autograd.grad(loss, leaf)
         if wait_ev is not None:
             torch.cuda.current_stream(dev).wait_event(wait_ev)
-        ws.backward(params, d_img, int(actived_sh_degree), accumulate_into, use_clamp=True, camera_grad=slot(i))
+        ws.backward(params, d_img, int(actived_sh_degree), accumulate_into, use_clamp=True, camera_grad=slot(i), antialiased=aa)
         losses.append(loss.detach())
 
     def one_probe(i, wait_ev):
@@ -376,7 +381,8 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
 
 class _ViewSlots:
     """The per-configuration state of render_views' GPU-driven path: capacities measured by the first (synchronising) batch and
-    one ViewWorkspace per stream slot, created from them."""
+    one ViewWorkspace per stream slot, created from them.  The antialiased mode is part of the configuration: it has fewer
+    pairs, so capacities measured with it on would overflow with it off."""
 
     def __init__(self, params, hw, tile):
         self.params_like, self.hw, self.tile = params, hw, tile
@@ -415,9 +421,9 @@ class _ViewSlots:
 _slot_cache: dict = {}
 
 
-def _view_slots(params, hw, tile, n_slots):
+def _view_slots(params, hw, tile, n_slots, antialiased=False):
     xyz = params["xyz"]
-    key = (xyz.device, tuple(xyz.shape[-2:]), hw, tile, params["sh_rest"].shape[0])
+    key = (xyz.device, tuple(xyz.shape[-2:]), hw, tile, params["sh_rest"].shape[0], bool(antialiased))
     ent = _slot_cache.get(key)
     if ent is None:
         ent = _slot_cache[key] = _ViewSlots(params, hw, tile)
