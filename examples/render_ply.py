@@ -2,6 +2,7 @@
 
     python examples/render_ply.py --ply point_cloud.ply --out /tmp/renders --views 8 [--colmap /path/to/colmap]
     python examples/render_ply.py --make /tmp/demo.ply --out /tmp/renders        # writes a synthetic cloud first
+    python examples/render_ply.py --ply mip_splatting.ply --filter-3d --antialiased    # a Mip-Splatting checkpoint
 
 Cameras: the poses of a COLMAP model when --colmap is given, else the Fibonacci lattice of scene.make_camera.  Forward only
 (the reference's example_metrics.py path): project -> bin -> sort -> composite, no gradients kept.
@@ -31,6 +32,8 @@ def main():
     ap.add_argument("--sh-degree", type=int, default=3)
     ap.add_argument("--antialiased", action="store_true",
                     help="opacity compensation of the 2D filter (for models trained in that mode, or renders at another resolution)")
+    ap.add_argument("--filter-3d", action="store_true",
+                    help="apply the file's filter_3D property (Mip-Splatting's 3D smoothing filter); the file must have it")
     a = ap.parse_args()
     path = a.ply
     if a.make:
@@ -43,6 +46,12 @@ def main():
     g = ply.params_from_ply(path, a.sh_degree)
     P = {k: torch.from_numpy(g[k]).to(dev) for k in PARAM_ORDER}
     A = [torch.from_numpy(g[k]).to(dev) for k in ("cluster_origin", "cluster_extend")]
+    filt = None
+    if a.filter_3d:
+        if "filter_3D" not in g:
+            ap.error(f"--filter-3d: {path} has no filter_3D property")
+        filt = torch.from_numpy(g["filter_3D"]).to(dev)
+        A = list(scene.cluster_aabb_torch(P["xyz"], P["scale"], P["rot"], filter_3d=filt))       # boxes of the widened splats
     cams = []
     if a.colmap:
         cs, ims, _ = colmap.read_model(a.colmap)
@@ -60,7 +69,7 @@ def main():
         for cam, hw, _ in cams:
             c = {k: torch.from_numpy(v).to(dev) for k, v in cam.items()}
             img, _, _ = pipeline.render_view_forward(P, A[0], A[1], c["frustumplane"], c["view"], c["proj"], a.sh_degree, hw, (8, 16),
-                                                     clamp_zero=True, antialiased=a.antialiased)
+                                                     clamp_zero=True, antialiased=a.antialiased, filter_3d=filt)
             imgs.append(img[0, :, : hw[0], : hw[1]])
     torch.cuda.synchronize()
     dt = time.perf_counter() - t0

@@ -84,14 +84,14 @@ def load_dataset(root, image_dir="images", dev=None):
     return frames, np.stack([p.xyz for p in P]), np.stack([p.rgb for p in P])
 
 
-def train(root, iters=300, views_per_step=8, log=print, refine_poses=False, antialiased=False):
+def train(root, iters=300, views_per_step=8, log=print, refine_poses=False, antialiased=False, filter_3d=False):
     from litegs_b200 import fused
     if refine_poses and int(os.environ.get("WORLD_SIZE", "1")) > 1:
         raise ValueError("--refine-poses runs on one GPU: multi-GPU pose refinement is not supported")
     keep = fused.CONFIG["true_sigmoid_grad"]
     fused.CONFIG["true_sigmoid_grad"] = True               # our own loops train with the true sigmoid derivative (SURVEY Q15)
     try:
-        return _train(root, iters, views_per_step, log, refine_poses, antialiased)
+        return _train(root, iters, views_per_step, log, refine_poses, antialiased, filter_3d)
     finally:
         fused.CONFIG["true_sigmoid_grad"] = keep
 
@@ -128,7 +128,7 @@ class _Poses:
         self.opt.step()
 
 
-def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=False):
+def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=False, filter_3d=False):
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", 0)))
     torch.cuda.set_device(dev)
     frames, xyz, rgb = load_dataset(root, dev=dev)
@@ -143,18 +143,26 @@ def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=Fal
     extent = float(np.linalg.norm(xyz.max(0) - xyz.min(0)) * 0.5)
     opt, sched = optimizer.get_optimizer(P, spatial_lr_scale=extent)
     hist = []
+    # Mip-Splatting's 3D smoothing filter: recomputed from ALL training cameras (every rank computes the same values, no
+    # collective) into the same tensor, so the captured per-view graphs keep reading it
+    filt = torch.empty_like(P["opacity"]) if filter_3d else None
+    hw_all = torch.tensor([[H, W]] * len(frames), dtype=torch.int32, device=dev) if filter_3d else None
     t0 = time.perf_counter()
     for it in range(iters):
         idx = [(it * views_per_step + j) % len(frames) for j in range(views_per_step)]
+        if filter_3d and it % 100 == 0:
+            all_cams = poses.cameras(list(range(len(frames)))) if poses else [f[0] for f in frames]
+            scene.filter_3d_device(P["xyz"], torch.cat([c["view"] for c in all_cams]), torch.cat([c["proj"] for c in all_cams]), hw_all,
+                                   out=filt)
         # positions and shapes move, so the chunk AABBs used for culling are refreshed from the parameters now and then
         if it % 50 == 0:
-            A = list(scene.cluster_aabb_torch(P["xyz"], P["scale"], P["rot"]))
+            A = list(scene.cluster_aabb_torch(P["xyz"], P["scale"], P["rot"], filter_3d=filt))
         cams = poses.cameras(idx) if poses else [frames[j][0] for j in idx]
         losses = render.render_views(views_per_step, lambda i: cams[i], None, A[0], A[1], P["xyz"], P["scale"], P["rot"],
                                      P["sh_0"], P["sh_rest"], P["opacity"], 3, (H, W), pp, acc.grads(),
                                      loss_and_grad_fn=lambda i, img: ssim.l1_ssim_loss_and_grad(img.contiguous(), frames[idx[i]][1], 0.2,
                                                                                               upstream=1.0 / views_per_step),
-                                     camera_grads=cgrads)
+                                     camera_grads=cgrads, filter_3d=filt)
         opt.step(acc)
         if poses:
             poses.step(idx, cgrads)
@@ -169,7 +177,7 @@ def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=Fal
         for j, (cam, gt, _) in enumerate(frames[:8]):
             cam = poses.cameras([j])[0] if poses else cam
             img = render.render_view(A[0], A[1], cam["frustumplane"], cam["view"], cam["proj"], P["xyz"], P["scale"], P["rot"], P["sh_0"],
-                                     P["sh_rest"], P["opacity"], 3, (H, W), pp)[0]
+                                     P["sh_rest"], P["opacity"], 3, (H, W), pp, filter_3d=filt)[0]
             mse.append(float(((img - gt) ** 2).mean()))
     psnr = -10.0 * np.log10(np.mean(mse))
     log(f"{iters} iterations x {views_per_step} views in {dt:.1f} s ({iters * views_per_step / dt:.0f} views/s incl. loss + optimizer); "
@@ -187,6 +195,8 @@ if __name__ == "__main__":
     ap.add_argument("--iters", type=int, default=300)
     ap.add_argument("--refine-poses", action="store_true", help="also optimise the camera extrinsics (one GPU)")
     ap.add_argument("--antialiased", action="store_true", help="train (and evaluate) in the antialiased mode")
+    ap.add_argument("--filter-3d", action="store_true",
+                    help="Mip-Splatting's 3D smoothing filter, from all training cameras at iteration 0 and every 100 iterations")
     ap.add_argument("--pose-noise", type=float, nargs=2, default=None, metavar=("DEG", "FRAC"),
                     help="with --make: perturb the written poses by DEG degrees and FRAC of the camera distance")
     a = ap.parse_args()
@@ -195,5 +205,5 @@ if __name__ == "__main__":
         root = make_dataset(a.make, pose_noise=a.pose_noise)
     if root is None:
         ap.error("give --data or --make")
-    h, _ = train(root, a.iters, refine_poses=a.refine_poses, antialiased=a.antialiased)
+    h, _ = train(root, a.iters, refine_poses=a.refine_poses, antialiased=a.antialiased, filter_3d=a.filter_3d)
     assert h[-1] < h[0]

@@ -257,12 +257,17 @@ int lgs_set_err_square_mode(int mode);
  * in the order, they emit nothing).
  * antialiased != 0: antialiased mode, ours (the reference has none).  The record's opacity is sigmoid(opacity) * rho with
  * rho = sqrt(det(M^T M) / det(M^T M + 0.3 I)), the opacity compensation of the 2D low-pass filter (DESIGN.md section 1);
- * the visibility test, the tile walk and the rasteriser all see that opacity.  0 = the reference's behaviour. */
+ * the visibility test, the tile walk and the rasteriser all see that opacity.  0 = the reference's behaviour.
+ * filter_3d f32[C*S] (clustered like opacity) or NULL: Mip-Splatting's 3D smoothing filter, ours (the reference has none).  Each
+ * Gaussian's activated scale becomes s' = sqrt(s^2 + f^2) in the whole chain (S.R, M, the 2D covariance, the tile walk) and its
+ * opacity sigmoid(opacity) * rho3 with rho3 = sqrt(prod_k s_k^2 / (s_k^2 + f^2)), before the antialiased factor
+ * (DESIGN.md section 1, "3D smoothing filter").  NULL = no filter, the same kernels as before. */
 int lgs_project_forward(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
                         const float* view_matrix, const float* proj_matrix, const float* position, const float* scale,
                         const float* rotation, const float* sh_base, const float* sh_rest, const float* opacity, int C,
                         int S, int A, int img_h, int img_w, int tile_h, int tile_w, float* packed_params,
-                        unsigned* depth_key, unsigned* iota, int* tile_count, int* totals, int antialiased, void* stream);
+                        unsigned* depth_key, unsigned* iota, int* tile_count, int* totals, const float* filter_3d, int antialiased,
+                        void* stream);
 
 /* duplicate_with_keys (GR/binning.cu:33-110) reading the packed record: offset = inclusive scan of the depth-ordered
  * counts, order = depth-sorted slot ids; keys/vals i32[cap] must be zero-initialised by the caller. */
@@ -284,14 +289,16 @@ int lgs_emit_pairs_u16(const float* packed_params, const int* offset, const unsi
  * The reference's operators return no view-matrix gradient (wrapper.py:285,407,845); this one is new.  Summed in a fixed
  * order (bit-reproducible), no host synchronisation; needs S % 32 == 0.
  * antialiased: must equal the value the forward of this view was given (ours, no reference counterpart).  The record
- * gradient is then taken at the compensated opacity and the gradient of rho flows into scale, rotation and the camera. */
+ * gradient is then taken at the compensated opacity and the gradient of rho flows into scale, rotation and the camera.
+ * filter_3d: the tensor the forward of this view was given, or NULL.  The filter is held constant: the raw scale gradient
+ * gains the rho3 term, and no gradient flows into the filter, the positions or the cameras through it. */
 int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
                          const float* view_matrix, const float* proj_matrix, const float* position, const float* scale,
                          const float* rotation, const float* opacity, int C, int S, int A, int rest_dim, int img_h,
                          int img_w, int true_sigmoid_grad, const float* packed_grad, const float* grad_inv_scaler,
                          int zero_outputs, float* g_position, float* g_scale, float* g_rotation, float* g_sh_base,
-                         float* g_sh_rest, float* g_opacity, float* touched, float* cam_partials, float* d_cam, int antialiased,
-                         void* stream);
+                         float* g_sh_rest, float* g_opacity, float* touched, float* cam_partials, float* d_cam,
+                         const float* filter_3d, int antialiased, void* stream);
 
 /* create_viewproj_forward, GR/compact.cu:17-141: view_params f32[V,7] (qw qx qy qz tx ty tz), recp_tan_half_fov_x f32[1] ->
  * view, proj, viewproj f32[V,4,4] (row-vector convention) and frustumplane f32[V,6,4].  One thread per view. */
@@ -350,6 +357,13 @@ int lgs_permute_rows(const float* src, const long long* idx, int R, int N, float
 /* get_cluster_AABB (litegs/scene/cluster.py:29-46) from the RAW clustered parameters xyz/scale f32[3,C,S], rot f32[4,C,S]
  * -> origin, extend f32[3,C]. */
 int lgs_cluster_aabb(const float* xyz, const float* scale, const float* rot, int C, int S, float* origin, float* extend, void* stream);
+/* Mip-Splatting's 3D smoothing filter (compute_3D_filter), ours: position f32[3,C,S] (every slot, the tail padding included),
+ * V cameras view / proj f32[V,4,4] (row-vector convention) and hw i32[V,2] (height, width) -> filter_3d f32[C*S].  Per Gaussian,
+ * f = (dist / focal) * sqrt(0.2), dist = the smallest view depth over the cameras that see it (depth > 0.2, projection within
+ * 15 % of the image border), focal = the largest P[0][0] W / 2.  Unseen Gaussians get the largest seen f (0 when none is seen).
+ * Exact fp32 operation order in DESIGN.md section 1; bit-reproducible, no host synchronisation, no gradient. */
+int lgs_filter_3d(const float* position, int C, int S, const float* view, const float* proj, const int* hw, int V,
+                  float* filter_3d, void* stream);
 
 /* ---- fused SSIM / L1 + SSIM loss (next row, SURVEY 8f rank 2; what trainer.py:145 calls) ------------------ */
 

@@ -65,10 +65,10 @@ SIGNATURES = {
     "lgs_set_forward_pairs": [_I],
     "lgs_set_err_square_mode": [_I],
     "lgs_set_deterministic": [_I],
-    "lgs_project_forward": [_I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P],
+    "lgs_project_forward": [_I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _I, _P],
     "lgs_emit_pairs": [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P],
     "lgs_project_backward": [_I, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _I,
-                             _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P],
+                             _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P],
     "lgs_create_viewproj_forward": [_P, _P, _I, _I, _I, _F, _F, _P, _P, _P, _P, _P],
     "lgs_create_viewproj_backward": [_P, _P, _P, _P, _P, _I, _I, _I, _F, _F, _P, _P, _P],
     "lgs_adam_update_chunk": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _D, _D, _D, _D, _P],
@@ -79,6 +79,7 @@ SIGNATURES = {
     "lgs_morton_codes": [_P, _P, _P, _I, _I, _P, _P],
     "lgs_permute_rows": [_P, _P, _I, _I, _P, _P],
     "lgs_cluster_aabb": [_P, _P, _P, _I, _I, _P, _P, _P],
+    "lgs_filter_3d": [_P, _I, _I, _P, _P, _P, _I, _P, _P],
     "lgs_adam_step_dense": [_P, _P, _P, _P, _P, _P, _P, _I, _I, _D, _D, _D, _I, _P],
     "lgs_ssim_num_block_sums": [_I, _I, _I, _I, ctypes.POINTER(_I)],
     "lgs_ssim_forward": [_P, _P, _I, _I, _I, _I, _F, _F, _I, _F, _P, _P, _P, _P, _P, _P],

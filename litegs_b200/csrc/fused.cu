@@ -50,17 +50,49 @@ __device__ __forceinline__ void fused_J(const float* __restrict__ P, const float
     J[0] = fx * rz; J[1] = 0.f; J[2] = 0.f; J[3] = fy * rz; J[4] = -fx * tx * rz2; J[5] = -fy * ty * rz2;
 }
 
+// Mip-Splatting's 3D smoothing filter (DESIGN.md section 1, "3D smoothing filter"): s'_k = sqrt(s_k^2 + f^2) and
+// rho3 = sqrt((r_0 r_1) r_2) with r_k = s_k^2 / (s_k^2 + f^2), every step one correctly rounded op in this order, so that
+// tests/filter3d_oracle.py reproduces it bit for bit.  With f = 0, s' = s and rho3 = 1 exactly (s^2 normal).
+struct Filter3D {
+    float s[3];                     // the unfiltered activated scale
+    float qf[3];                    // s_k^2 + f^2
+    float f2, rho3;
+};
+
+__device__ __forceinline__ void filter_3d_factor(float f, const float* s, Filter3D& F)
+{
+    F.f2 = __fmul_rn(f, f);
+    float r[3];
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        const float q = __fmul_rn(s[k], s[k]);
+        F.s[k] = s[k];
+        F.qf[k] = __fadd_rn(q, F.f2);
+        r[k] = __fdiv_rn(q, F.qf[k]);
+    }
+    F.rho3 = __fsqrt_rn(__fmul_rn(__fmul_rn(r[0], r[1]), r[2]));
+}
+
 // The forward chain shared by both directions.  Vm/P are the view / projection matrices (row-vector).
+// F3D: the 3D filter f3d is applied: t.s holds the filtered scale s' and t.o the filtered opacity sigma(o_raw) * rho3; F keeps
+// the unfiltered scale and the factors the backward needs.
+template <bool F3D = false>
 __device__ __forceinline__ void project_chain(const float* __restrict__ Vm, const float* __restrict__ P, const float* p,
                                               const float* s_raw, const float* q_raw, float o_raw, int H, int W,
-                                              ProjIntermediates& t)
+                                              ProjIntermediates& t, float f3d = 0.0f, Filter3D* F = nullptr)
 {
 #pragma unroll
     for (int k = 0; k < 3; k++) t.s[k] = expf(s_raw[k]);
+    if constexpr (F3D) {
+        filter_3d_factor(f3d, t.s, *F);
+#pragma unroll
+        for (int k = 0; k < 3; k++) t.s[k] = __fsqrt_rn(F->qf[k]);
+    }
     t.rn = 1.0f / sqrtf(q_raw[0] * q_raw[0] + q_raw[1] * q_raw[1] + q_raw[2] * q_raw[2] + q_raw[3] * q_raw[3] + 1e-12f);
 #pragma unroll
     for (int k = 0; k < 4; k++) t.qn[k] = q_raw[k] * t.rn;
     t.o = 1.0f / (1.0f + expf(-o_raw));
+    if constexpr (F3D) t.o = __fmul_rn(t.o, F->rho3);
     float cc[3];
     lgs_camera_center(Vm, cc);
     float d0 = p[0] - cc[0], d1 = p[1] - cc[1], d2 = p[2] - cc[2];
@@ -132,13 +164,15 @@ __device__ __forceinline__ void antialias_factor(const float* M, AAFactor& f)
 
 // grid = allocated chunks (all M: chunks >= *visible_num write an invisible record), block = chunk size
 // AA: the record's opacity is sigma(o_raw) * rho (antialiased mode); everything downstream reads it from the record.
-template <int DEG, int TH, int TW, bool AA>
+// F3D: the 3D smoothing filter filter_3d[src] widens the scale and scales the opacity by rho3 before AA sees either.
+template <int DEG, int TH, int TW, bool AA, bool F3D>
 __global__ void project_forward_kernel(
     const int64_t* __restrict__ chunk_ids, const int* __restrict__ visible_num, const float* __restrict__ view,
     const float* __restrict__ proj, const float* __restrict__ pos, const float* __restrict__ scale,
     const float* __restrict__ rot, const float* __restrict__ sh0, const float* __restrict__ shr,
     const float* __restrict__ opac, int C, int S, int H, int W, int gx, int gy, SplatRec* __restrict__ recs,
-    unsigned* __restrict__ depth_key, unsigned* __restrict__ iota, int* __restrict__ tile_count, int* __restrict__ totals)
+    unsigned* __restrict__ depth_key, unsigned* __restrict__ iota, int* __restrict__ tile_count, int* __restrict__ totals,
+    const float* __restrict__ filter_3d)
 {
     const int a = blockIdx.x, s = threadIdx.x;
     const size_t dst = (size_t)a * S + s;
@@ -153,7 +187,12 @@ __global__ void project_forward_kernel(
         float sr_[3] = { scale[src], scale[CS + src], scale[2 * CS + src] };
         float q[4] = { rot[src], rot[CS + src], rot[2 * CS + src], rot[3 * CS + src] };
         ProjIntermediates t;
-        project_chain(view, proj, p, sr_, q, opac[src], H, W, t);
+        if constexpr (F3D) {
+            Filter3D F;
+            project_chain<true>(view, proj, p, sr_, q, opac[src], H, W, t, filter_3d[src], &F);
+        } else {
+            project_chain(view, proj, p, sr_, q, opac[src], H, W, t);
+        }
         if constexpr (AA) {
             AAFactor f;
             antialias_factor(t.M, f);
@@ -217,7 +256,7 @@ extern "C" int lgs_project_forward(int sh_degree, const int64_t* visible_chunk_i
                                    const float* scale, const float* rotation, const float* sh_base, const float* sh_rest,
                                    const float* opacity, int C, int S, int A, int img_h, int img_w, int tile_h, int tile_w,
                                    float* packed_params, unsigned* depth_key, unsigned* iota, int* tile_count, int* totals,
-                                   int antialiased, void* stream)
+                                   const float* filter_3d, int antialiased, void* stream)
 {
     LGS_REQUIRE(sh_degree >= 0 && sh_degree <= 3, "project_forward: sh_degree %d not in 0..3", sh_degree);
     LGS_REQUIRE(lgs_tile_ok(tile_h, tile_w), "project_forward: tile %dx%d not one of 8x16, 12x16, 16x16, 8x8", tile_h, tile_w);
@@ -226,16 +265,17 @@ extern "C" int lgs_project_forward(int sh_degree, const int64_t* visible_chunk_i
     LGS_CUDA(cudaMemsetAsync(totals, 0, 3 * sizeof(int), st));
     if (A == 0) return LGS_OK;
     int gx = (img_w + tile_w - 1) / tile_w, gy = (img_h + tile_h - 1) / tile_h;
-#define PF(D, AA) project_forward_kernel<D, TH, TW, AA><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num, view_matrix, proj_matrix, \
-        position, scale, rotation, sh_base, sh_rest, opacity, C, S, img_h, img_w, gx, gy, (SplatRec*)packed_params, depth_key, iota,    \
-        tile_count, totals)
-    if (antialiased) {
-        LGS_DISPATCH_TILE(tile_h, tile_w,
-            switch (sh_degree) { case 0: PF(0, true); break; case 1: PF(1, true); break; case 2: PF(2, true); break; default: PF(3, true); })
+#define PF(D, AA, F3) project_forward_kernel<D, TH, TW, AA, F3><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num, view_matrix,  \
+        proj_matrix, position, scale, rotation, sh_base, sh_rest, opacity, C, S, img_h, img_w, gx, gy, (SplatRec*)packed_params,     \
+        depth_key, iota, tile_count, totals, filter_3d)
+#define PF_DEG(AA, F3) LGS_DISPATCH_TILE(tile_h, tile_w,                                                                            \
+        switch (sh_degree) { case 0: PF(0, AA, F3); break; case 1: PF(1, AA, F3); break; case 2: PF(2, AA, F3); break; default: PF(3, AA, F3); })
+    if (filter_3d != nullptr) {
+        if (antialiased) { PF_DEG(true, true) } else { PF_DEG(false, true) }
     } else {
-        LGS_DISPATCH_TILE(tile_h, tile_w,
-            switch (sh_degree) { case 0: PF(0, false); break; case 1: PF(1, false); break; case 2: PF(2, false); break; default: PF(3, false); })
+        if (antialiased) { PF_DEG(true, false) } else { PF_DEG(false, false) }
     }
+#undef PF_DEG
 #undef PF
     LGS_CHECK_LAUNCH("project_forward_kernel");
     return LGS_OK;
@@ -425,14 +465,17 @@ __device__ __forceinline__ float warp_sum32_transposed(float* v)
 // chunk (chunks at or past the visible count write zeros); camera_grad_sum_kernel folds the rows.
 // AA: antialiased mode.  The record gradient is taken at o_eff = sigma(o_raw) * rho; d o = d o_eff * rho, and the rho path
 // adds d det(M^T M) and d det(M^T M + 0.3 I) to d cov2d before dM = 2 M G, so ds, dq and the camera path all see it.
-template <int DEG, bool CAM, bool AA>
+// F3D: 3D smoothing filter.  With g = d o3 (after the AA step), d sigma = g rho3 and
+// d s_raw_k = s_k (ds'_k (s_k / s'_k)) + (g o3) (f^2 / qf_k); f is held constant.
+template <int DEG, bool CAM, bool AA, bool F3D>
 __global__ void project_backward_kernel(
     const int64_t* __restrict__ chunk_ids, const int* __restrict__ visible_num, const float* __restrict__ view,
     const float* __restrict__ proj, const float* __restrict__ pos, const float* __restrict__ scale,
     const float* __restrict__ rot, const float* __restrict__ opac, int C, int S, int A, int rest_dim, int H, int W,
     int true_sigmoid, int accumulate, const float* __restrict__ grad /*[A*S,12]*/, const float* __restrict__ inv_scaler,
     float* __restrict__ g_pos, float* __restrict__ g_scale, float* __restrict__ g_rot, float* __restrict__ g_sh0,
-    float* __restrict__ g_shr, float* __restrict__ g_opac, float* __restrict__ touched, float* __restrict__ cam_partials)
+    float* __restrict__ g_shr, float* __restrict__ g_opac, float* __restrict__ touched, float* __restrict__ cam_partials,
+    const float* __restrict__ filter_3d)
 {
     const int a = blockIdx.x, s = threadIdx.x;
     if (a >= visible_num[0]) {
@@ -465,7 +508,12 @@ __global__ void project_backward_kernel(
         float q[4] = { rot[src], rot[CS + src], rot[2 * CS + src], rot[3 * CS + src] };
         const float o_raw = opac[src];
         ProjIntermediates t;
-        project_chain(view, proj, p, sr_, q, o_raw, H, W, t);
+        Filter3D F;
+        if constexpr (F3D) {
+            project_chain<true>(view, proj, p, sr_, q, o_raw, H, W, t, filter_3d[src], &F);
+        } else {
+            project_chain(view, proj, p, sr_, q, o_raw, H, W, t);
+        }
         AAFactor f;
         float o_rec = t.o;                                  // the record's opacity
         if constexpr (AA) {
@@ -524,8 +572,17 @@ __global__ void project_backward_kernel(
         dq[2] = 2 * x * (dT[3] + dT[1]) + 2 * r_ * (dT[6] - dT[2]) + 2 * z * (dT[5] + dT[7]) - 4 * y * (dT[8] + dT[0]);
         dq[3] = 2 * r_ * (dT[1] - dT[3]) + 2 * x * (dT[6] + dT[2]) + 2 * y * (dT[5] + dT[7]) - 4 * z * (dT[4] + dT[0]);
         // activation chain (GR/compact.cu:925-952)
+        if constexpr (F3D) {
+            // ds is the gradient at s' (t.s); t.o is o3 and d_o is d o3
+            const float go3 = __fmul_rn(d_o, t.o);
 #pragma unroll
-        for (int k = 0; k < 3; k++) o_sc[k] = t.s[k] * ds[k];
+            for (int k = 0; k < 3; k++)
+                o_sc[k] = __fadd_rn(__fmul_rn(F.s[k], __fmul_rn(ds[k], __fdiv_rn(F.s[k], t.s[k]))), __fmul_rn(go3, __fdiv_rn(F.f2, F.qf[k])));
+            d_o = __fmul_rn(d_o, F.rho3);
+        } else {
+#pragma unroll
+            for (int k = 0; k < 3; k++) o_sc[k] = t.s[k] * ds[k];
+        }
         const float dot = dq[0] * t.qn[0] + dq[1] * t.qn[1] + dq[2] * t.qn[2] + dq[3] * t.qn[3];
 #pragma unroll
         for (int k = 0; k < 4; k++) o_q[k] = t.rn * (dq[k] - dot * t.qn[k]);
@@ -654,7 +711,7 @@ extern "C" int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_
                                     int rest_dim, int img_h, int img_w, int true_sigmoid_grad, const float* packed_grad,
                                     const float* grad_inv_scaler, int zero_outputs, float* g_position, float* g_scale,
                                     float* g_rotation, float* g_sh_base, float* g_sh_rest, float* g_opacity, float* touched,
-                                    float* cam_partials, float* d_cam, int antialiased, void* stream)
+                                    float* cam_partials, float* d_cam, const float* filter_3d, int antialiased, void* stream)
 {
     LGS_REQUIRE(sh_degree >= 0 && sh_degree <= 3, "project_backward: sh_degree %d not in 0..3", sh_degree);
     LGS_REQUIRE(rest_dim >= (sh_degree + 1) * (sh_degree + 1) - 1, "project_backward: sh_rest has %d rows, degree %d needs %d", rest_dim,
@@ -678,15 +735,18 @@ extern "C" int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_
         LGS_CUDA(cudaMemsetAsync(g_sh_rest, 0, sizeof(float) * (size_t)rest_dim * 3 * AS, st));
         LGS_CUDA(cudaMemsetAsync(g_opacity, 0, sizeof(float) * AS, st));
     }
-#define PB(D, K, AA) project_backward_kernel<D, K, AA><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num, view_matrix, proj_matrix, \
-        position, scale, rotation, opacity, C, S, A, rest_dim, img_h, img_w, true_sigmoid_grad, accumulate, packed_grad, grad_inv_scaler,  \
-        g_position, g_scale, g_rotation, g_sh_base, g_sh_rest, g_opacity, touched, cam_partials)
-#define PB_DEG(K, AA) switch (sh_degree) { case 0: PB(0, K, AA); break; case 1: PB(1, K, AA); break; case 2: PB(2, K, AA); break; default: PB(3, K, AA); }
-    if (antialiased) {
-        if (cam) { PB_DEG(true, true) } else { PB_DEG(false, true) }
+#define PB(D, K, AA, F3) project_backward_kernel<D, K, AA, F3><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num, view_matrix,    \
+        proj_matrix, position, scale, rotation, opacity, C, S, A, rest_dim, img_h, img_w, true_sigmoid_grad, accumulate, packed_grad,  \
+        grad_inv_scaler, g_position, g_scale, g_rotation, g_sh_base, g_sh_rest, g_opacity, touched, cam_partials, filter_3d)
+#define PB_DEG(K, AA, F3) switch (sh_degree) { case 0: PB(0, K, AA, F3); break; case 1: PB(1, K, AA, F3); break;                      \
+                                               case 2: PB(2, K, AA, F3); break; default: PB(3, K, AA, F3); }
+#define PB_CAM(AA, F3) if (cam) { PB_DEG(true, AA, F3) } else { PB_DEG(false, AA, F3) }
+    if (filter_3d != nullptr) {
+        if (antialiased) { PB_CAM(true, true) } else { PB_CAM(false, true) }
     } else {
-        if (cam) { PB_DEG(true, false) } else { PB_DEG(false, false) }
+        if (antialiased) { PB_CAM(true, false) } else { PB_CAM(false, false) }
     }
+#undef PB_CAM
 #undef PB_DEG
 #undef PB
     LGS_CHECK_LAUNCH("project_backward_kernel");

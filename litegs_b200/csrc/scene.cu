@@ -103,6 +103,95 @@ __global__ void cluster_aabb_kernel(const float* __restrict__ xyz, const float* 
     }
 }
 
+// Mip-Splatting's 3D smoothing filter (DESIGN.md section 1, "3D smoothing filter"), computed from the training cameras.
+// Per Gaussian p and camera v, every op single-rounded and without contraction:
+//   x/y/z_v = ((p0 V[0][c] + p1 V[1][c]) + p2 V[2][c]) + V[3][c]     (c = 0, 1, 2)
+//   fx = (P[0][0] W) 0.5, fy = (P[1][1] H) 0.5, zc = max(z_v, 0.001), u = (x_v / zc) fx + W 0.5, w = (y_v / zc) fy + H 0.5
+//   valid: z_v > 0.2 and (-0.15 W) <= u <= (1.15 W) and (-0.15 H) <= w <= (1.15 H)
+//   dist = min(100000, z_v over the valid cameras), focal = max of fx over all cameras, f = (dist / focal) 0.4472136
+// A Gaussian no camera sees gets the largest f of the seen ones (division and product by positive constants are monotone
+// under rounding, so that is the f of the largest seen dist), or 0 when no Gaussian is seen.
+constexpr int LGS_F3D_THREADS = 256;
+constexpr int LGS_F3D_CAM_FLOATS = 20;     // V[0..3][0..2], fx, fy, W/2, H/2, the four screen bounds
+
+__global__ void __launch_bounds__(LGS_F3D_THREADS) filter_3d_kernel(const float* __restrict__ xyz, int N, const float* __restrict__ view,
+                                                                    const float* __restrict__ proj, const int* __restrict__ hw, int V,
+                                                                    float* __restrict__ out, unsigned* __restrict__ max_bits)
+{
+    __shared__ float s_cam[LGS_F3D_THREADS][LGS_F3D_CAM_FLOATS + 1];
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const bool live = i < N;
+    const float p0 = live ? xyz[i] : 0.f, p1 = live ? xyz[(size_t)N + i] : 0.f, p2 = live ? xyz[2 * (size_t)N + i] : 0.f;
+    float dist = 100000.0f, focal = 0.0f;
+    bool seen = false;
+    for (int base = 0; base < V; base += LGS_F3D_THREADS) {
+        const int v = base + threadIdx.x;
+        if (v < V) {
+            const float* Vm = view + (size_t)v * 16;
+            const float H = (float)hw[2 * v], W = (float)hw[2 * v + 1];
+            float* c = s_cam[threadIdx.x];
+#pragma unroll
+            for (int r = 0; r < 4; r++)
+#pragma unroll
+                for (int k = 0; k < 3; k++) c[r * 3 + k] = Vm[r * 4 + k];
+            c[12] = __fmul_rn(__fmul_rn(proj[(size_t)v * 16], W), 0.5f);
+            c[13] = __fmul_rn(__fmul_rn(proj[(size_t)v * 16 + 5], H), 0.5f);
+            c[14] = __fmul_rn(W, 0.5f); c[15] = __fmul_rn(H, 0.5f);
+            c[16] = __fmul_rn(-0.15f, W); c[17] = __fmul_rn(1.15f, W);
+            c[18] = __fmul_rn(-0.15f, H); c[19] = __fmul_rn(1.15f, H);
+        }
+        __syncthreads();
+        const int nb = min(LGS_F3D_THREADS, V - base);
+        for (int j = 0; j < nb; j++) {
+            const float* c = s_cam[j];
+            focal = fmaxf(focal, c[12]);
+            const float z = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(p0, c[2]), __fmul_rn(p1, c[5])), __fmul_rn(p2, c[8])), c[11]);
+            if (!(z > 0.2f)) continue;
+            const float x = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(p0, c[0]), __fmul_rn(p1, c[3])), __fmul_rn(p2, c[6])), c[9]);
+            const float y = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(p0, c[1]), __fmul_rn(p1, c[4])), __fmul_rn(p2, c[7])), c[10]);
+            const float zc = fmaxf(z, 0.001f);
+            const float u = __fadd_rn(__fmul_rn(__fdiv_rn(x, zc), c[12]), c[14]);
+            const float w = __fadd_rn(__fmul_rn(__fdiv_rn(y, zc), c[13]), c[15]);
+            if (u >= c[16] && u <= c[17] && w >= c[18] && w <= c[19]) {
+                dist = fminf(dist, z);
+                seen = true;
+            }
+        }
+        __syncthreads();
+    }
+    const float f = __fmul_rn(__fdiv_rn(dist, focal), 0.4472136f);
+    // seen f > 0 (dist > 0.2): positive floats order like their bit patterns, so the integer maximum is exact and order-free
+    const unsigned wmax = __reduce_max_sync(0xffffffffu, (live && seen) ? __float_as_uint(f) : 0u);
+    if ((threadIdx.x & 31) == 0 && wmax != 0u) atomicMax(max_bits, wmax);
+    if (live) out[i] = seen ? f : -1.0f;
+}
+
+// fills the unseen Gaussians (marked -1 by filter_3d_kernel) with the largest seen f
+__global__ void filter_3d_fill_kernel(float* __restrict__ out, int N, const unsigned* __restrict__ max_bits)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < N && out[i] < 0.0f) out[i] = __uint_as_float(*max_bits);
+}
+
+extern "C" int lgs_filter_3d(const float* position, int C, int S, const float* view, const float* proj, const int* hw, int V,
+                             float* filter_3d, void* stream)
+{
+    LGS_REQUIRE(C >= 0 && S >= 1 && V >= 1, "filter_3d: bad sizes C=%d S=%d V=%d", C, S, V);
+    LGS_REQUIRE((long long)C * S < (1ll << 31), "filter_3d: %lld Gaussians exceed the 32-bit index", (long long)C * S);
+    const int N = C * S;
+    if (N == 0) return LGS_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    unsigned* max_bits = nullptr;
+    LGS_CUDA(cudaMallocAsync((void**)&max_bits, sizeof(unsigned), st));
+    LGS_CUDA(cudaMemsetAsync(max_bits, 0, sizeof(unsigned), st));
+    filter_3d_kernel<<<lgs_cdiv(N, LGS_F3D_THREADS), LGS_F3D_THREADS, 0, st>>>(position, N, view, proj, hw, V, filter_3d, max_bits);
+    LGS_CHECK_LAUNCH("filter_3d_kernel");
+    filter_3d_fill_kernel<<<lgs_cdiv(N, 256), 256, 0, st>>>(filter_3d, N, max_bits);
+    LGS_CHECK_LAUNCH("filter_3d_fill_kernel");
+    LGS_CUDA(cudaFreeAsync(max_bits, st));
+    return LGS_OK;
+}
+
 extern "C" int lgs_cluster_aabb(const float* xyz, const float* scale, const float* rot, int C, int S, float* origin, float* extend,
                                 void* stream)
 {

@@ -63,6 +63,7 @@ class ViewState:
     last: torch.Tensor               # i16[1,1,Hp,Wp] (unsigned 16-bit counts)
     tile_order: Optional[torch.Tensor] = None   # i32[1,tiles]: tile ids, heaviest backward work first
     antialiased: bool = False        # antialiased mode (DESIGN.md section 1): the backward must use the forward's setting
+    filter_3d: Optional[torch.Tensor] = None    # 3D smoothing filter f32[1,C,S] the forward used (DESIGN.md section 1), or None
 
 
 class _Pinned:
@@ -77,18 +78,34 @@ class _Pinned:
         return b
 
 
+def check_filter_3d(filter_3d: Optional[torch.Tensor], xyz: torch.Tensor) -> Optional[torch.Tensor]:
+    """filter_3d must be None or a contiguous float32 tensor on xyz's device, clustered like the opacity ([1,C,S])."""
+    if filter_3d is None:
+        return None
+    C, S = xyz.shape[-2:]
+    if not (filter_3d.device == xyz.device and filter_3d.dtype == _F32 and filter_3d.is_contiguous()
+            and tuple(filter_3d.shape[-2:]) == (C, S) and filter_3d.numel() == C * S):
+        raise RuntimeError(f"filter_3d must be a contiguous float32 tensor of shape [1,{C},{S}] on {xyz.device}")
+    return filter_3d.detach()
+
+
 def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_extend: torch.Tensor, frustumplane: torch.Tensor,
                         view_matrix: torch.Tensor, proj_matrix: torch.Tensor, sh_degree: int, hw: tuple, tile: tuple,
                         enable_statistic: bool = False, specific_tiles: Optional[torch.Tensor] = None, clamp_zero: bool = False,
-                        antialiased: bool = False):
+                        antialiased: bool = False, filter_3d: Optional[torch.Tensor] = None):
     """Forward of one view.  params: xyz[3,C,S] scale[3,C,S] rot[4,C,S] sh_0[1,3,C,S] sh_rest[R,3,C,S]
     opacity[1,C,S] (raw, clustered; float32 CUDA, contiguous).  Returns (img f32[1,3,Hp,Wp] padded to whole
     tiles, ViewState, (fragment_count, fragment_weight) or None).
 
     antialiased: scale each splat's opacity by the compensation of the 2D low-pass filter (DESIGN.md section 1), so that its
-    integrated alpha does not depend on the resolution.  The state remembers it for the backward."""
+    integrated alpha does not depend on the resolution.  The state remembers it for the backward.
+
+    filter_3d: Mip-Splatting's 3D smoothing filter f32[1,C,S] (scene.filter_3d_device), or None.  Each Gaussian is drawn with
+    the scale sqrt(s^2 + f^2) and its opacity scaled by the matching volume ratio (DESIGN.md section 1); the state keeps the
+    tensor for the backward, which must see the same values."""
     xyz = params["xyz"]
     dev = xyz.device
+    filter_3d = check_filter_3d(filter_3d, xyz)
     C, S = xyz.shape[-2:]
     H, W = int(hw[0]), int(hw[1])
     th, tw = int(tile[0]), int(tile[1])
@@ -117,7 +134,7 @@ def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_exte
         _lib.call("lgs_project_forward", int(sh_degree), _ptr(ids), ctypes.c_void_p(counters.data_ptr()), _ptr(view_matrix),
                   _ptr(proj_matrix), _ptr(xyz), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["sh_0"]),
                   _ptr(params["sh_rest"]), _ptr(params["opacity"]), C, S, M, H, W, th, tw, _ptr(packed), _ptr(dkey), _ptr(iota),
-                  _ptr(tcount), ctypes.c_void_p(counters.data_ptr() + 4), int(bool(antialiased)), st)
+                  _ptr(tcount), ctypes.c_void_p(counters.data_ptr() + 4), _ptr(filter_3d), int(bool(antialiased)), st)
         pinned = _Pinned.get(dev)
         pinned.copy_(counters, non_blocking=True)
         torch.cuda.current_stream(dev).synchronize()
@@ -188,7 +205,8 @@ def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_exte
             _lib.call("lgs_tile_order", _ptr(work), 1, ntile, _ptr(order), st)
     state = ViewState(sh_degree=int(sh_degree), hw=(H, W), tile=(th, tw), n_chunks_visible=nvis, n_pairs=D, chunk_ids=ids,
                       counters=counters, view=view_matrix, proj=proj_matrix, packed=packed, tile_count=tcount,
-                      sorted_pid=sorted_pid, ranges=ranges, T=T, last=last, tile_order=order, antialiased=bool(antialiased))
+                      sorted_pid=sorted_pid, ranges=ranges, T=T, last=last, tile_order=order, antialiased=bool(antialiased),
+                      filter_3d=filter_3d)
     return img, state, stats
 
 
@@ -245,7 +263,7 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
                           _ptr(state.view), _ptr(state.proj), _ptr(xyz), _ptr(params["scale"]), _ptr(params["rot"]),
                           _ptr(params["opacity"]), C, S, A, R, H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(pg), None, 2,
                           _ptr(d["xyz"]), _ptr(d["scale"]), _ptr(d["rot"]), _ptr(d["sh_0"]), _ptr(d["sh_rest"]), _ptr(d["opacity"]),
-                          _ptr(d.get("_touched")), *cam_args, int(state.antialiased), st)   # "_touched": chunk marks for the fused optimizer step
+                          _ptr(d.get("_touched")), *cam_args, _ptr(state.filter_3d), int(state.antialiased), st)   # "_touched": chunk marks for the fused optimizer step
             elif camera_grad is not None:
                 camera_grad.zero_()
             return None, pg
@@ -260,7 +278,7 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
             _lib.call("lgs_project_backward", state.sh_degree, _ptr(state.chunk_ids), ctypes.c_void_p(state.counters.data_ptr()),
                       _ptr(state.view), _ptr(state.proj), _ptr(xyz), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["opacity"]),
                       C, S, A, R, H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(pg), None, 0, _ptr(g_pos), _ptr(g_sc), _ptr(g_rot),
-                      _ptr(g_s0), _ptr(g_sr), _ptr(g_op), None, *cam_args, int(state.antialiased), st)
+                      _ptr(g_s0), _ptr(g_sr), _ptr(g_op), None, *cam_args, _ptr(state.filter_3d), int(state.antialiased), st)
         elif camera_grad is not None:
             camera_grad.zero_()
     return [g_pos, g_sc, g_rot, g_s0, g_sr, g_op], pg
@@ -332,7 +350,7 @@ class ViewWorkspace:
         self.views_done = 0
 
     # -- enqueue ---------------------------------------------------------------------------------------------------
-    def _forward_kernels(self, params, cluster_origin, cluster_extend, sh_degree, clamp_zero, antialiased):
+    def _forward_kernels(self, params, cluster_origin, cluster_extend, sh_degree, clamp_zero, antialiased, filter_3d):
         dev, st = self.dev, _stream(self.dev)
         H, W = self.hw
         th, tw = self.tile
@@ -344,7 +362,7 @@ class ViewWorkspace:
         _lib.call("lgs_project_forward", int(sh_degree), _ptr(self.chunk_ids), ctypes.c_void_p(cnt), _ptr(self.cam_view), _ptr(self.cam_proj),
                   _ptr(params["xyz"]), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["sh_0"]), _ptr(params["sh_rest"]),
                   _ptr(params["opacity"]), C, S, C, H, W, th, tw, _ptr(self.packed), _ptr(self.dkey), _ptr(self.iota), _ptr(self.tcount),
-                  ctypes.c_void_p(cnt + 4), int(antialiased), st)
+                  ctypes.c_void_p(cnt + 4), _ptr(filter_3d), int(antialiased), st)
         _lib.call("lgs_view_params", ctypes.c_void_p(cnt), S, D, self.planned_bits, ctypes.c_void_p(vp), _ptr(self.sticky), st)
         n_dev, d_dev, bias_dev = ctypes.c_void_p(vp), ctypes.c_void_p(vp + 4), ctypes.c_void_p(vp + 8)
         wsz = ctypes.c_size_t(self.ws_bytes)
@@ -365,7 +383,7 @@ class ViewWorkspace:
         if order:
             _lib.call("lgs_tile_order", _ptr(self.work), 1, self.ntile, _ptr(self.tile_order), st)
 
-    def _backward_kernels(self, params, sh_degree, accumulate_into, use_clamp, camera_grad, antialiased):
+    def _backward_kernels(self, params, sh_degree, accumulate_into, use_clamp, camera_grad, antialiased, filter_3d):
         st = _stream(self.dev)
         H, W = self.hw
         th, tw = self.tile
@@ -381,7 +399,8 @@ class ViewWorkspace:
                   _ptr(self.cam_proj), _ptr(params["xyz"]), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["opacity"]), C, S, C, R,
                   H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(self.pg), None, 2, _ptr(d["xyz"]), _ptr(d["scale"]), _ptr(d["rot"]),
                   _ptr(d["sh_0"]), _ptr(d["sh_rest"]), _ptr(d["opacity"]), _ptr(d.get("_touched")),
-                  _ptr(self.cam_partials) if camera_grad else None, _ptr(self.d_cam) if camera_grad else None, int(antialiased), st)
+                  _ptr(self.cam_partials) if camera_grad else None, _ptr(self.d_cam) if camera_grad else None, _ptr(filter_3d),
+                  int(antialiased), st)
 
     def _run(self, kind, sig, fn):
         """Eager the first time a pointer signature is seen, captured into a CUDA graph the second time, replayed afterwards."""
@@ -404,22 +423,29 @@ class ViewWorkspace:
         self._graphs[key] = g
         g.replay()
 
-    def forward(self, params, cluster_origin, cluster_extend, cam, sh_degree, clamp_zero=True, antialiased=False):
+    def forward(self, params, cluster_origin, cluster_extend, cam, sh_degree, clamp_zero=True, antialiased=False, filter_3d=None):
         """cam: dict(view, proj, frustumplane) of device tensors.  Returns the padded image (a view of the workspace).
-        antialiased: antialiased mode (DESIGN.md section 1); the backward of this view must be given the same value."""
+        antialiased: antialiased mode (DESIGN.md section 1); the backward of this view must be given the same value.
+        filter_3d: 3D smoothing filter f32[1,C,S] or None; the backward of this view must be given the same tensor.  Its data
+        pointer is part of the graph signature: a replayed graph reads whatever the tensor holds, so recomputing it in place
+        (scene.filter_3d_device(..., out=)) needs no new capture."""
+        filter_3d = check_filter_3d(filter_3d, params["xyz"])
         self.cam_view.copy_(cam["view"], non_blocking=True)
         self.cam_proj.copy_(cam["proj"], non_blocking=True)
         self.cam_planes.copy_(cam["frustumplane"], non_blocking=True)
         sig = (tuple(params[k].data_ptr() for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")), cluster_origin.data_ptr(),
-               cluster_extend.data_ptr(), int(sh_degree), bool(clamp_zero), bool(CONFIG["tile_order"]), bool(antialiased))
-        self._run("fwd", sig, lambda: self._forward_kernels(params, cluster_origin, cluster_extend, sh_degree, clamp_zero, antialiased))
+               cluster_extend.data_ptr(), int(sh_degree), bool(clamp_zero), bool(CONFIG["tile_order"]),
+               0 if filter_3d is None else filter_3d.data_ptr(), bool(antialiased))
+        self._run("fwd", sig, lambda: self._forward_kernels(params, cluster_origin, cluster_extend, sh_degree, clamp_zero, antialiased,
+                                                            filter_3d))
         self.views_done += 1
         return self.img
 
-    def backward(self, params, d_img, sh_degree, accumulate_into, use_clamp=True, camera_grad=None, antialiased=False):
+    def backward(self, params, d_img, sh_degree, accumulate_into, use_clamp=True, camera_grad=None, antialiased=False, filter_3d=None):
         """d_img f32[1,3,H,W] or [1,3,Hp,Wp]: gradient of the loss w.r.t. the (clamped) image.  camera_grad (optional f32[2,4,4]
         CUDA tensor) receives (d view_matrix, d proj_matrix) of this view, copied on the stream after the backward.
-        antialiased: the value the forward of this view was given."""
+        antialiased, filter_3d: the values the forward of this view was given."""
+        filter_3d = check_filter_3d(filter_3d, params["xyz"])
         if camera_grad is not None and not (camera_grad.is_cuda and camera_grad.dtype == _F32 and tuple(camera_grad.shape) == (2, 4, 4)):
             raise RuntimeError("camera_grad must be a float32 CUDA tensor of shape [2,4,4]")
         H, W = self.hw
@@ -432,9 +458,9 @@ class ViewWorkspace:
         sig = (tuple(params[k].data_ptr() for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")),
                tuple(accumulate_into[k].data_ptr() for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")),
                0 if accumulate_into.get("_touched") is None else accumulate_into["_touched"].data_ptr(), int(sh_degree), bool(use_clamp),
-               bool(CONFIG["tile_order"]), bool(antialiased), camera_grad is not None)
+               bool(CONFIG["tile_order"]), bool(antialiased), 0 if filter_3d is None else filter_3d.data_ptr(), camera_grad is not None)
         cam = camera_grad is not None
-        self._run("bwd", sig, lambda: self._backward_kernels(params, sh_degree, accumulate_into, use_clamp, cam, antialiased))
+        self._run("bwd", sig, lambda: self._backward_kernels(params, sh_degree, accumulate_into, use_clamp, cam, antialiased, filter_3d))
         if cam:
             camera_grad.copy_(self.d_cam, non_blocking=True)
 
@@ -470,15 +496,16 @@ class CapacityExceeded(RuntimeError):
         self.pairs, self.pair_capacity, self.depth_bits, self.planned_depth_bits = pairs, pair_capacity, depth_bits, planned_depth_bits
 
 
-def probe_view_sizes(params, cluster_origin, cluster_extend, cams, sh_degree, hw, tile, antialiased=False):
+def probe_view_sizes(params, cluster_origin, cluster_extend, cams, sh_degree, hw, tile, antialiased=False, filter_3d=None):
     """One synchronising forward per camera (the cold path) -> (max pairs, max depth-key bits): the first-epoch sizing step of
-    the reference's feedback protocol, used to dimension a ViewWorkspace.  antialiased: size for that mode (it has fewer pairs)."""
+    the reference's feedback protocol, used to dimension a ViewWorkspace.  antialiased, filter_3d: size for that mode and filter
+    (both change the pair count)."""
     max_pairs, max_bits = 0, 1
     p = {k: params[k].detach() for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")}
     with torch.no_grad():
         for cam in cams:
             _, st, _ = render_view_forward(p, cluster_origin, cluster_extend, cam["frustumplane"], cam["view"], cam["proj"], sh_degree, hw, tile,
-                                           antialiased=antialiased)
+                                           antialiased=antialiased, filter_3d=filter_3d)
             max_pairs = max(max_pairs, st.n_pairs)
             c = st.counters.cpu()
             kmin, kmax = ~int(c[2]) & 0xFFFFFFFF, int(c[3]) & 0xFFFFFFFF

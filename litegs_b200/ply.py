@@ -6,7 +6,9 @@ file format): ``binary_little_endian 1.0``, one ``vertex`` element of float32 pr
 
 with the SH rest coefficients channel-major (``f_rest_[c (K-1) + k]``), log-scales, opacity logits and (w,x,y,z) rotations
 stored raw.  ``save_ply`` / ``load_ply`` keep the reference's signatures (``[C, N]`` arrays, SH as ``[1,3,N]`` / ``[K-1,3,N]``);
-``params_from_ply`` / ``params_to_ply`` convert to and from this package's clustered parameter dict.
+``params_from_ply`` / ``params_to_ply`` convert to and from this package's clustered parameter dict.  Checkpoints trained with
+Mip-Splatting's 3D smoothing filter carry it as one more float property, ``filter_3D``, after ``rot_3``; it is written when given
+and read (by name) into the dict's ``"filter_3D"`` entry when the file has it.
 """
 from __future__ import annotations
 
@@ -24,14 +26,16 @@ def _names(n_dc: int, n_rest: int):
             [f"scale_{i}" for i in range(3)] + [f"rot_{i}" for i in range(4)])
 
 
-def save_ply(path: str, xyz, scale, rot, sh_0, sh_rest, opacity) -> None:
-    """xyz [3,N] scale [3,N] rot [4,N] sh_0 [1,3,N] sh_rest [K-1,3,N] opacity [1,N] (raw parameters)."""
+def save_ply(path: str, xyz, scale, rot, sh_0, sh_rest, opacity, filter_3d=None) -> None:
+    """xyz [3,N] scale [3,N] rot [4,N] sh_0 [1,3,N] sh_rest [K-1,3,N] opacity [1,N] (raw parameters); filter_3d [1,N] or None
+    (written as the last property, filter_3D)."""
     xyz = np.asarray(xyz, np.float32); n = xyz.shape[1]
     dc = np.asarray(sh_0, np.float32).transpose(2, 1, 0).reshape(n, -1)            # [N, 3]
     rest = np.asarray(sh_rest, np.float32).transpose(2, 1, 0).reshape(n, -1)       # [N, 3 (K-1)], channel-major
     cols = np.concatenate([xyz.T, np.zeros((n, 3), np.float32), dc, rest, np.asarray(opacity, np.float32).T,
-                           np.asarray(scale, np.float32).T, np.asarray(rot, np.float32).T], axis=1).astype("<f4")
-    names = _names(dc.shape[1], rest.shape[1])
+                           np.asarray(scale, np.float32).T, np.asarray(rot, np.float32).T] +
+                          ([] if filter_3d is None else [np.asarray(filter_3d, np.float32).reshape(1, n).T]), axis=1).astype("<f4")
+    names = _names(dc.shape[1], rest.shape[1]) + ([] if filter_3d is None else ["filter_3D"])
     assert cols.shape[1] == len(names)
     header = "ply\nformat binary_little_endian 1.0\nelement vertex %d\n" % n + "".join(f"property float {a}\n" for a in names) + "end_header\n"
     d = os.path.dirname(path)
@@ -83,7 +87,10 @@ def _read_vertex_table(path: str):
 def load_ply(path: str, sh_degree: int):
     """-> xyz [3,N], scale [3,N], rot [4,N], sh_0 [1,3,N], sh_rest [K-1,3,N], opacity [1,N]  (float32), the reference's
     return order (ply.py:47-87).  Files with fewer SH bands than sh_degree are zero-extended; more is an error."""
-    t = _read_vertex_table(path)
+    return _params_of_table(_read_vertex_table(path), path, sh_degree)
+
+
+def _params_of_table(t, path: str, sh_degree: int):
     n = t.shape[0]
     col = lambda name: np.asarray(t[name], np.float32)
     xyz = np.stack([col("x"), col("y"), col("z")])
@@ -102,8 +109,13 @@ def load_ply(path: str, sh_degree: int):
 
 
 def params_from_ply(path: str, sh_degree: int = 3, chunk: int = 128, morton: bool = True) -> dict:
-    """PLY -> clustered parameter dict (+ cluster_origin / cluster_extend, n_points), Morton sorted like scene.make_scene."""
-    vals = dict(zip(PARAM_KEYS, load_ply(path, sh_degree)))
+    """PLY -> clustered parameter dict (+ cluster_origin / cluster_extend, n_points), Morton sorted like scene.make_scene.
+    A file with the filter_3D property also gives "filter_3D" [1,C,S]; the chunk boxes stay those of the unfiltered splats
+    (scene.cluster_aabb(..., filter_3d=) gives the filtered ones)."""
+    t = _read_vertex_table(path)
+    vals = dict(zip(PARAM_KEYS, _params_of_table(t, path, sh_degree)))
+    if "filter_3D" in t.dtype.names:
+        vals["filter_3D"] = np.asarray(t["filter_3D"], np.float32)[None]
     n = vals["xyz"].shape[-1]
     order = scene.morton_order(vals["xyz"]) if morton else np.arange(n)
     out = {k: scene.cluster(np.ascontiguousarray(v[..., order]), chunk) for k, v in vals.items()}
@@ -113,7 +125,9 @@ def params_from_ply(path: str, sh_degree: int = 3, chunk: int = 128, morton: boo
 
 
 def params_to_ply(path: str, params: dict, n_points: int | None = None) -> None:
-    """Clustered parameter dict -> PLY; n_points drops the padding of the last chunk."""
-    flat = {k: np.asarray(params[k]).reshape(*np.asarray(params[k]).shape[:-2], -1) for k in PARAM_KEYS}
+    """Clustered parameter dict -> PLY; n_points drops the padding of the last chunk.  A "filter_3D" entry ([1,C,S]) is written
+    as the filter_3D property."""
+    keys = PARAM_KEYS + (("filter_3D",) if params.get("filter_3D") is not None else ())
+    flat = {k: np.asarray(params[k]).reshape(*np.asarray(params[k]).shape[:-2], -1) for k in keys}
     n = flat["xyz"].shape[-1] if n_points is None else int(n_points)
-    save_ply(path, *[flat[k][..., :n] for k in PARAM_KEYS])
+    save_ply(path, *[flat[k][..., :n] for k in PARAM_KEYS], filter_3d=flat["filter_3D"][..., :n] if "filter_3D" in flat else None)

@@ -133,14 +133,15 @@ def _feed_statistics(state, stats, packed_grad, tile):
 class _RenderViewFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, xyz, scale, rot, sh_0, sh_rest, opacity, cluster_origin, cluster_extend, frustumplane,
-                view_matrix, proj_matrix, sh_degree, H, W, th, tw, sparse_grad, enable_transmitance, accumulate_into, antialiased):
+                view_matrix, proj_matrix, sh_degree, H, W, th, tw, sparse_grad, enable_transmitance, accumulate_into, antialiased,
+                filter_3d):
         params = dict(xyz=xyz, scale=scale, rot=rot, sh_0=sh_0, sh_rest=sh_rest, opacity=opacity)
         stat = bool(StatisticsHelperInst.bStart)
         ctx.set_materialize_grads(False)       # an unused transmittance output must not cost a zero-filled gradient image
         # the kernel writes clamp(c,0,1) directly (render/__init__.py:87 does it as a separate pass) ...
         img, state, stats = pipeline.render_view_forward(params, cluster_origin, cluster_extend, frustumplane, view_matrix,
                                                          proj_matrix, sh_degree, (H, W), (th, tw), enable_statistic=stat, clamp_zero=True,
-                                                         antialiased=antialiased)
+                                                         antialiased=antialiased, filter_3d=filter_3d)
         ctx.state = state
         ctx.stats = stats
         ctx.stat = stat
@@ -174,7 +175,7 @@ class _RenderViewFn(torch.autograd.Function):
             g_proj = cam[1].reshape(state.proj.shape) if ctx.needs_input_grad[10] else None
         if grads is None:          # gradients went straight into the caller's dense buffers
             ctx.state = None
-            return (None,) * 9 + (g_view, g_proj) + (None,) * 9
+            return (None,) * 9 + (g_view, g_proj) + (None,) * 10
         C, S = xyz.shape[-2:]
         ids = state.chunk_ids[: state.n_chunks_visible]
         out = []
@@ -182,11 +183,11 @@ class _RenderViewFn(torch.autograd.Function):
             ct = CompactedTensor((*g.shape[:-2], C, S), ids, g)
             out.append(ct if ctx.sparse else ct.to_dense())
         ctx.state = None
-        return (*out, None, None, None, g_view, g_proj, None, None, None, None, None, None, None, None, None)
+        return (*out, None, None, None, g_view, g_proj, None, None, None, None, None, None, None, None, None, None)
 
 
 def render_view(cluster_origin, cluster_extend, frustumplane, view_matrix, proj_matrix,
-                xyz, scale, rot, sh_0, sh_rest, opacity, actived_sh_degree: int, output_shape, pp, accumulate_into=None):
+                xyz, scale, rot, sh_0, sh_rest, opacity, actived_sh_degree: int, output_shape, pp, accumulate_into=None, filter_3d=None):
     """render_preprocess + render of one view on the fused pipeline.
 
     Same inputs as the two reference calls (raw clustered parameters, chunk AABBs, camera); returns the five values of the
@@ -194,14 +195,16 @@ def render_view(cluster_origin, cluster_extend, frustumplane, view_matrix, proj_
     None, depth=None, normal=None, last_contributor [1,1,Hp,Wp]).  Gradients reach the six parameter tensors as CompactedTensor (pp.sparse_grad) or dense
     tensors -- or, with ``accumulate_into`` (dict of dense gradient tensors, e.g. ``GradAccumulator.grads()``), are
     ADDED into those buffers by the backward kernel itself and ``param.grad`` stays untouched (multi-view batches,
-    data-parallel training).  ``pp.antialiased`` (absent = False) selects the antialiased mode (DESIGN.md section 1)."""
+    data-parallel training).  ``pp.antialiased`` (absent = False) selects the antialiased mode (DESIGN.md section 1).
+    ``filter_3d`` (f32[1,C,S] or None): Mip-Splatting's 3D smoothing filter (scene.filter_3d_device, DESIGN.md section 1); it is
+    an input without a gradient."""
     if not pp.cluster_size:
         raise RuntimeError("render_view needs the clustered layout (cluster_size > 0); use render_preprocess + render otherwise")
     H, W = int(output_shape[0]), int(output_shape[1])
     th, tw = int(pp.tile_size[0]), int(pp.tile_size[1])
     img, T, last = _RenderViewFn.apply(xyz, scale, rot, sh_0, sh_rest, opacity, cluster_origin, cluster_extend, frustumplane,
                                        view_matrix, proj_matrix, int(actived_sh_degree), H, W, th, tw, pp.sparse_grad,
-                                       pp.enable_transmitance, accumulate_into, bool(getattr(pp, "antialiased", False)))
+                                       pp.enable_transmitance, accumulate_into, bool(getattr(pp, "antialiased", False)), filter_3d)
     img = img[..., :H, :W]          # already clamped to [0,1] by the kernel
     trans = T[..., :H, :W] if pp.enable_transmitance else None
     return img, trans, None, None, last
@@ -226,7 +229,7 @@ def _streams(dev, n):
 
 def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_extend,
                  xyz, scale, rot, sh_0, sh_rest, opacity, actived_sh_degree: int, output_shape, pp,
-                 accumulate_into: dict, n_streams: int = 4, loss_and_grad_fn=None, camera_grads=None):
+                 accumulate_into: dict, n_streams: int = 4, loss_and_grad_fn=None, camera_grads=None, filter_3d=None):
     """Forward + backward of a batch of views with the gradients summed into ``accumulate_into`` (dense tensors shaped
     like the parameters, e.g. ``GradAccumulator.grads()``).  This is the per-rank body of a data-parallel step.
 
@@ -243,8 +246,11 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
     handed to the function is the kernel's clamp(0,1) output and its gradient goes straight to the raster backward.
 
     ``camera_grads`` (optional contiguous f32[n_views,2,4,4] CUDA tensor): slot i receives (d view_matrix, d proj_matrix) of view i
-    (pipeline.render_view_backward), on every path; it is complete when this function returns (the current stream waits)."""
+    (pipeline.render_view_backward), on every path; it is complete when this function returns (the current stream waits).
+
+    ``filter_3d`` (f32[1,C,S] or None): the 3D smoothing filter every view of the batch is drawn with (see render_view)."""
     dev = xyz.device
+    filter_3d = pipeline.check_filter_3d(filter_3d, xyz)
     if camera_grads is not None and not (camera_grads.is_cuda and camera_grads.dtype == torch.float32 and camera_grads.is_contiguous()
                                          and tuple(camera_grads.shape) == (n_views, 2, 4, 4)):
         raise RuntimeError(f"camera_grads must be a contiguous float32 CUDA tensor of shape [{n_views},2,4,4]")
@@ -263,7 +269,7 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
         cam = camera_fn(i)
         img_p, state, stats = pipeline.render_view_forward(params, cluster_origin, cluster_extend, cam["frustumplane"], cam["view"],
                                                            cam["proj"], int(actived_sh_degree), (H, W), (th, tw), enable_statistic=stat,
-                                                           clamp_zero=True, antialiased=aa)
+                                                           clamp_zero=True, antialiased=aa, filter_3d=filter_3d)
         if loss_and_grad_fn is not None:
             loss, d_img = loss_and_grad_fn(i, img_p[..., :H, :W])
         else:                          # autograd only through the user's loss, never through the render kernels
@@ -289,7 +295,7 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
         if camera_grads is not None:              # leaves of this call: their .grad is view i's camera gradient
             view, proj = view.detach().requires_grad_(True), proj.detach().requires_grad_(True)
         img = render_view(cluster_origin, cluster_extend, cam["frustumplane"], view, proj, xyz, scale, rot, sh_0, sh_rest,
-                          opacity, actived_sh_degree, output_shape, pp, accumulate_into=accumulate_into)[0]
+                          opacity, actived_sh_degree, output_shape, pp, accumulate_into=accumulate_into, filter_3d=filter_3d)[0]
         loss = loss_fn(i, img)
         if wait_ev is not None:          # the previous view's accumulate (other stream) must have landed
             torch.cuda.current_stream(dev).wait_event(wait_ev)
@@ -307,14 +313,15 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
     # path and measures the capacities (the reference's cold first epoch); statistics runs keep the synchronising path.
     slots = None
     if direct and pipeline.SYNC_FREE and not stat:
-        slots = _view_slots(params, (H, W), (th, tw), max(1, n_streams), aa)
+        slots = _view_slots(params, (H, W), (th, tw), max(1, n_streams), aa, filter_3d is not None)
         if slots.big:
             slots = None
     probe = {"pairs": 0, "bits": 1} if (slots is not None and slots.ws is None) else None
 
     def one_ws(i, wait_ev, ws):
         cam = camera_fn(i)
-        img_p = ws.forward(params, cluster_origin, cluster_extend, cam, int(actived_sh_degree), clamp_zero=True, antialiased=aa)
+        img_p = ws.forward(params, cluster_origin, cluster_extend, cam, int(actived_sh_degree), clamp_zero=True, antialiased=aa,
+                           filter_3d=filter_3d)
         if loss_and_grad_fn is not None:
             loss, d_img = loss_and_grad_fn(i, img_p[..., :H, :W])
         else:
@@ -326,7 +333,8 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
                 (d_img,) = torch.autograd.grad(loss, leaf)
         if wait_ev is not None:
             torch.cuda.current_stream(dev).wait_event(wait_ev)
-        ws.backward(params, d_img, int(actived_sh_degree), accumulate_into, use_clamp=True, camera_grad=slot(i), antialiased=aa)
+        ws.backward(params, d_img, int(actived_sh_degree), accumulate_into, use_clamp=True, camera_grad=slot(i), antialiased=aa,
+                    filter_3d=filter_3d)
         losses.append(loss.detach())
 
     def one_probe(i, wait_ev):
@@ -381,8 +389,8 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
 
 class _ViewSlots:
     """The per-configuration state of render_views' GPU-driven path: capacities measured by the first (synchronising) batch and
-    one ViewWorkspace per stream slot, created from them.  The antialiased mode is part of the configuration: it has fewer
-    pairs, so capacities measured with it on would overflow with it off."""
+    one ViewWorkspace per stream slot, created from them.  The antialiased mode and the use of a 3D filter are part of the
+    configuration: both change the pair count, so capacities measured with one setting could overflow with another."""
 
     def __init__(self, params, hw, tile):
         self.params_like, self.hw, self.tile = params, hw, tile
@@ -421,9 +429,9 @@ class _ViewSlots:
 _slot_cache: dict = {}
 
 
-def _view_slots(params, hw, tile, n_slots, antialiased=False):
+def _view_slots(params, hw, tile, n_slots, antialiased=False, filtered=False):
     xyz = params["xyz"]
-    key = (xyz.device, tuple(xyz.shape[-2:]), hw, tile, params["sh_rest"].shape[0], bool(antialiased))
+    key = (xyz.device, tuple(xyz.shape[-2:]), hw, tile, params["sh_rest"].shape[0], bool(antialiased), bool(filtered))
     ent = _slot_cache.get(key)
     if ent is None:
         ent = _slot_cache[key] = _ViewSlots(params, hw, tile)

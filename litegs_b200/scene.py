@@ -106,12 +106,15 @@ def quat_to_R(q: np.ndarray) -> np.ndarray:
     ])
 
 
-def cluster_aabb(xyz_c: np.ndarray, scale_c: np.ndarray, rot_c: np.ndarray):
+def cluster_aabb(xyz_c: np.ndarray, scale_c: np.ndarray, rot_c: np.ndarray, filter_3d=None):
     """Chunk AABBs from raw (log-scale, unnormalised quaternion) clustered params;
-    semantics of reference litegs/scene/cluster.py:29-46 -> (origin [3,C], extend [3,C])."""
+    semantics of reference litegs/scene/cluster.py:29-46 -> (origin [3,C], extend [3,C]).
+    filter_3d ([1,C,S] or None): the boxes cover the splats widened by the 3D smoothing filter, scale sqrt(s^2 + f^2)."""
     C, S = xyz_c.shape[-2:]
     xyz = xyz_c.reshape(3, -1).astype(np.float64)
     s = np.exp(scale_c.reshape(3, -1).astype(np.float64))
+    if filter_3d is not None:
+        s = np.sqrt(s * s + np.asarray(filter_3d, np.float64).reshape(1, -1) ** 2)
     q = rot_c.reshape(4, -1).astype(np.float64)
     q = q / np.linalg.norm(q, axis=0, keepdims=True)
     T = quat_to_R(q) * s[:, None, :]
@@ -121,13 +124,16 @@ def cluster_aabb(xyz_c: np.ndarray, scale_c: np.ndarray, rot_c: np.ndarray):
     return ((hi + lo) / 2).astype(np.float32), ((hi - lo) / 2).astype(np.float32)
 
 
-def cluster_aabb_torch(xyz_c, scale_c, rot_c):
+def cluster_aabb_torch(xyz_c, scale_c, rot_c, filter_3d=None):
     """cluster_aabb on torch tensors of any device (the chunk maintenance step of a training loop: positions and shapes
-    move, the culling boxes follow without a host round trip).  Same semantics, float32 -> (origin [3,C], extend [3,C])."""
+    move, the culling boxes follow without a host round trip).  Same semantics, float32 -> (origin [3,C], extend [3,C]).
+    filter_3d ([1,C,S] or None): as in cluster_aabb."""
     import torch
     C, S = xyz_c.shape[-2:]
     xyz = xyz_c.reshape(3, -1).float()
     s = torch.exp(scale_c.reshape(3, -1).float())
+    if filter_3d is not None:
+        s = torch.sqrt(s * s + filter_3d.reshape(1, -1).float().square())
     q = rot_c.reshape(4, -1).float()
     q = q / q.norm(dim=0, keepdim=True)
     r, x, y, z = q[0], q[1], q[2], q[3]
@@ -182,6 +188,34 @@ def cluster_aabb_device(xyz_c, scale_c, rot_c):
         extend = torch.empty((3, C), dtype=torch.float32, device=dev)
         _lib.call("lgs_cluster_aabb", _ptr(x), _ptr(s), _ptr(q), C, S, _ptr(origin), _ptr(extend), _stream(dev))
     return origin, extend
+
+
+def filter_3d_device(xyz_c, views, projs, hw, out=None):
+    """Mip-Splatting's 3D smoothing filter (compute_3D_filter) in two kernels (csrc/scene.cu, DESIGN.md section 1): xyz_c
+    f32[3,C,S] on CUDA (every slot, the tail padding included), the training cameras views / projs f32[V,4,4] (row-vector
+    convention) and hw (V image sizes (height, width): i32[V,2] tensor or sequence) -> f32[1,C,S], no gradient.
+
+    out: an f32[1,C,S] tensor to write in place (keeps the data pointer, so CUDA graphs captured with it stay valid).  No host
+    synchronisation: it can run inside a training step."""
+    import torch
+    from . import _lib
+    from .fused import _f32c, _ptr, _stream
+    x = _f32c(xyz_c.detach(), "xyz")
+    C, S = x.shape[-2:]
+    dev = x.device
+    V = _f32c(views.detach().to(dev), "views").reshape(-1, 4, 4)
+    P = _f32c(projs.detach().to(dev), "projs").reshape(-1, 4, 4)
+    hw_t = torch.as_tensor(hw, dtype=torch.int32).to(dev).reshape(-1, 2).contiguous()
+    nv = V.shape[0]
+    if nv < 1 or P.shape[0] != nv or hw_t.shape[0] != nv:
+        raise RuntimeError(f"filter_3d_device: {V.shape[0]} views, {P.shape[0]} projections and {hw_t.shape[0]} image sizes")
+    if out is None:
+        out = torch.empty((1, C, S), dtype=torch.float32, device=dev)
+    elif not (out.device == dev and out.dtype == torch.float32 and out.is_contiguous() and out.numel() == C * S):
+        raise RuntimeError(f"filter_3d_device: out must be a contiguous float32 tensor of {C * S} elements on {dev}")
+    with torch.cuda.device(dev):
+        _lib.call("lgs_filter_3d", _ptr(x), C, S, _ptr(V), _ptr(P), _ptr(hw_t), nv, _ptr(out), _stream(dev))
+    return out
 
 
 def morton_codes_device(xyz, bits: int = 21):
