@@ -3,6 +3,7 @@
     python examples/train_colmap.py --make /tmp/synth_colmap          # writes a synthetic dataset first (renders of a hidden scene)
     python examples/train_colmap.py --data /path/to/colmap --iters 2000
     python examples/train_colmap.py --make /tmp/noisy --pose-noise 1 0.02 --refine-poses     # learn the camera poses too
+    python examples/train_colmap.py --make /tmp/noisy --pose-noise 1 0.02 --refine-poses --exact-grad   # ... with the J and SH terms
 
 Reads ``sparse/0/{cameras,images,points3D}.bin`` and ``images/*`` (litegs_b200.colmap; same files and conventions as the
 reference's ``litegs/io_manager/colmap.py`` + ``litegs/data.py``), initialises Gaussians from the SfM points the way
@@ -84,14 +85,14 @@ def load_dataset(root, image_dir="images", dev=None):
     return frames, np.stack([p.xyz for p in P]), np.stack([p.rgb for p in P])
 
 
-def train(root, iters=300, views_per_step=8, log=print, refine_poses=False, antialiased=False, filter_3d=False):
+def train(root, iters=300, views_per_step=8, log=print, refine_poses=False, antialiased=False, filter_3d=False, exact_grad=False):
     from litegs_b200 import fused
     if refine_poses and int(os.environ.get("WORLD_SIZE", "1")) > 1:
         raise ValueError("--refine-poses runs on one GPU: multi-GPU pose refinement is not supported")
     keep = fused.CONFIG["true_sigmoid_grad"]
     fused.CONFIG["true_sigmoid_grad"] = True               # our own loops train with the true sigmoid derivative (SURVEY Q15)
     try:
-        return _train(root, iters, views_per_step, log, refine_poses, antialiased, filter_3d)
+        return _train(root, iters, views_per_step, log, refine_poses, antialiased, filter_3d, exact_grad)
     finally:
         fused.CONFIG["true_sigmoid_grad"] = keep
 
@@ -128,7 +129,7 @@ class _Poses:
         self.opt.step()
 
 
-def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=False, filter_3d=False):
+def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=False, filter_3d=False, exact_grad=False):
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", 0)))
     torch.cuda.set_device(dev)
     frames, xyz, rgb = load_dataset(root, dev=dev)
@@ -138,7 +139,7 @@ def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=Fal
     cgrads = torch.empty((views_per_step, 2, 4, 4), dtype=torch.float32, device=dev) if poses else None
     g = colmap.gaussians_from_points(xyz, rgb, sh_degree=3)
     P = {k: torch.from_numpy(g[k]).to(dev) for k in PARAM_ORDER}
-    pp = PipelineParams(tile_size=(8, 16), sparse_grad=True, antialiased=antialiased)
+    pp = PipelineParams(tile_size=(8, 16), sparse_grad=True, antialiased=antialiased, exact_grad=exact_grad)
     acc = lgs_dist.GradAccumulator(P)
     extent = float(np.linalg.norm(xyz.max(0) - xyz.min(0)) * 0.5)
     opt, sched = optimizer.get_optimizer(P, spatial_lr_scale=extent)
@@ -197,6 +198,8 @@ if __name__ == "__main__":
     ap.add_argument("--antialiased", action="store_true", help="train (and evaluate) in the antialiased mode")
     ap.add_argument("--filter-3d", action="store_true",
                     help="Mip-Splatting's 3D smoothing filter, from all training cameras at iteration 0 and every 100 iterations")
+    ap.add_argument("--exact-grad", action="store_true",
+                    help="exact position and camera gradients: also through the ray-space Jacobian and the SH view direction")
     ap.add_argument("--pose-noise", type=float, nargs=2, default=None, metavar=("DEG", "FRAC"),
                     help="with --make: perturb the written poses by DEG degrees and FRAC of the camera distance")
     a = ap.parse_args()
@@ -205,5 +208,6 @@ if __name__ == "__main__":
         root = make_dataset(a.make, pose_noise=a.pose_noise)
     if root is None:
         ap.error("give --data or --make")
-    h, _ = train(root, a.iters, refine_poses=a.refine_poses, antialiased=a.antialiased, filter_3d=a.filter_3d)
+    h, _ = train(root, a.iters, refine_poses=a.refine_poses, antialiased=a.antialiased, filter_3d=a.filter_3d,
+                 exact_grad=a.exact_grad)
     assert h[-1] < h[0]

@@ -22,24 +22,26 @@ from litegs_b200.arguments import PipelineParams  # noqa: E402
 from litegs_b200.dist import PARAM_ORDER  # noqa: E402
 
 
-def train(n_gaussians=50_000, hw=(270, 480), n_views=16, iters=100, seed=0, device=None, log=print, perturb=0.3, antialiased=False):
+def train(n_gaussians=50_000, hw=(270, 480), n_views=16, iters=100, seed=0, device=None, log=print, perturb=0.3, antialiased=False,
+          exact_grad=False):
     """Returns the list of per-iteration mean losses (rank-local views)."""
     keep = fused.CONFIG["true_sigmoid_grad"]
     fused.CONFIG["true_sigmoid_grad"] = True               # our own loops train with the true sigmoid derivative (SURVEY Q15)
     try:
-        return _train(n_gaussians, hw, n_views, iters, seed, device, log, perturb, antialiased)
+        return _train(n_gaussians, hw, n_views, iters, seed, device, log, perturb, antialiased, exact_grad)
     finally:
         fused.CONFIG["true_sigmoid_grad"] = keep
 
 
-def _train(n_gaussians, hw, n_views, iters, seed, device, log, perturb, antialiased=False):
+def _train(n_gaussians, hw, n_views, iters, seed, device, log, perturb, antialiased=False, exact_grad=False):
     import torch.distributed as dist
     world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
     rank = dist.get_rank() if world > 1 else 0
     dev = device or torch.device("cuda", int(os.environ.get("LOCAL_RANK", 0)))
     torch.cuda.set_device(dev)
     H, W = hw
-    pp = PipelineParams(tile_size=(8, 16), sparse_grad=True, antialiased=antialiased)     # targets and model in the same mode
+    pp = PipelineParams(tile_size=(8, 16), sparse_grad=True, antialiased=antialiased,     # targets and model in the same mode
+                        exact_grad=exact_grad)
     truth = scene.make_scene(n_gaussians, sh_degree=3, seed=seed)
     T = {k: torch.from_numpy(truth[k]).to(dev) for k in PARAM_ORDER}
     A = [torch.from_numpy(truth[k]).to(dev) for k in ("cluster_origin", "cluster_extend")]
@@ -87,11 +89,14 @@ def main():
     ap.add_argument("--views", type=int, default=16)
     ap.add_argument("--iters", type=int, default=200)
     ap.add_argument("--antialiased", action="store_true", help="render the targets and train in the antialiased mode")
+    ap.add_argument("--exact-grad", action="store_true",
+                    help="exact position gradients: also through the ray-space Jacobian and the SH view direction")
     args = ap.parse_args()
     import torch.distributed as dist
     if int(os.environ.get("WORLD_SIZE", "1")) > 1:
         dist.init_process_group("nccl")
-    hist = train(args.gaussians, (args.height, args.width), args.views, args.iters, antialiased=args.antialiased)
+    hist = train(args.gaussians, (args.height, args.width), args.views, args.iters, antialiased=args.antialiased,
+                 exact_grad=args.exact_grad)
     if dist.is_initialized():
         dist.destroy_process_group()
     assert hist[-1] < hist[0], "the loss did not decrease"

@@ -291,14 +291,23 @@ int lgs_emit_pairs_u16(const float* packed_params, const int* offset, const unsi
  * antialiased: must equal the value the forward of this view was given (ours, no reference counterpart).  The record
  * gradient is then taken at the compensated opacity and the gradient of rho flows into scale, rotation and the camera.
  * filter_3d: the tensor the forward of this view was given, or NULL.  The filter is held constant: the raw scale gradient
- * gains the rho3 term, and no gradient flows into the filter, the positions or the cameras through it. */
+ * gains the rho3 term, and no gradient flows into the filter, the positions or the cameras through it.
+ * exact_grad != 0: exact gradient mode, ours (the reference drops both terms).  g_position, and d_cam when given, also
+ * receive the terms through the ray-space Jacobian J (its dependence on the view-space position and on proj[0][0],
+ * proj[1][1]) and through the SH view direction (its dependence on the position and on the camera centre) (DESIGN.md
+ * section 1, "Exact gradient mode").  The other five gradients are unchanged.  sh_base, sh_rest: the coefficients the forward
+ * was given.  sh_base is not read (the constant band has no direction term; it may be NULL).  sh_rest is read only when
+ * exact_grad != 0 and sh_degree > 0 (its rows of the active degree) and must be non-NULL then; at degree 0 it may be NULL, as
+ * an empty tensor's pointer is.  With exact_grad != 0 the chunk size S is limited by the register use of the instantiation
+ * (384 for the heaviest; a larger S is refused with an error naming the limit).  0 = the kernels without the terms. */
 int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
                          const float* view_matrix, const float* proj_matrix, const float* position, const float* scale,
                          const float* rotation, const float* opacity, int C, int S, int A, int rest_dim, int img_h,
                          int img_w, int true_sigmoid_grad, const float* packed_grad, const float* grad_inv_scaler,
                          int zero_outputs, float* g_position, float* g_scale, float* g_rotation, float* g_sh_base,
                          float* g_sh_rest, float* g_opacity, float* touched, float* cam_partials, float* d_cam,
-                         const float* filter_3d, int antialiased, void* stream);
+                         const float* filter_3d, int antialiased, const float* sh_base, const float* sh_rest, int exact_grad,
+                         void* stream);
 
 /* create_viewproj_forward, GR/compact.cu:17-141: view_params f32[V,7] (qw qx qy qz tx ty tz), recp_tan_half_fov_x f32[1] ->
  * view, proj, viewproj f32[V,4,4] (row-vector convention) and frustumplane f32[V,6,4].  One thread per view. */

@@ -14,3 +14,5 @@ class PipelineParams:
     # ours, not the reference's: antialiased mode of the fused path (DESIGN.md section 1).  Readers use
     # getattr(pp, "antialiased", False), so the reference's own PipelineParams keeps working.
     antialiased: bool = False
+    # ours as well: exact gradient mode of the fused path's backward (DESIGN.md section 1), read as getattr(pp, "exact_grad", False)
+    exact_grad: bool = False

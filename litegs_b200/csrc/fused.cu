@@ -50,6 +50,28 @@ __device__ __forceinline__ void fused_J(const float* __restrict__ P, const float
     J[0] = fx * rz; J[1] = 0.f; J[2] = 0.f; J[3] = fy * rz; J[4] = -fx * tx * rz2; J[5] = -fy * ty * rz2;
 }
 
+// Exact gradient mode (DESIGN.md section 1): one axis of fused_J backwards, as written.  p = P00 (P11), n = W (H), t = tx (ty);
+// dJd = d J00 (J11), dJ2 = d J20 (J21), rz and rz2 as in fused_J.  Each clamp passes the gradient to the operand it returned;
+// at a tie that is the position, not the limit.  Adds to d t, d tz and d rz; returns d p.
+__device__ __forceinline__ float fused_J_axis_backward(float p, float n, float t, float tz, float rz, float rz2, float dJd, float dJ2,
+                                                       float& dt, float& dtz, float& drz)
+{
+    const float f = p * n * 0.5f;
+    const float l = tz / p * 1.3f;
+    const float m = fminf(t, l);
+    const float th = fmaxf(m, -l);
+    const float df = dJd * rz - dJ2 * th * rz2;              // J_d = f rz, J_2 = -f th rz2
+    const float dth = -dJ2 * f * rz2;
+    drz += dJd * f - 2.0f * dJ2 * f * th * rz;
+    float dm = dth, dl = 0.0f;
+    if (m < -l) { dm = 0.0f; dl = -dth; }
+    float dtt = dm;
+    if (t > l) { dtt = 0.0f; dl += dm; }
+    dt += dtt;
+    dtz += dl * 1.3f / p;
+    return df * n * 0.5f - dl * l / p;
+}
+
 // Mip-Splatting's 3D smoothing filter (DESIGN.md section 1, "3D smoothing filter"): s'_k = sqrt(s_k^2 + f^2) and
 // rho3 = sqrt((r_0 r_1) r_2) with r_k = s_k^2 / (s_k^2 + f^2), every step one correctly rounded op in this order, so that
 // tests/filter3d_oracle.py reproduces it bit for bit.  With f = 0, s' = s and rho3 = 1 exactly (s^2 normal).
@@ -467,7 +489,10 @@ __device__ __forceinline__ float warp_sum32_transposed(float* v)
 // adds d det(M^T M) and d det(M^T M + 0.3 I) to d cov2d before dM = 2 M G, so ds, dq and the camera path all see it.
 // F3D: 3D smoothing filter.  With g = d o3 (after the AA step), d sigma = g rho3 and
 // d s_raw_k = s_k (ds'_k (s_k / s'_k)) + (g o3) (f^2 / qf_k); f is held constant.
-template <int DEG, bool CAM, bool AA, bool F3D>
+// EXACT: exact gradient mode.  d xyz (and, with CAM, the camera gradient) gain the terms through J (dJ = V3x3^T (T^T dM),
+// back through fused_J to the view-space position and P00, P11) and through the SH view direction (reads sh_rest of the
+// active degree).  The other gradients are the same instructions as without it.
+template <int DEG, bool CAM, bool AA, bool F3D, bool EXACT>
 __global__ void project_backward_kernel(
     const int64_t* __restrict__ chunk_ids, const int* __restrict__ visible_num, const float* __restrict__ view,
     const float* __restrict__ proj, const float* __restrict__ pos, const float* __restrict__ scale,
@@ -475,7 +500,7 @@ __global__ void project_backward_kernel(
     int true_sigmoid, int accumulate, const float* __restrict__ grad /*[A*S,12]*/, const float* __restrict__ inv_scaler,
     float* __restrict__ g_pos, float* __restrict__ g_scale, float* __restrict__ g_rot, float* __restrict__ g_sh0,
     float* __restrict__ g_shr, float* __restrict__ g_opac, float* __restrict__ touched, float* __restrict__ cam_partials,
-    const float* __restrict__ filter_3d)
+    const float* __restrict__ filter_3d, const float* __restrict__ shr)
 {
     const int a = blockIdx.x, s = threadIdx.x;
     if (a >= visible_num[0]) {
@@ -549,12 +574,12 @@ __global__ void project_backward_kernel(
         }
         // cov2d backward: dT = 2 M G (VJ)^T (GR/transform.cu:861-880)
         float dT[9];
-        float dM[CAM ? 6 : 1];
+        float dM[(CAM || EXACT) ? 6 : 1];
 #pragma unroll
         for (int r = 0; r < 3; r++) {
             float dM0 = 2.f * (t.M[r * 2] * G[0] + t.M[r * 2 + 1] * G[2]);
             float dM1 = 2.f * (t.M[r * 2] * G[1] + t.M[r * 2 + 1] * G[3]);
-            if constexpr (CAM) { dM[r * 2] = dM0; dM[r * 2 + 1] = dM1; }
+            if constexpr (CAM || EXACT) { dM[r * 2] = dM0; dM[r * 2 + 1] = dM1; }
 #pragma unroll
             for (int k = 0; k < 3; k++) dT[r * 3 + k] = dM0 * t.VJ[k * 2] + dM1 * t.VJ[k * 2 + 1];
         }
@@ -595,6 +620,27 @@ __global__ void project_backward_kernel(
         float dv[4];
 #pragma unroll
         for (int k = 0; k < 4; k++) dv[k] = dh[0] * P[k * 4] + dh[1] * P[k * 4 + 1] + dh[2] * P[k * 4 + 2] + dh[3] * P[k * 4 + 3] + 0.f;
+        float dp00 = 0.f, dp11 = 0.f;
+        if constexpr (EXACT) {
+            // J term: dVJ = T^T dM, dJ[k][c] = sum_a V3[a][k] dVJ[a][c]; only J00, J11, J20, J21 depend on anything
+            float dVJ[6];
+#pragma unroll
+            for (int r = 0; r < 3; r++)
+#pragma unroll
+                for (int c = 0; c < 2; c++)
+                    dVJ[r * 2 + c] = t.R[r] * t.s[0] * dM[c] + t.R[3 + r] * t.s[1] * dM[2 + c] + t.R[6 + r] * t.s[2] * dM[4 + c];
+            const float dJ00 = Vm[0] * dVJ[0] + Vm[4] * dVJ[2] + Vm[8] * dVJ[4];
+            const float dJ11 = Vm[1] * dVJ[1] + Vm[5] * dVJ[3] + Vm[9] * dVJ[5];
+            const float dJ20 = Vm[2] * dVJ[0] + Vm[6] * dVJ[2] + Vm[10] * dVJ[4];
+            const float dJ21 = Vm[2] * dVJ[1] + Vm[6] * dVJ[3] + Vm[10] * dVJ[5];
+            const float tz = t.v[2];
+            const float rz = 1.0f / fmaxf(tz, 1e-2f), rz2 = rz * rz;
+            float dtz = 0.f, drz = 0.f;
+            dp00 = fused_J_axis_backward(P[0], (float)W, t.v[0], tz, rz, rz2, dJ00, dJ20, dv[0], dtz, drz);
+            dp11 = fused_J_axis_backward(P[5], (float)H, t.v[1], tz, rz, rz2, dJ11, dJ21, dv[1], dtz, drz);
+            if (!(tz < 1e-2f)) dtz -= rz2 * drz;             // below the depth floor rz is constant
+            dv[2] += dtz;
+        }
 #pragma unroll
         for (int k = 0; k < 3; k++) o_pos[k] = dv[0] * Vm[k * 4] + dv[1] * Vm[k * 4 + 1] + dv[2] * Vm[k * 4 + 2] + dv[3] * Vm[k * 4 + 3];
         if constexpr (CAM) {
@@ -604,6 +650,7 @@ __global__ void project_backward_kernel(
             for (int k = 0; k < 4; k++)
 #pragma unroll
                 for (int j = 0; j < 4; j++) { cam[k * 4 + j] = pt[k] * dv[j]; cam[16 + k * 4 + j] = t.v[k] * dh[j]; }
+            if constexpr (EXACT) { cam[16] += dp00; cam[21] += dp11; }
             // Sigma2 path through the V3x3 factor of M = T.V3x3.J, J frozen: dVJ = T^T dM, dV3[a][k] = sum_c dVJ[a][c] J[k][c]
             float J[6];
             fused_J(P, t.v, H, W, J);
@@ -620,6 +667,36 @@ __global__ void project_backward_kernel(
         // SH coefficients (GR/compact.cu:655-823); the direction is treated as constant
         lgs_sh_basis<DEG>(t.dirn[0], t.dirn[1], t.dirn[2], shb);
         dcol3[0] = dcol[0]; dcol3[1] = dcol[1]; dcol3[2] = dcol[2];
+        if constexpr (EXACT && DEG > 0) {
+            // SH direction term: w_k = sum_c sh[k][c] dcol_c, g_u = sum_k w_k d b_k / du, g_d = n (g_u - u (u . g_u)) with
+            // d = p - cc and n = 1 / sqrt(|d|^2 + 1e-12) as in project_chain; d xyz += g_d, d cc = -g_d
+            float w[K];
+            w[0] = 0.f;
+#pragma unroll
+            for (int k = 1; k < K; k++) {
+                const float* sk = shr + (size_t)(k - 1) * 3 * CS + src;
+                w[k] = sk[0] * dcol[0] + sk[CS] * dcol[1] + sk[2 * CS] * dcol[2];
+            }
+            float gu[3];
+            lgs_sh_basis_grad<DEG>(t.dirn[0], t.dirn[1], t.dirn[2], w, gu);
+            float cc[3];
+            lgs_camera_center(Vm, cc);
+            const float d0 = p[0] - cc[0], d1 = p[1] - cc[1], d2 = p[2] - cc[2];
+            const float dn = 1.0f / sqrtf(d0 * d0 + d1 * d1 + d2 * d2 + 1e-12f);
+            const float ug = t.dirn[0] * gu[0] + t.dirn[1] * gu[1] + t.dirn[2] * gu[2];
+            float gd[3];
+#pragma unroll
+            for (int m = 0; m < 3; m++) { gd[m] = dn * (gu[m] - t.dirn[m] * ug); o_pos[m] += gd[m]; }
+            if constexpr (CAM) {
+                // cc_m = sum_k (-V[3][k]) V[m][k]: d V[3][k] += sum_m g_d[m] V[m][k], d V[m][k] += g_d[m] V[3][k]
+#pragma unroll
+                for (int k = 0; k < 3; k++) {
+                    cam[12 + k] += gd[0] * Vm[k] + gd[1] * Vm[4 + k] + gd[2] * Vm[8 + k];
+#pragma unroll
+                    for (int m = 0; m < 3; m++) cam[m * 4 + k] += gd[m] * Vm[12 + k];
+                }
+            }
+        }
     }
     if constexpr (CAM) {
         // chunk sum in a fixed order: warps by the transposing butterfly, then warp 0..nw-1 in sequence (S % 32 == 0)
@@ -702,6 +779,19 @@ __global__ void __launch_bounds__(1024) camera_grad_sum_kernel(const float* __re
     }
 }
 
+// Largest block an EXACT instantiation can be launched with.  The kernel has no launch bounds (the default instantiations
+// must keep their code), and the heaviest EXACT ones use up to 168 registers, which allows 384 threads instead of 1024
+// (DESIGN.md section 1, "Exact gradient mode").  Read once per instantiation, on its first (eager) use.
+template <int DEG, bool CAM, bool AA, bool F3D>
+static int project_backward_exact_max_threads()
+{
+    static const int n = [] {
+        cudaFuncAttributes a;
+        return cudaFuncGetAttributes(&a, project_backward_kernel<DEG, CAM, AA, F3D, true>) == cudaSuccess ? a.maxThreadsPerBlock : 0;
+    }();
+    return n;
+}
+
 // mode 0: outputs are compacted [..,A,S] and assigned; mode 1: same, cleared first (rows of chunks >= *visible_num and
 // sh_rest rows above the active degree must read as zero); mode 2: outputs are the DENSE [..,C,S] gradient tensors and
 // this view's gradients are accumulated into them (the multi-view / data-parallel path: no compacted round trip).
@@ -711,7 +801,8 @@ extern "C" int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_
                                     int rest_dim, int img_h, int img_w, int true_sigmoid_grad, const float* packed_grad,
                                     const float* grad_inv_scaler, int zero_outputs, float* g_position, float* g_scale,
                                     float* g_rotation, float* g_sh_base, float* g_sh_rest, float* g_opacity, float* touched,
-                                    float* cam_partials, float* d_cam, const float* filter_3d, int antialiased, void* stream)
+                                    float* cam_partials, float* d_cam, const float* filter_3d, int antialiased,
+                                    const float* sh_base, const float* sh_rest, int exact_grad, void* stream)
 {
     LGS_REQUIRE(sh_degree >= 0 && sh_degree <= 3, "project_backward: sh_degree %d not in 0..3", sh_degree);
     LGS_REQUIRE(rest_dim >= (sh_degree + 1) * (sh_degree + 1) - 1, "project_backward: sh_rest has %d rows, degree %d needs %d", rest_dim,
@@ -720,6 +811,9 @@ extern "C" int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_
     const bool cam = d_cam != nullptr;
     LGS_REQUIRE((cam_partials != nullptr) == cam, "project_backward: cam_partials and d_cam are both given or both NULL");
     LGS_REQUIRE(!cam || S % 32 == 0, "project_backward: the camera gradient needs a chunk size that is a multiple of 32, got %d", S);
+    LGS_REQUIRE(!exact_grad || sh_degree == 0 || sh_rest != nullptr, "project_backward: exact_grad at SH degree %d needs sh_rest",
+                sh_degree);
+    (void)sh_base;                                  // the constant band has no direction term
     cudaStream_t st = (cudaStream_t)stream;
     if (A == 0) {
         if (cam) LGS_CUDA(cudaMemsetAsync(d_cam, 0, 32 * sizeof(float), st));
@@ -735,17 +829,26 @@ extern "C" int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_
         LGS_CUDA(cudaMemsetAsync(g_sh_rest, 0, sizeof(float) * (size_t)rest_dim * 3 * AS, st));
         LGS_CUDA(cudaMemsetAsync(g_opacity, 0, sizeof(float) * AS, st));
     }
-#define PB(D, K, AA, F3) project_backward_kernel<D, K, AA, F3><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num, view_matrix,    \
-        proj_matrix, position, scale, rotation, opacity, C, S, A, rest_dim, img_h, img_w, true_sigmoid_grad, accumulate, packed_grad,  \
-        grad_inv_scaler, g_position, g_scale, g_rotation, g_sh_base, g_sh_rest, g_opacity, touched, cam_partials, filter_3d)
-#define PB_DEG(K, AA, F3) switch (sh_degree) { case 0: PB(0, K, AA, F3); break; case 1: PB(1, K, AA, F3); break;                      \
-                                               case 2: PB(2, K, AA, F3); break; default: PB(3, K, AA, F3); }
-#define PB_CAM(AA, F3) if (cam) { PB_DEG(true, AA, F3) } else { PB_DEG(false, AA, F3) }
-    if (filter_3d != nullptr) {
-        if (antialiased) { PB_CAM(true, true) } else { PB_CAM(false, true) }
-    } else {
-        if (antialiased) { PB_CAM(true, false) } else { PB_CAM(false, false) }
+#define PB(D, K, AA, F3, EX) {                                                                                                      \
+        if constexpr (EX) {                                                                                                         \
+            const int mt = project_backward_exact_max_threads<D, K, AA, F3>();                                                      \
+            LGS_REQUIRE(S <= mt, "project_backward: exact_grad with this configuration supports chunk sizes up to %d, got %d", mt, S); \
+        }                                                                                                                           \
+        project_backward_kernel<D, K, AA, F3, EX><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num,                            \
+        view_matrix, proj_matrix, position, scale, rotation, opacity, C, S, A, rest_dim, img_h, img_w, true_sigmoid_grad, accumulate,  \
+        packed_grad, grad_inv_scaler, g_position, g_scale, g_rotation, g_sh_base, g_sh_rest, g_opacity, touched, cam_partials,        \
+        filter_3d, sh_rest); }
+#define PB_DEG(K, AA, F3, EX) switch (sh_degree) { case 0: PB(0, K, AA, F3, EX); break; case 1: PB(1, K, AA, F3, EX); break;          \
+                                                   case 2: PB(2, K, AA, F3, EX); break; default: PB(3, K, AA, F3, EX); }
+#define PB_CAM(AA, F3, EX) if (cam) { PB_DEG(true, AA, F3, EX) } else { PB_DEG(false, AA, F3, EX) }
+#define PB_MODE(EX)                                                                                                                 \
+    if (filter_3d != nullptr) {                                                                                                     \
+        if (antialiased) { PB_CAM(true, true, EX) } else { PB_CAM(false, true, EX) }                                                \
+    } else {                                                                                                                        \
+        if (antialiased) { PB_CAM(true, false, EX) } else { PB_CAM(false, false, EX) }                                              \
     }
+    if (exact_grad) { PB_MODE(true) } else { PB_MODE(false) }
+#undef PB_MODE
 #undef PB_CAM
 #undef PB_DEG
 #undef PB

@@ -30,6 +30,39 @@ __device__ __forceinline__ void lgs_sh_basis(float x, float y, float z, float* b
     }
 }
 
+// g = sum_k w[k] * d b_k / d(x, y, z) for k = 1 .. (DEG+1)^2 - 1 (b_0 is constant), the polynomial derivatives of
+// lgs_sh_basis at the point (x, y, z) (not projected onto the sphere: the caller applies the normalisation's Jacobian).
+template <int DEG>
+__device__ __forceinline__ void lgs_sh_basis_grad(float x, float y, float z, const float* w, float* g)
+{
+    g[0] = 0.f; g[1] = 0.f; g[2] = 0.f;
+    if constexpr (DEG > 0) {
+        const float C1 = 0.4886025119029199f;
+        g[0] -= C1 * w[3]; g[1] -= C1 * w[1]; g[2] += C1 * w[2];
+        if constexpr (DEG > 1) {
+            const float C20 = 1.0925484305920792f, C22 = 0.31539156525252005f, C24 = 0.5462742152960396f;
+            g[0] += C20 * (y * w[4] - z * w[7]) + 2.0f * x * (C24 * w[8] - C22 * w[6]);
+            g[1] += C20 * (x * w[4] - z * w[5]) - 2.0f * y * (C22 * w[6] + C24 * w[8]);
+            g[2] += -C20 * (y * w[5] + x * w[7]) + 4.0f * C22 * z * w[6];
+            if constexpr (DEG > 2) {
+                const float C30 = -0.5900435899266435f, C31 = 2.890611442640554f, C32 = -0.4570457994644658f;
+                const float C33 = 0.3731763325901154f, C34 = -0.4570457994644658f, C35 = 1.445305721320277f;
+                const float C36 = -0.5900435899266435f;
+                // __fmul_rn: products the compiler cannot share with lgs_sh_basis's, whose FMA contraction (and so the sh_rest
+                // gradient) must not depend on whether this function is called
+                const float xx = __fmul_rn(x, x), yy = __fmul_rn(y, y), zz = __fmul_rn(z, z);
+                const float xy = __fmul_rn(x, y), yz = __fmul_rn(y, z), xz = __fmul_rn(x, z);
+                g[0] += 6.0f * C30 * xy * w[9] + C31 * yz * w[10] - 2.0f * C32 * xy * w[11] - 6.0f * C33 * xz * w[12] +
+                        C34 * (4.0f * zz - 3.0f * xx - yy) * w[13] + 2.0f * C35 * xz * w[14] + 3.0f * C36 * (xx - yy) * w[15];
+                g[1] += 3.0f * C30 * (xx - yy) * w[9] + C31 * xz * w[10] + C32 * (4.0f * zz - xx - 3.0f * yy) * w[11] -
+                        6.0f * C33 * yz * w[12] - 2.0f * C34 * xy * w[13] - 2.0f * C35 * yz * w[14] - 6.0f * C36 * xy * w[15];
+                g[2] += C31 * xy * w[10] + 8.0f * C32 * yz * w[11] + C33 * (6.0f * zz - 3.0f * xx - 3.0f * yy) * w[12] +
+                        8.0f * C34 * xz * w[13] + C35 * (xx - yy) * w[14];
+            }
+        }
+    }
+}
+
 // camera centre = -t . R^T with t = V[3,:3], R = V[:3,:3]   (GR/compact.cu:875-879)
 __device__ __forceinline__ void lgs_camera_center(const float* __restrict__ Vm, float* c)
 {

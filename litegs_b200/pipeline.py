@@ -213,7 +213,7 @@ def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_exte
 def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_trans: Optional[torch.Tensor] = None,
                          enable_statistic: bool = False, specific_tiles: Optional[torch.Tensor] = None,
                          accumulate_into: Optional[dict] = None, clamped_img: Optional[torch.Tensor] = None,
-                         camera_grad: Optional[torch.Tensor] = None):
+                         camera_grad: Optional[torch.Tensor] = None, exact_grad: bool = False):
     """Backward of one view: d_img f32[1,3,Hp,Wp] (padded) -> compacted parameter gradients
     (xyz[3,A,S], scale[3,A,S], rot[4,A,S], sh_0[1,3,A,S], sh_rest[R,3,A,S], opacity[1,A,S]) with
     A = state.n_chunks_visible, plus packed_grad (whose slot 9 carries the statistics term).
@@ -223,7 +223,10 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
     (returns (None, packed_grad)).  An optional "_touched" entry (f32[C]) receives 1 at every visible chunk.
 
     camera_grad: optional contiguous f32[2,4,4] CUDA tensor that receives (d view_matrix, d proj_matrix) of this view, with
-    J and the SH view direction held constant (DESIGN.md section 1).  It is assigned, not accumulated."""
+    J and the SH view direction held constant (DESIGN.md section 1).  It is assigned, not accumulated.
+
+    exact_grad: exact gradient mode (DESIGN.md section 1): the xyz gradient and camera_grad also carry the terms through the
+    ray-space Jacobian J and through the SH view direction.  The other gradients and the forward do not depend on it."""
     xyz = params["xyz"]
     dev = xyz.device
     C, S = xyz.shape[-2:]
@@ -244,6 +247,7 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
         st = _stream(dev)
         cam_partials = None if camera_grad is None else torch.empty((max(A, 1), 32), dtype=_F32, device=dev)
         cam_args = (_ptr(cam_partials), _ptr(camera_grad))
+        exact_args = (_ptr(params["sh_0"]), _ptr(params["sh_rest"]), int(bool(exact_grad)))
         pg = torch.empty((1, Nmax, 12), dtype=_F32, device=dev)
         if specific_tiles is None:
             specific_tiles = state.tile_order          # every tile, longest lists first (None = index order)
@@ -263,7 +267,7 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
                           _ptr(state.view), _ptr(state.proj), _ptr(xyz), _ptr(params["scale"]), _ptr(params["rot"]),
                           _ptr(params["opacity"]), C, S, A, R, H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(pg), None, 2,
                           _ptr(d["xyz"]), _ptr(d["scale"]), _ptr(d["rot"]), _ptr(d["sh_0"]), _ptr(d["sh_rest"]), _ptr(d["opacity"]),
-                          _ptr(d.get("_touched")), *cam_args, _ptr(state.filter_3d), int(state.antialiased), st)   # "_touched": chunk marks for the fused optimizer step
+                          _ptr(d.get("_touched")), *cam_args, _ptr(state.filter_3d), int(state.antialiased), *exact_args, st)   # "_touched": chunk marks for the fused optimizer step
             elif camera_grad is not None:
                 camera_grad.zero_()
             return None, pg
@@ -278,7 +282,7 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
             _lib.call("lgs_project_backward", state.sh_degree, _ptr(state.chunk_ids), ctypes.c_void_p(state.counters.data_ptr()),
                       _ptr(state.view), _ptr(state.proj), _ptr(xyz), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["opacity"]),
                       C, S, A, R, H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(pg), None, 0, _ptr(g_pos), _ptr(g_sc), _ptr(g_rot),
-                      _ptr(g_s0), _ptr(g_sr), _ptr(g_op), None, *cam_args, _ptr(state.filter_3d), int(state.antialiased), st)
+                      _ptr(g_s0), _ptr(g_sr), _ptr(g_op), None, *cam_args, _ptr(state.filter_3d), int(state.antialiased), *exact_args, st)
         elif camera_grad is not None:
             camera_grad.zero_()
     return [g_pos, g_sc, g_rot, g_s0, g_sr, g_op], pg
@@ -383,7 +387,7 @@ class ViewWorkspace:
         if order:
             _lib.call("lgs_tile_order", _ptr(self.work), 1, self.ntile, _ptr(self.tile_order), st)
 
-    def _backward_kernels(self, params, sh_degree, accumulate_into, use_clamp, camera_grad, antialiased, filter_3d):
+    def _backward_kernels(self, params, sh_degree, accumulate_into, use_clamp, camera_grad, antialiased, filter_3d, exact_grad):
         st = _stream(self.dev)
         H, W = self.hw
         th, tw = self.tile
@@ -400,7 +404,7 @@ class ViewWorkspace:
                   H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(self.pg), None, 2, _ptr(d["xyz"]), _ptr(d["scale"]), _ptr(d["rot"]),
                   _ptr(d["sh_0"]), _ptr(d["sh_rest"]), _ptr(d["opacity"]), _ptr(d.get("_touched")),
                   _ptr(self.cam_partials) if camera_grad else None, _ptr(self.d_cam) if camera_grad else None, _ptr(filter_3d),
-                  int(antialiased), st)
+                  int(antialiased), _ptr(params["sh_0"]), _ptr(params["sh_rest"]), int(exact_grad), st)
 
     def _run(self, kind, sig, fn):
         """Eager the first time a pointer signature is seen, captured into a CUDA graph the second time, replayed afterwards."""
@@ -441,10 +445,12 @@ class ViewWorkspace:
         self.views_done += 1
         return self.img
 
-    def backward(self, params, d_img, sh_degree, accumulate_into, use_clamp=True, camera_grad=None, antialiased=False, filter_3d=None):
+    def backward(self, params, d_img, sh_degree, accumulate_into, use_clamp=True, camera_grad=None, antialiased=False, filter_3d=None,
+                 exact_grad=False):
         """d_img f32[1,3,H,W] or [1,3,Hp,Wp]: gradient of the loss w.r.t. the (clamped) image.  camera_grad (optional f32[2,4,4]
         CUDA tensor) receives (d view_matrix, d proj_matrix) of this view, copied on the stream after the backward.
-        antialiased, filter_3d: the values the forward of this view was given."""
+        antialiased, filter_3d: the values the forward of this view was given.  exact_grad: exact gradient mode (DESIGN.md
+        section 1); a backward-only choice, so it is part of the backward graph's signature and of nothing else."""
         filter_3d = check_filter_3d(filter_3d, params["xyz"])
         if camera_grad is not None and not (camera_grad.is_cuda and camera_grad.dtype == _F32 and tuple(camera_grad.shape) == (2, 4, 4)):
             raise RuntimeError("camera_grad must be a float32 CUDA tensor of shape [2,4,4]")
@@ -458,9 +464,11 @@ class ViewWorkspace:
         sig = (tuple(params[k].data_ptr() for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")),
                tuple(accumulate_into[k].data_ptr() for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")),
                0 if accumulate_into.get("_touched") is None else accumulate_into["_touched"].data_ptr(), int(sh_degree), bool(use_clamp),
-               bool(CONFIG["tile_order"]), bool(antialiased), 0 if filter_3d is None else filter_3d.data_ptr(), camera_grad is not None)
+               bool(CONFIG["tile_order"]), bool(antialiased), 0 if filter_3d is None else filter_3d.data_ptr(), bool(exact_grad),
+               camera_grad is not None)
         cam = camera_grad is not None
-        self._run("bwd", sig, lambda: self._backward_kernels(params, sh_degree, accumulate_into, use_clamp, cam, antialiased, filter_3d))
+        self._run("bwd", sig, lambda: self._backward_kernels(params, sh_degree, accumulate_into, use_clamp, cam, antialiased, filter_3d,
+                                                             bool(exact_grad)))
         if cam:
             camera_grad.copy_(self.d_cam, non_blocking=True)
 

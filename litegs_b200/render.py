@@ -69,10 +69,14 @@ def render(view_matrix, proj_matrix, xyz, scale, rot, color, opacity,
            valid_length, feedback_binning_allocate_size, idx_tensor,
            actived_sh_degree: int, output_shape, pp):
     """Projection -> binning -> rasterisation; returns (img, transmittance, depth, normal, primitive_visible)
-    as render/__init__.py:50-94.  The antialiased mode exists on the fused path only (render_view, render_views)."""
+    as render/__init__.py:50-94.  The antialiased and exact gradient modes exist on the fused path only (render_view,
+    render_views)."""
     if getattr(pp, "antialiased", False):
         raise RuntimeError("pp.antialiased is set, but the op-by-op render() has no antialiased mode and would draw every splat "
                            "without its opacity compensation; render through render_view or render_views instead")
+    if getattr(pp, "exact_grad", False):
+        raise RuntimeError("pp.exact_grad is set, but the op-by-op render() has no exact gradient mode and would return position "
+                           "gradients with J and the SH direction held constant; render through render_view or render_views instead")
     nvtx.range_push("Proj")
     view_pos, ndc_pos = wrapper.MVPTransform.apply(xyz, view_matrix, proj_matrix, valid_length)
     transform_matrix = wrapper.CreateTransformMatrix.call_fused(scale, rot, valid_length)
@@ -134,7 +138,7 @@ class _RenderViewFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, xyz, scale, rot, sh_0, sh_rest, opacity, cluster_origin, cluster_extend, frustumplane,
                 view_matrix, proj_matrix, sh_degree, H, W, th, tw, sparse_grad, enable_transmitance, accumulate_into, antialiased,
-                filter_3d):
+                filter_3d, exact_grad):
         params = dict(xyz=xyz, scale=scale, rot=rot, sh_0=sh_0, sh_rest=sh_rest, opacity=opacity)
         stat = bool(StatisticsHelperInst.bStart)
         ctx.set_materialize_grads(False)       # an unused transmittance output must not cost a zero-filled gradient image
@@ -148,6 +152,7 @@ class _RenderViewFn(torch.autograd.Function):
         ctx.sparse = bool(sparse_grad)
         ctx.trans = bool(enable_transmitance)
         ctx.accumulate_into = accumulate_into
+        ctx.exact_grad = bool(exact_grad)           # backward only: the forward does not depend on it
         ctx.save_for_backward(xyz, scale, rot, sh_0, sh_rest, opacity, img)
         ctx.mark_non_differentiable(state.last)
         return img, state.T, state.last
@@ -166,7 +171,8 @@ class _RenderViewFn(torch.autograd.Function):
             cam = torch.empty((2, 4, 4), dtype=torch.float32, device=xyz.device)
         grads, pg = pipeline.render_view_backward(params, state, g_img, g_T if (ctx.trans and g_T is not None) else None,
                                                   enable_statistic=ctx.stat,
-                                                  accumulate_into=ctx.accumulate_into, clamped_img=img_out, camera_grad=cam)
+                                                  accumulate_into=ctx.accumulate_into, clamped_img=img_out, camera_grad=cam,
+                                                  exact_grad=ctx.exact_grad)
         if ctx.stat:
             _feed_statistics(state, ctx.stats, pg, state.tile)
         g_view = g_proj = None
@@ -175,7 +181,7 @@ class _RenderViewFn(torch.autograd.Function):
             g_proj = cam[1].reshape(state.proj.shape) if ctx.needs_input_grad[10] else None
         if grads is None:          # gradients went straight into the caller's dense buffers
             ctx.state = None
-            return (None,) * 9 + (g_view, g_proj) + (None,) * 10
+            return (None,) * 9 + (g_view, g_proj) + (None,) * 11
         C, S = xyz.shape[-2:]
         ids = state.chunk_ids[: state.n_chunks_visible]
         out = []
@@ -183,7 +189,7 @@ class _RenderViewFn(torch.autograd.Function):
             ct = CompactedTensor((*g.shape[:-2], C, S), ids, g)
             out.append(ct if ctx.sparse else ct.to_dense())
         ctx.state = None
-        return (*out, None, None, None, g_view, g_proj, None, None, None, None, None, None, None, None, None, None)
+        return (*out, None, None, None, g_view, g_proj, None, None, None, None, None, None, None, None, None, None, None)
 
 
 def render_view(cluster_origin, cluster_extend, frustumplane, view_matrix, proj_matrix,
@@ -196,6 +202,8 @@ def render_view(cluster_origin, cluster_extend, frustumplane, view_matrix, proj_
     tensors -- or, with ``accumulate_into`` (dict of dense gradient tensors, e.g. ``GradAccumulator.grads()``), are
     ADDED into those buffers by the backward kernel itself and ``param.grad`` stays untouched (multi-view batches,
     data-parallel training).  ``pp.antialiased`` (absent = False) selects the antialiased mode (DESIGN.md section 1).
+    ``pp.exact_grad`` (absent = False) selects the exact gradient mode (DESIGN.md section 1): the xyz and camera gradients also
+    carry the terms through the ray-space Jacobian J and the SH view direction.
     ``filter_3d`` (f32[1,C,S] or None): Mip-Splatting's 3D smoothing filter (scene.filter_3d_device, DESIGN.md section 1); it is
     an input without a gradient."""
     if not pp.cluster_size:
@@ -204,7 +212,8 @@ def render_view(cluster_origin, cluster_extend, frustumplane, view_matrix, proj_
     th, tw = int(pp.tile_size[0]), int(pp.tile_size[1])
     img, T, last = _RenderViewFn.apply(xyz, scale, rot, sh_0, sh_rest, opacity, cluster_origin, cluster_extend, frustumplane,
                                        view_matrix, proj_matrix, int(actived_sh_degree), H, W, th, tw, pp.sparse_grad,
-                                       pp.enable_transmitance, accumulate_into, bool(getattr(pp, "antialiased", False)), filter_3d)
+                                       pp.enable_transmitance, accumulate_into, bool(getattr(pp, "antialiased", False)), filter_3d,
+                                       bool(getattr(pp, "exact_grad", False)))
     img = img[..., :H, :W]          # already clamped to [0,1] by the kernel
     trans = T[..., :H, :W] if pp.enable_transmitance else None
     return img, trans, None, None, last
@@ -259,6 +268,7 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
     H, W = int(output_shape[0]), int(output_shape[1])
     th, tw = int(pp.tile_size[0]), int(pp.tile_size[1])
     aa = bool(getattr(pp, "antialiased", False))
+    exact = bool(getattr(pp, "exact_grad", False))
     direct = loss_and_grad_fn is not None or _DIRECT_VIEWS
     if direct:
         params = dict(xyz=xyz.detach(), scale=scale.detach(), rot=rot.detach(), sh_0=sh_0.detach(), sh_rest=sh_rest.detach(),
@@ -284,7 +294,7 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
         if wait_ev is not None:
             torch.cuda.current_stream(dev).wait_event(wait_ev)
         _, pg_ = pipeline.render_view_backward(params, state, d_img, None, enable_statistic=stat, accumulate_into=accumulate_into,
-                                               clamped_img=img_p, camera_grad=slot(i))
+                                               clamped_img=img_p, camera_grad=slot(i), exact_grad=exact)
         if stat:
             _feed_statistics(state, stats, pg_, (th, tw))
         losses.append(loss.detach())
@@ -334,7 +344,7 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
         if wait_ev is not None:
             torch.cuda.current_stream(dev).wait_event(wait_ev)
         ws.backward(params, d_img, int(actived_sh_degree), accumulate_into, use_clamp=True, camera_grad=slot(i), antialiased=aa,
-                    filter_3d=filter_3d)
+                    filter_3d=filter_3d, exact_grad=exact)
         losses.append(loss.detach())
 
     def one_probe(i, wait_ev):
