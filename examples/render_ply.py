@@ -3,9 +3,12 @@
     python examples/render_ply.py --ply point_cloud.ply --out /tmp/renders --views 8 [--colmap /path/to/colmap]
     python examples/render_ply.py --make /tmp/demo.ply --out /tmp/renders        # writes a synthetic cloud first
     python examples/render_ply.py --ply mip_splatting.ply --filter-3d --antialiased    # a Mip-Splatting checkpoint
+    python examples/render_ply.py --make /tmp/demo.ply --out /tmp/renders --depth      # also depth maps (e.g. for TSDF fusion)
 
 Cameras: the poses of a COLMAP model when --colmap is given, else the Fibonacci lattice of scene.make_camera.  Forward only
-(the reference's example_metrics.py path): project -> bin -> sort -> composite, no gradients kept.
+(the reference's example_metrics.py path): project -> bin -> sort -> composite, no gradients kept.  With --depth each view also
+writes <name>_depth.npy (D = sum w z, the accumulated view-space depth, f32[H,W]) and <name>_alpha.npy (1 - T, f32[H,W]); the
+expected depth is D / alpha where alpha > 0.
 """
 import argparse
 import os
@@ -34,6 +37,7 @@ def main():
                     help="opacity compensation of the 2D filter (for models trained in that mode, or renders at another resolution)")
     ap.add_argument("--filter-3d", action="store_true",
                     help="apply the file's filter_3D property (Mip-Splatting's 3D smoothing filter); the file must have it")
+    ap.add_argument("--depth", action="store_true", help="also write the accumulated depth D and 1 - T of each view as .npy")
     a = ap.parse_args()
     path = a.ply
     if a.make:
@@ -62,20 +66,25 @@ def main():
         cams = [(scene.make_camera(i, a.views, a.width, a.height), (a.height, a.width), f"view_{i:04d}.png") for i in range(a.views)]
     import PIL.Image
     os.makedirs(a.out, exist_ok=True)
-    imgs = []
+    imgs, depths = [], []
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     with torch.no_grad():
         for cam, hw, _ in cams:
             c = {k: torch.from_numpy(v).to(dev) for k, v in cam.items()}
-            img, _, _ = pipeline.render_view_forward(P, A[0], A[1], c["frustumplane"], c["view"], c["proj"], a.sh_degree, hw, (8, 16),
-                                                     clamp_zero=True, antialiased=a.antialiased, filter_3d=filt)
+            img, st, _ = pipeline.render_view_forward(P, A[0], A[1], c["frustumplane"], c["view"], c["proj"], a.sh_degree, hw, (8, 16),
+                                                      clamp_zero=True, antialiased=a.antialiased, filter_3d=filt, render_depth=a.depth)
             imgs.append(img[0, :, : hw[0], : hw[1]])
+            if a.depth:
+                depths.append((st.depth[0, 0, : hw[0], : hw[1]], 1.0 - st.T[0, 0, : hw[0], : hw[1]]))
     torch.cuda.synchronize()
     dt = time.perf_counter() - t0
     for (cam, hw, name), img in zip(cams, imgs):
         PIL.Image.fromarray((img.permute(1, 2, 0) * 255.0 + 0.5).clamp(0, 255).to(torch.uint8).cpu().numpy()).save(
             os.path.join(a.out, os.path.splitext(name)[0] + ".png"))
+    for (_, _, name), (d, alpha) in zip(cams, depths):
+        np.save(os.path.join(a.out, os.path.splitext(name)[0] + "_depth.npy"), d.cpu().numpy())
+        np.save(os.path.join(a.out, os.path.splitext(name)[0] + "_alpha.npy"), alpha.cpu().numpy())
     print(f"{g['n_points']} Gaussians, {len(cams)} views rendered in {dt * 1e3:.1f} ms ({len(cams) / dt:.0f} views/s forward only) -> {a.out}")
 
 

@@ -4,11 +4,15 @@
     python examples/train_colmap.py --data /path/to/colmap --iters 2000
     python examples/train_colmap.py --make /tmp/noisy --pose-noise 1 0.02 --refine-poses     # learn the camera poses too
     python examples/train_colmap.py --make /tmp/noisy --pose-noise 1 0.02 --refine-poses --exact-grad   # ... with the J and SH terms
+    python examples/train_colmap.py --make /tmp/synth_depth --depth-weight 0.1     # also supervise the expected depth
 
 Reads ``sparse/0/{cameras,images,points3D}.bin`` and ``images/*`` (litegs_b200.colmap; same files and conventions as the
 reference's ``litegs/io_manager/colmap.py`` + ``litegs/data.py``), initialises Gaussians from the SfM points the way
 ``litegs/scene/point.py:7-19`` does, and trains appearance + geometry with the fused L1+SSIM loss and the fused Adam step.
 No densification (that policy is out of scope, SURVEY 2.1): the point count stays what COLMAP delivered.
+With ``--depth-weight W`` and a ``depths/`` directory beside ``images/`` (``depths/<image stem>.npy``, f32[H,W] expected depth,
+NaN where unknown -- ``--make`` writes the hidden scene's), the loss gains W * mean |ED - target| over the known pixels, with
+ED = D / (1 - T) from the depth mode (DESIGN.md section 1, "Depth").
 """
 import argparse
 import os
@@ -33,23 +37,31 @@ def make_dataset(root, n_gaussians=60_000, n_views=24, hw=(270, 480), n_points=2
     axis and a translation of that fraction of the camera's distance, as noisy SfM poses are; the images stay exact."""
     dev = dev or torch.device("cuda:0")
     H, W = hw
-    pp = PipelineParams(tile_size=(8, 16), sparse_grad=True)
+    pp = PipelineParams(tile_size=(8, 16), sparse_grad=True, render_depth=True, enable_transmitance=True)
     truth = scene.make_scene(n_gaussians, sh_degree=3, seed=seed, log_scale_range=log_scale_range)
     T = {k: torch.from_numpy(truth[k]).to(dev) for k in PARAM_ORDER}
     A = [torch.from_numpy(truth[k]).to(dev) for k in ("cluster_origin", "cluster_extend")]
 
+    eds = {}
+
     def render_fn(i, cam):
         c = {k: torch.from_numpy(v).to(dev) for k, v in cam.items()}
         with torch.no_grad():
-            img = render.render_view(A[0], A[1], c["frustumplane"], c["view"], c["proj"], T["xyz"], T["scale"], T["rot"], T["sh_0"],
-                                     T["sh_rest"], T["opacity"], 3, (H, W), pp)[0]
+            img, trans, depth, _, _ = render.render_view(A[0], A[1], c["frustumplane"], c["view"], c["proj"], T["xyz"], T["scale"], T["rot"],
+                                                         T["sh_0"], T["sh_rest"], T["opacity"], 3, (H, W), pp)
+            alpha = 1.0 - trans[0, 0]
+            # the hidden scene's expected depth where it is mostly opaque, unknown elsewhere
+            eds[i] = torch.where(alpha > 0.5, depth[0, 0] / alpha.clamp_min(0.5), torch.full_like(alpha, float("nan"))).cpu().numpy()
         return (img[0].permute(1, 2, 0) * 255.0 + 0.5).clamp(0, 255).to(torch.uint8).cpu().numpy()
 
     rng = np.random.default_rng(seed + 7)
     xyz = truth["xyz"].reshape(3, -1).T
     sel = rng.choice(xyz.shape[0], size=min(n_points, xyz.shape[0]), replace=False)
     rgb = np.clip((truth["sh_0"].reshape(3, -1).T[sel] * colmap.SH_C0 + 0.5) * 255.0, 0, 255).astype(np.uint8)
-    colmap.write_synthetic_dataset(root, xyz[sel].astype(np.float64), rgb, n_views, W, H, render_fn=render_fn)
+    names = colmap.write_synthetic_dataset(root, xyz[sel].astype(np.float64), rgb, n_views, W, H, render_fn=render_fn)
+    os.makedirs(os.path.join(root, "depths"), exist_ok=True)
+    for i, name in enumerate(names):
+        np.save(os.path.join(root, "depths", os.path.splitext(name)[0] + ".npy"), eds[i].astype(np.float32))
     if pose_noise is not None:
         deg, frac = pose_noise
         cams, images, pts = colmap.read_model(root)
@@ -85,14 +97,48 @@ def load_dataset(root, image_dir="images", dev=None):
     return frames, np.stack([p.xyz for p in P]), np.stack([p.rgb for p in P])
 
 
-def train(root, iters=300, views_per_step=8, log=print, refine_poses=False, antialiased=False, filter_3d=False, exact_grad=False):
+def load_depths(root, dev=None):
+    """Expected-depth targets f32[1,1,H,W] (NaN = unknown) aligned with load_dataset's frames, from root/depths/<image stem>.npy;
+    None when the dataset has no depths directory."""
+    if not os.path.isdir(os.path.join(root, "depths")):
+        return None
+    dev = dev or torch.device("cuda:0")
+    cams, images, _ = colmap.read_model(root)
+    out = []
+    for im in sorted(images.values(), key=lambda v: v.name):
+        if cams[im.camera_id].model != "PINHOLE":
+            continue
+        d = np.load(os.path.join(root, "depths", os.path.splitext(im.name)[0] + ".npy")).astype(np.float32)
+        out.append(torch.from_numpy(d).to(dev)[None, None].contiguous())
+    return out
+
+
+def depth_loss_and_grad(depth, trans, target, weight, upstream=1.0):
+    """weight * mean |ED - target| over the pixels with a finite target and 1 - T > 1e-3, ED = depth / (1 - trans) ->
+    (loss, d_depth, d_trans), each gradient scaled by upstream."""
+    alpha = 1.0 - trans
+    valid = torch.isfinite(target) & (alpha > 1e-3)
+    n = valid.sum().clamp_min(1)
+    a = alpha.clamp_min(1e-3)
+    ed = depth / a
+    r = torch.where(valid, ed - torch.nan_to_num(target), torch.zeros_like(ed))
+    loss = weight * r.abs().sum() / n
+    g_ed = torch.where(valid, torch.sign(r), torch.zeros_like(r)) * (weight * upstream / n)
+    return loss, g_ed / a, g_ed * ed / a
+
+
+def train(root, iters=300, views_per_step=8, log=print, refine_poses=False, antialiased=False, filter_3d=False, exact_grad=False,
+          depth_weight=0.0, metrics=None):
+    """Returns (loss history, PSNR).  depth_weight > 0 adds the expected-depth term (the dataset must have depths/).
+    metrics (a dict, optional) receives "ed_error": mean |ED - target| over the known pixels of 8 training views, when the
+    dataset has depths."""
     from litegs_b200 import fused
     if refine_poses and int(os.environ.get("WORLD_SIZE", "1")) > 1:
         raise ValueError("--refine-poses runs on one GPU: multi-GPU pose refinement is not supported")
     keep = fused.CONFIG["true_sigmoid_grad"]
     fused.CONFIG["true_sigmoid_grad"] = True               # our own loops train with the true sigmoid derivative (SURVEY Q15)
     try:
-        return _train(root, iters, views_per_step, log, refine_poses, antialiased, filter_3d, exact_grad)
+        return _train(root, iters, views_per_step, log, refine_poses, antialiased, filter_3d, exact_grad, depth_weight, metrics)
     finally:
         fused.CONFIG["true_sigmoid_grad"] = keep
 
@@ -129,17 +175,22 @@ class _Poses:
         self.opt.step()
 
 
-def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=False, filter_3d=False, exact_grad=False):
+def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=False, filter_3d=False, exact_grad=False,
+           depth_weight=0.0, metrics=None):
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", 0)))
     torch.cuda.set_device(dev)
     frames, xyz, rgb = load_dataset(root, dev=dev)
+    targets = load_depths(root, dev=dev)
+    if depth_weight > 0 and targets is None:
+        raise ValueError(f"--depth-weight needs expected-depth targets in {os.path.join(root, 'depths')}")
+    use_depth = depth_weight > 0
     H, W = frames[0][2]
     poses = _Poses(frames, (H, W), dev) if refine_poses else None
     extr0 = poses.extr.detach().clone() if poses else None
     cgrads = torch.empty((views_per_step, 2, 4, 4), dtype=torch.float32, device=dev) if poses else None
     g = colmap.gaussians_from_points(xyz, rgb, sh_degree=3)
     P = {k: torch.from_numpy(g[k]).to(dev) for k in PARAM_ORDER}
-    pp = PipelineParams(tile_size=(8, 16), sparse_grad=True, antialiased=antialiased, exact_grad=exact_grad)
+    pp = PipelineParams(tile_size=(8, 16), sparse_grad=True, antialiased=antialiased, exact_grad=exact_grad, render_depth=use_depth)
     acc = lgs_dist.GradAccumulator(P)
     extent = float(np.linalg.norm(xyz.max(0) - xyz.min(0)) * 0.5)
     opt, sched = optimizer.get_optimizer(P, spatial_lr_scale=extent)
@@ -159,10 +210,18 @@ def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=Fal
         if it % 50 == 0:
             A = list(scene.cluster_aabb_torch(P["xyz"], P["scale"], P["rot"], filter_3d=filt))
         cams = poses.cameras(idx) if poses else [frames[j][0] for j in idx]
+
+        def colour_loss(i, img):
+            return ssim.l1_ssim_loss_and_grad(img.contiguous(), frames[idx[i]][1], 0.2, upstream=1.0 / views_per_step)
+
+        def colour_and_depth_loss(i, img, depth, trans):
+            loss, d_img = colour_loss(i, img)
+            ld, d_depth, d_trans = depth_loss_and_grad(depth, trans, targets[idx[i]], depth_weight, upstream=1.0 / views_per_step)
+            return loss + ld, d_img, d_depth, d_trans
+
         losses = render.render_views(views_per_step, lambda i: cams[i], None, A[0], A[1], P["xyz"], P["scale"], P["rot"],
                                      P["sh_0"], P["sh_rest"], P["opacity"], 3, (H, W), pp, acc.grads(),
-                                     loss_and_grad_fn=lambda i, img: ssim.l1_ssim_loss_and_grad(img.contiguous(), frames[idx[i]][1], 0.2,
-                                                                                              upstream=1.0 / views_per_step),
+                                     loss_and_grad_fn=colour_and_depth_loss if use_depth else colour_loss,
                                      camera_grads=cgrads, filter_3d=filt)
         opt.step(acc)
         if poses:
@@ -173,14 +232,22 @@ def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=Fal
             log(f"iter {it:5d}  loss {hist[-1]:.5f}")
     torch.cuda.synchronize(dev)
     dt = time.perf_counter() - t0
+    pp_eval = PipelineParams(tile_size=(8, 16), sparse_grad=True, antialiased=antialiased, render_depth=targets is not None,
+                             enable_transmitance=targets is not None)
     with torch.no_grad():
-        mse = []
+        mse, ed_err = [], []
         for j, (cam, gt, _) in enumerate(frames[:8]):
             cam = poses.cameras([j])[0] if poses else cam
-            img = render.render_view(A[0], A[1], cam["frustumplane"], cam["view"], cam["proj"], P["xyz"], P["scale"], P["rot"], P["sh_0"],
-                                     P["sh_rest"], P["opacity"], 3, (H, W), pp, filter_3d=filt)[0]
+            img, trans, depth, _, _ = render.render_view(A[0], A[1], cam["frustumplane"], cam["view"], cam["proj"], P["xyz"], P["scale"],
+                                                         P["rot"], P["sh_0"], P["sh_rest"], P["opacity"], 3, (H, W), pp_eval, filter_3d=filt)
             mse.append(float(((img - gt) ** 2).mean()))
+            if targets is not None:
+                ed_err.append(float(depth_loss_and_grad(depth, trans, targets[j], 1.0)[0]))
     psnr = -10.0 * np.log10(np.mean(mse))
+    if ed_err:
+        log(f"expected-depth error over 8 training views: {np.mean(ed_err):.4f}")
+        if metrics is not None:
+            metrics["ed_error"] = float(np.mean(ed_err))
     log(f"{iters} iterations x {views_per_step} views in {dt:.1f} s ({iters * views_per_step / dt:.0f} views/s incl. loss + optimizer); "
         f"{xyz.shape[0]} Gaussians, PSNR over 8 training views {psnr:.2f} dB")
     if poses:
@@ -200,6 +267,8 @@ if __name__ == "__main__":
                     help="Mip-Splatting's 3D smoothing filter, from all training cameras at iteration 0 and every 100 iterations")
     ap.add_argument("--exact-grad", action="store_true",
                     help="exact position and camera gradients: also through the ray-space Jacobian and the SH view direction")
+    ap.add_argument("--depth-weight", type=float, default=0.0,
+                    help="weight of the mean |expected depth - target| term (needs depths/<image stem>.npy, written by --make)")
     ap.add_argument("--pose-noise", type=float, nargs=2, default=None, metavar=("DEG", "FRAC"),
                     help="with --make: perturb the written poses by DEG degrees and FRAC of the camera distance")
     a = ap.parse_args()
@@ -209,5 +278,5 @@ if __name__ == "__main__":
     if root is None:
         ap.error("give --data or --make")
     h, _ = train(root, a.iters, refine_poses=a.refine_poses, antialiased=a.antialiased, filter_3d=a.filter_3d,
-                 exact_grad=a.exact_grad)
+                 exact_grad=a.exact_grad, depth_weight=a.depth_weight)
     assert h[-1] < h[0]

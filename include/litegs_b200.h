@@ -201,12 +201,16 @@ int lgs_pack_params(const float* ndc, const float* cov2d_inv, const float* color
  * (render/__init__.py:87) -- then pass the image back to lgs_rasterize_backward as `clamped_img`.
  * last_contributor holds an UNSIGNED 16-bit count (the reference reads it back as unsigned short, GR/raster.cu:683-686),
  * saturated at 65535.  tile_work i32[V,tiles] (nullable): per tile, the deepest list position any of its pixels consumed
- * = the backward's trip count, input of lgs_tile_order (zero it first when specific_tiles is given). */
+ * = the backward's trip count, input of lgs_tile_order (zero it first when specific_tiles is given).
+ * depth f32[V,1,Hp,Wp] or NULL, ours (the reference leaves its depth image zero): per pixel D = sum_i w_i z_i with the weights of
+ * the colour and z_i the record's depth slot (the view-space z on the fused path), not clamped (DESIGN.md section 1, "Depth").
+ * Only the default kernel renders depth: with bulk staging or the pixel-pair forward selected, a non-NULL depth is refused.
+ * NULL = no depth, the same kernels as before. */
 int lgs_rasterize_forward_packed(const int* sorted_points, const int* start_index, const float* packed_params,
                                  const int* specific_tiles, int n_specific, int V, int N, int cap, int img_h, int img_w,
                                  int tile_h, int tile_w, int enable_statistic, int clamp_zero, float* img,
                                  float* transmittance, short* last_contributor, int* fragment_count,
-                                 float* fragment_weight, int* tile_work, void* stream);
+                                 float* fragment_weight, int* tile_work, float* depth, void* stream);
 
 /* order i32[V,tiles] = 1-based tile ids by descending work (heaviest lists first), to be passed as specific_tiles:
  * the device-side form of the reference's tile scheduling by last epoch's blend count (render/__init__.py:75-79,
@@ -217,13 +221,18 @@ int lgs_tile_order(const int* work, int V, int ntile, int* order, void* stream);
  * scratch (zeroed here); d_trans_img, clamped_img (the forward's clamp_zero=1 output: blocks the gradient where a
  * colour was clamped up to 0) and grad_inv_scaler (DEVICE f32[1]) may be NULL.  Outputs d_ndc
  * f32[V,4,N], d_cov2d_inv f32[V,2,2,N], d_color f32[V,3,N], d_opacity f32[1,N] (view 0 only, as the
- * reference), err_sum/err_square_sum f32[V,1,N].  Pass d_ndc=NULL to skip the unpack (fused path). */
+ * reference), err_sum/err_square_sum f32[V,1,N].  Pass d_ndc=NULL to skip the unpack (fused path).
+ * d_depth f32[V,1,Hp,Wp] or NULL, ours: dL/dD of the forward's depth image.  It joins the alpha gradient as one more colour
+ * channel with colour z, and packed_grad slot 10 receives sum_pixels w g_z = dL/dz (consumed by lgs_project_backward with depth
+ * = 1; the unpack ignores it).  Only the pixel-pair kernel (the default, and the deterministic mode) takes it: with the scalar
+ * kernel or bulk staging selected, a non-NULL d_depth is refused.  NULL = no depth gradient, the same kernels as before. */
 int lgs_rasterize_backward(const int* sorted_points, const int* start_index, const float* packed_params,
                            const int* specific_tiles, int n_specific, const float* final_transmittance,
                            const short* last_contributor, const float* d_img, const float* d_trans_img,
                            const float* clamped_img, const float* grad_inv_scaler, int V, int N, int cap, int img_h, int img_w, int tile_h,
                            int tile_w, int enable_statistic, float* packed_grad, float* d_ndc, float* d_cov2d_inv,
-                           float* d_color, float* d_opacity, float* err_sum, float* err_square_sum, void* stream);
+                           float* d_color, float* d_opacity, float* err_sum, float* err_square_sum, const float* d_depth,
+                           void* stream);
 
 /* staging selector for the raster kernels: 0 = cp.async / LDGSTS (default), 1 = cp.async.bulk + mbarrier */
 int lgs_set_staging(int bulk);
@@ -299,7 +308,10 @@ int lgs_emit_pairs_u16(const float* packed_params, const int* offset, const unsi
  * was given.  sh_base is not read (the constant band has no direction term; it may be NULL).  sh_rest is read only when
  * exact_grad != 0 and sh_degree > 0 (its rows of the active degree) and must be non-NULL then; at degree 0 it may be NULL, as
  * an empty tensor's pointer is.  With exact_grad != 0 the chunk size S is limited by the register use of the instantiation
- * (384 for the heaviest; a larger S is refused with an error naming the limit).  0 = the kernels without the terms. */
+ * (384 for the heaviest; a larger S is refused with an error naming the limit).  0 = the kernels without the terms.
+ * depth != 0: depth mode, ours.  packed_grad slot 10 (dL/dz from lgs_rasterize_backward's d_depth) is added to the view-space
+ * z gradient: it reaches g_position through the view matrix and d_cam as d view[k][2] += p~_k dz; d proj gets nothing from it.
+ * It is exact in both gradient conventions (z depends on neither J nor the SH direction).  0 = slot 10 is not read. */
 int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
                          const float* view_matrix, const float* proj_matrix, const float* position, const float* scale,
                          const float* rotation, const float* opacity, int C, int S, int A, int rest_dim, int img_h,
@@ -307,7 +319,7 @@ int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_id, const i
                          int zero_outputs, float* g_position, float* g_scale, float* g_rotation, float* g_sh_base,
                          float* g_sh_rest, float* g_opacity, float* touched, float* cam_partials, float* d_cam,
                          const float* filter_3d, int antialiased, const float* sh_base, const float* sh_rest, int exact_grad,
-                         void* stream);
+                         int depth, void* stream);
 
 /* create_viewproj_forward, GR/compact.cu:17-141: view_params f32[V,7] (qw qx qy qz tx ty tz), recp_tan_half_fov_x f32[1] ->
  * view, proj, viewproj f32[V,4,4] (row-vector convention) and frustumplane f32[V,6,4].  One thread per view. */

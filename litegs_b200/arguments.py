@@ -16,3 +16,6 @@ class PipelineParams:
     antialiased: bool = False
     # ours as well: exact gradient mode of the fused path's backward (DESIGN.md section 1), read as getattr(pp, "exact_grad", False)
     exact_grad: bool = False
+    # ours as well: per-pixel depth on the fused path (DESIGN.md section 1, "Depth"), read as getattr(pp, "render_depth", False);
+    # enable_depth above keeps the reference's meaning
+    render_depth: bool = False

@@ -64,10 +64,12 @@ static_assert(sizeof(SplatRec) == 48, "SplatRec must be 48 bytes");
 // 12-float gradient accumulator, same indexing as raster_backward's RED targets.  The geometry slots hold RAW moments
 // of dL/dpower over the splat's pixels (dx = mu_x - x_pixel, dy = mu_y - y_pixel, s_k = sum_pixels dpw dy^k per column):
 //   0: sum dx s0   1: sum s1   2: sum dx^2 s0   3: sum dx s1   4: sum s2   5,6,7: d colour   8: sum s0   9: err_sq
+//   10: d view-space z = sum_pixels w g_z (depth mode only, LGS_GRAD_DEPTH; zero otherwise)
 // and the consumer (unpack_kernel / project_backward_kernel) turns them into the gradients of GR/raster.cu:826-841 with the
 // splat's conic (A, B, C) and opacity o once per splat:
 //   dmu_x = -(A m0 + B m1)  dmu_y = -(B m0 + C m1)  dA = -m2/2  dB(total) = -m3  dC = -m4/2  do = m8 / o
 #define LGS_GRAD_FLOATS 12
+#define LGS_GRAD_DEPTH 10
 struct LgsRasterGrad { float dmx, dmy, dA, dB, dC, dop; };
 #ifdef __CUDACC__
 __device__ __forceinline__ void lgs_finish_raster_grad(const float4& a, const float4& c, const float4& e, float A, float B, float C,

@@ -492,7 +492,9 @@ __device__ __forceinline__ float warp_sum32_transposed(float* v)
 // EXACT: exact gradient mode.  d xyz (and, with CAM, the camera gradient) gain the terms through J (dJ = V3x3^T (T^T dM),
 // back through fused_J to the view-space position and P00, P11) and through the SH view direction (reads sh_rest of the
 // active degree).  The other gradients are the same instructions as without it.
-template <int DEG, bool CAM, bool AA, bool F3D, bool EXACT>
+// DEPTH: depth mode.  Record slot LGS_GRAD_DEPTH (d view-space z) joins dv.z: it reaches d xyz through V and the camera gradient as
+// dV[k][2] += p~_k dz, and nothing reaches d proj.  A Gaussian whose only gradient is that slot is not skipped.
+template <int DEG, bool CAM, bool AA, bool F3D, bool EXACT, bool DEPTH>
 __global__ void project_backward_kernel(
     const int64_t* __restrict__ chunk_ids, const int* __restrict__ visible_num, const float* __restrict__ view,
     const float* __restrict__ proj, const float* __restrict__ pos, const float* __restrict__ scale,
@@ -517,7 +519,7 @@ __global__ void project_backward_kernel(
     const float4* g4 = reinterpret_cast<const float4*>(grad + dst * LGS_GRAD_FLOATS);
     const float4 ga = g4[0], gb = g4[1], gc = g4[2];
     const bool any = (ga.x != 0.f) | (ga.y != 0.f) | (ga.z != 0.f) | (ga.w != 0.f) | (gb.x != 0.f) | (gb.y != 0.f) |
-                     (gb.z != 0.f) | (gb.w != 0.f) | (gc.x != 0.f);
+                     (gb.z != 0.f) | (gb.w != 0.f) | (gc.x != 0.f) | (DEPTH && gc.z != 0.f);
     float o_pos[3] = { 0.f, 0.f, 0.f }, o_sc[3] = { 0.f, 0.f, 0.f }, o_q[4] = { 0.f, 0.f, 0.f, 0.f }, o_op = 0.f;
     float shb[16], dcol3[3] = { 0.f, 0.f, 0.f };       // SH basis and colour gradient: d sh[k][c] = shb[k] * dcol3[c]
 #pragma unroll
@@ -620,6 +622,7 @@ __global__ void project_backward_kernel(
         float dv[4];
 #pragma unroll
         for (int k = 0; k < 4; k++) dv[k] = dh[0] * P[k * 4] + dh[1] * P[k * 4 + 1] + dh[2] * P[k * 4 + 2] + dh[3] * P[k * 4 + 3] + 0.f;
+        if constexpr (DEPTH) dv[2] += gc.z * sc;          // d view-space z of the depth channel (slot LGS_GRAD_DEPTH = gc.z)
         float dp00 = 0.f, dp11 = 0.f;
         if constexpr (EXACT) {
             // J term: dVJ = T^T dM, dJ[k][c] = sum_a V3[a][k] dVJ[a][c]; only J00, J11, J20, J21 depend on anything
@@ -782,12 +785,12 @@ __global__ void __launch_bounds__(1024) camera_grad_sum_kernel(const float* __re
 // Largest block an EXACT instantiation can be launched with.  The kernel has no launch bounds (the default instantiations
 // must keep their code), and the heaviest EXACT ones use up to 168 registers, which allows 384 threads instead of 1024
 // (DESIGN.md section 1, "Exact gradient mode").  Read once per instantiation, on its first (eager) use.
-template <int DEG, bool CAM, bool AA, bool F3D>
+template <int DEG, bool CAM, bool AA, bool F3D, bool DEPTH>
 static int project_backward_exact_max_threads()
 {
     static const int n = [] {
         cudaFuncAttributes a;
-        return cudaFuncGetAttributes(&a, project_backward_kernel<DEG, CAM, AA, F3D, true>) == cudaSuccess ? a.maxThreadsPerBlock : 0;
+        return cudaFuncGetAttributes(&a, project_backward_kernel<DEG, CAM, AA, F3D, true, DEPTH>) == cudaSuccess ? a.maxThreadsPerBlock : 0;
     }();
     return n;
 }
@@ -795,6 +798,7 @@ static int project_backward_exact_max_threads()
 // mode 0: outputs are compacted [..,A,S] and assigned; mode 1: same, cleared first (rows of chunks >= *visible_num and
 // sh_rest rows above the active degree must read as zero); mode 2: outputs are the DENSE [..,C,S] gradient tensors and
 // this view's gradients are accumulated into them (the multi-view / data-parallel path: no compacted round trip).
+// depth: 1 = the record gradient carries a depth slot (lgs_rasterize_backward was given d_depth), 0 = it does not.
 extern "C" int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
                                     const float* view_matrix, const float* proj_matrix, const float* position,
                                     const float* scale, const float* rotation, const float* opacity, int C, int S, int A,
@@ -802,7 +806,7 @@ extern "C" int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_
                                     const float* grad_inv_scaler, int zero_outputs, float* g_position, float* g_scale,
                                     float* g_rotation, float* g_sh_base, float* g_sh_rest, float* g_opacity, float* touched,
                                     float* cam_partials, float* d_cam, const float* filter_3d, int antialiased,
-                                    const float* sh_base, const float* sh_rest, int exact_grad, void* stream)
+                                    const float* sh_base, const float* sh_rest, int exact_grad, int depth, void* stream)
 {
     LGS_REQUIRE(sh_degree >= 0 && sh_degree <= 3, "project_backward: sh_degree %d not in 0..3", sh_degree);
     LGS_REQUIRE(rest_dim >= (sh_degree + 1) * (sh_degree + 1) - 1, "project_backward: sh_rest has %d rows, degree %d needs %d", rest_dim,
@@ -829,25 +833,29 @@ extern "C" int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_
         LGS_CUDA(cudaMemsetAsync(g_sh_rest, 0, sizeof(float) * (size_t)rest_dim * 3 * AS, st));
         LGS_CUDA(cudaMemsetAsync(g_opacity, 0, sizeof(float) * AS, st));
     }
-#define PB(D, K, AA, F3, EX) {                                                                                                      \
+#define PB(D, K, AA, F3, EX, Z) {                                                                                                   \
         if constexpr (EX) {                                                                                                         \
-            const int mt = project_backward_exact_max_threads<D, K, AA, F3>();                                                      \
+            const int mt = project_backward_exact_max_threads<D, K, AA, F3, Z>();                                                   \
             LGS_REQUIRE(S <= mt, "project_backward: exact_grad with this configuration supports chunk sizes up to %d, got %d", mt, S); \
         }                                                                                                                           \
-        project_backward_kernel<D, K, AA, F3, EX><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num,                            \
+        project_backward_kernel<D, K, AA, F3, EX, Z><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num,                         \
         view_matrix, proj_matrix, position, scale, rotation, opacity, C, S, A, rest_dim, img_h, img_w, true_sigmoid_grad, accumulate,  \
         packed_grad, grad_inv_scaler, g_position, g_scale, g_rotation, g_sh_base, g_sh_rest, g_opacity, touched, cam_partials,        \
         filter_3d, sh_rest); }
-#define PB_DEG(K, AA, F3, EX) switch (sh_degree) { case 0: PB(0, K, AA, F3, EX); break; case 1: PB(1, K, AA, F3, EX); break;          \
-                                                   case 2: PB(2, K, AA, F3, EX); break; default: PB(3, K, AA, F3, EX); }
-#define PB_CAM(AA, F3, EX) if (cam) { PB_DEG(true, AA, F3, EX) } else { PB_DEG(false, AA, F3, EX) }
-#define PB_MODE(EX)                                                                                                                 \
+#define PB_DEG(K, AA, F3, EX, Z) switch (sh_degree) { case 0: PB(0, K, AA, F3, EX, Z); break; case 1: PB(1, K, AA, F3, EX, Z); break; \
+                                                      case 2: PB(2, K, AA, F3, EX, Z); break; default: PB(3, K, AA, F3, EX, Z); }
+#define PB_CAM(AA, F3, EX, Z) if (cam) { PB_DEG(true, AA, F3, EX, Z) } else { PB_DEG(false, AA, F3, EX, Z) }
+#define PB_MODE(EX, Z)                                                                                                              \
     if (filter_3d != nullptr) {                                                                                                     \
-        if (antialiased) { PB_CAM(true, true, EX) } else { PB_CAM(false, true, EX) }                                                \
+        if (antialiased) { PB_CAM(true, true, EX, Z) } else { PB_CAM(false, true, EX, Z) }                                          \
     } else {                                                                                                                        \
-        if (antialiased) { PB_CAM(true, false, EX) } else { PB_CAM(false, false, EX) }                                              \
+        if (antialiased) { PB_CAM(true, false, EX, Z) } else { PB_CAM(false, false, EX, Z) }                                        \
     }
-    if (exact_grad) { PB_MODE(true) } else { PB_MODE(false) }
+    if (depth) {
+        if (exact_grad) { PB_MODE(true, true) } else { PB_MODE(false, true) }
+    } else {
+        if (exact_grad) { PB_MODE(true, false) } else { PB_MODE(false, false) }
+    }
 #undef PB_MODE
 #undef PB_CAM
 #undef PB_DEG

@@ -73,6 +73,26 @@ __device__ __forceinline__ void blend_pixel(float a, float cr, float cg, float c
         : "+f"(Ts), "+f"(Cr), "+f"(Cg), "+f"(Cb), "+f"(nf)
         : "f"(a), "f"(cr), "f"(cg), "f"(cb), "f"(ts_min), "f"(a_min), "f"(neg_ki));
 }
+// blend_pixel plus the depth channel: one more predicated FMA, D += z w, with the same weight as the colour.
+__device__ __forceinline__ void blend_pixel_depth(float a, float cr, float cg, float cb, float z, float& Ts, float& Cr, float& Cg,
+                                                  float& Cb, float& D, float& nf, float ts_min, float a_min, float neg_ki)
+{
+    asm("{\n"
+        ".reg .pred pa, pk;\n"
+        ".reg .f32 w;\n"
+        "setp.gt.f32 pa, %0, %10;\n"
+        "@pa add.f32 %5, %5, 0f3F800000;\n"
+        "setp.ge.and.f32 pk, %6, %11, pa;\n"
+        "mul.f32 w, %6, %0;\n"
+        "@pk fma.rn.f32 %1, %7, w, %1;\n"
+        "@pk fma.rn.f32 %2, %8, w, %2;\n"
+        "@pk fma.rn.f32 %3, %9, w, %3;\n"
+        "@pk fma.rn.f32 %4, %13, w, %4;\n"
+        "@pk fma.rn.f32 %0, %12, w, %0;\n"
+        "}\n"
+        : "+f"(Ts), "+f"(Cr), "+f"(Cg), "+f"(Cb), "+f"(D), "+f"(nf)
+        : "f"(a), "f"(cr), "f"(cg), "f"(cb), "f"(ts_min), "f"(a_min), "f"(neg_ki), "f"(z));
+}
 
 // ---- asynchronous staging primitives -------------------------------------------------------------
 __device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
@@ -158,25 +178,28 @@ struct Stager {
     // PRE: lane l then rewrites ITS record of the shared-memory copy into the form the pixel loops consume -- the conic pre-multiplied
     // for ex2 (A,B,C -> -0.5 log2e A, -log2e B, -0.5 log2e C) and o 256/255 in the depth slot -- so that these four multiplies are
     // done once per record instead of once per record by each of the 32 lanes (same fp32 products, bit-identical results).
-    template <bool PRE = false>
+    // DEPTH: the view-space z the depth slot held moves to the staged copy's pad0 first (the global record is not changed).
+    template <bool PRE = false, bool DEPTH = false>
     __device__ __forceinline__ void wait(int which, bool more_in_flight)
     {
         if (BULK) {
             mbar_wait(&bar[which], (phase_bits >> which) & 1u);
             phase_bits ^= (1u << which);
             pending &= ~(1u << which);
-            if (PRE) { prescale(which); __syncwarp(); }
+            if (PRE) { prescale<DEPTH>(which); __syncwarp(); }
         } else {
             if (more_in_flight) cp_async_wait<1>(); else cp_async_wait<0>();
-            if (PRE) prescale(which);            // the lane's own copy has landed (it waited on its own group)
+            if (PRE) prescale<DEPTH>(which);     // the lane's own copy has landed (it waited on its own group)
             __syncwarp();
         }
     }
+    template <bool DEPTH>
     __device__ __forceinline__ void prescale(int which)
     {
         SplatRec* r = buf + which * 32 + lane;
         const float2 ab = *reinterpret_cast<const float2*>(&r->A);
         const float2 co = *reinterpret_cast<const float2*>(&r->C);
+        if (DEPTH) r->pad0 = r->depth;
         *reinterpret_cast<float2*>(&r->A) = make_float2((-0.5f * LOG2E) * ab.x, (-LOG2E) * ab.y);
         r->C = (-0.5f * LOG2E) * co.x;
         r->depth = co.y * (256.0f / 255.0f);
@@ -215,13 +238,16 @@ __global__ void pack_kernel(const float* __restrict__ ndc, const float* __restri
 
 // ---- forward ---------------------------------------------------------------------------------------
 // PAIRS: blend the lane's pixels two at a time (add2/mul2/fma2; A/B switch, lgs_set_forward_pairs / env LGS_FWD_PAIRS).
-template <int TH, int TW, bool STAT, bool BULK, bool PAIRS = false>
+// DEPTH: also D = sum w z (the record's view-space z, DESIGN.md section 1 "Depth") into depth_out f32[V,1,Hp,Wp], unclamped;
+// built on the default form only (scalar body, cp.async staging).
+template <int TH, int TW, bool STAT, bool BULK, bool PAIRS = false, bool DEPTH = false>
 __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_forward_kernel(
     const int* __restrict__ sorted, const int* __restrict__ start_index, const SplatRec* __restrict__ recs,
     const int* __restrict__ tiles, int n_sel, float* __restrict__ img, float* __restrict__ Tout, unsigned short* __restrict__ last,
     int* __restrict__ frag_count, float* __restrict__ frag_weight, int* __restrict__ tile_work, int gx, int ntile, int cap, int N,
-    int Hp, int Wp, int clamp_zero)
+    int Hp, int Wp, int clamp_zero, float* __restrict__ depth_out)
 {
+    static_assert(!DEPTH || (!BULK && !PAIRS), "the depth channel exists on the default forward only");
     constexpr int PPT = TH * TW / 32;
     __shared__ __align__(128) SplatRec s_rec[WARPS_PER_BLOCK][2][32];
     __shared__ __align__(8) uint64_t s_bar[WARPS_PER_BLOCK][2];
@@ -248,9 +274,13 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_forward_kernel(
     // (exact up to 2^24; a predicated FADD on the FMA pipe instead of integer ops on the half-rate ALU pipe).
     constexpr float KS = 256.0f / 255.0f, KI = 255.0f / 256.0f;
     constexpr float TS_MIN = T_MIN * KI, A_MIN_S = ALPHA_MIN * KS;
-    float Ts[PPT], Cr[PPT], Cg[PPT], Cb[PPT], nf[PPT];
+    float Ts[PPT], Cr[PPT], Cg[PPT], Cb[PPT], nf[PPT], Dz[DEPTH ? PPT : 1];
 #pragma unroll
     for (int j = 0; j < PPT; j++) { Ts[j] = KI; Cr[j] = Cg[j] = Cb[j] = 0.0f; nf[j] = 0.0f; }
+    if (DEPTH) {
+#pragma unroll
+        for (int j = 0; j < PPT; j++) Dz[j] = 0.0f;
+    }
 
     if (count > 0) {
         Stager<BULK> st;
@@ -267,7 +297,7 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_forward_kernel(
                 int nn = (c + 2) * 32 + lane;
                 id_next = (nn < count) ? ids[nn] : -1;
             }
-            st.template wait<true>(c & 1, more);
+            st.template wait<true, DEPTH>(c & 1, more);
             const SplatRec* chunk = &s_rec[warp][c & 1][0];
             const int nk = min(32, count - c * 32);
             int my_id = 0;
@@ -327,7 +357,8 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_forward_kernel(
                         const bool ok = (Ts[j] > TS_MIN) && (a >= A_MIN_S);
                         if (ok) { fcount++; wsum += a * Ts[j]; }
                     }
-                    blend_pixel(a, q1.z, q1.w, cb, Ts[j], Cr[j], Cg[j], Cb[j], nf[j], TS_MIN, A_MIN_S, -KI);
+                    if (DEPTH) blend_pixel_depth(a, q1.z, q1.w, cb, chunk[k].pad0, Ts[j], Cr[j], Cg[j], Cb[j], Dz[j], nf[j], TS_MIN, A_MIN_S, -KI);
+                    else blend_pixel(a, q1.z, q1.w, cb, Ts[j], Cr[j], Cg[j], Cb[j], nf[j], TS_MIN, A_MIN_S, -KI);
                 }
                 }
                 if (STAT) {
@@ -358,6 +389,7 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_forward_kernel(
         img[((size_t)b * 3 + 1) * plane + po] = fmaxf(fminf(Cg[j], 1.0f), lo);
         img[((size_t)b * 3 + 2) * plane + po] = fmaxf(fminf(Cb[j], 1.0f), lo);
         Tout[(size_t)b * plane + po] = Ts[j] * KS;
+        if (DEPTH) depth_out[(size_t)b * plane + po] = Dz[j];
         // the contributor count is a 16-bit tensor in the reference contract (read back as unsigned short,
         // GR/raster.cu:683-686): saturate instead of wrapping when a pixel stays active past 65535 list entries
         last[(size_t)b * plane + po] = (unsigned short)__float2uint_rn(fminf(nf[j], 65535.0f));
@@ -598,20 +630,24 @@ __device__ __forceinline__ float2 bc2(float a) { return make_float2(a, a); }
 // longer depends on the order in which tiles reach a splat, so two runs give bit-identical gradients (SURVEY 7 asks for such a
 // mode next to the fp32 RED default, whose run-to-run spread is ~1e-6 relative).  `grad` then points at i64[N][LGS_GRAD_FLOATS].
 #define LGS_DET_SCALE 68719476736.0                      // 2^36: |value| < 1.3e8, resolution 1.5e-11
-template <int TH, int TW, bool STAT, bool TRANS, bool DET = false>
+// DEPTH: d_depth f32[V,1,Hp,Wp] = dL/dD is one more colour channel with "colour" z (the staged pad0): z g_z joins the (c - R) . g
+// dot product, and sum w g_z is reduced into slot LGS_GRAD_DEPTH.  That value is the last row of a parked splat; with STAT it makes
+// 11 rows, so only 2 splats are parked per flush (RG * NV <= 32 lanes).
+template <int TH, int TW, bool STAT, bool TRANS, bool DET = false, bool DEPTH = false>
 __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kernel(
     const int* __restrict__ sorted, const int* __restrict__ start_index, const SplatRec* __restrict__ recs,
     const int* __restrict__ tiles, int n_sel, const float* __restrict__ Tfinal, const unsigned short* __restrict__ last,
     const float* __restrict__ d_img, const float* __restrict__ d_trans, const float* __restrict__ clamped_img,
-    float* __restrict__ grad, int gx, int ntile, int cap, int N, int Hp, int Wp, int err_mode)
+    float* __restrict__ grad, int gx, int ntile, int cap, int N, int Hp, int Wp, int err_mode, const float* __restrict__ d_depth)
 {
     constexpr int PPT = TH * TW / 32, NP = PPT / 2;
     static_assert(PPT % 2 == 0, "pixels per lane must pair up");
-    constexpr int NV = STAT ? 10 : 9;                       // values reduced per (tile, splat)
+    constexpr int NV = 9 + (STAT ? 1 : 0) + (DEPTH ? 1 : 0);   // values reduced per (tile, splat)
+    constexpr int RG = (LGS_RG * NV <= 32) ? LGS_RG : 2;      // splats parked per flush
     constexpr float KS = 256.0f / 255.0f, A_MIN_S = ALPHA_MIN * KS;
     __shared__ __align__(128) SplatRec s_rec[WARPS_PER_BLOCK][2][32];
     __shared__ __align__(8) uint64_t s_bar[WARPS_PER_BLOCK][2];
-    __shared__ __align__(16) float s_acc[WARPS_PER_BLOCK][LGS_RG * NV][LGS_ROWF];
+    __shared__ __align__(16) float s_acc[WARPS_PER_BLOCK][RG * NV][LGS_ROWF];
     __shared__ int s_pid[WARPS_PER_BLOCK][4];               // ids of the splats parked in s_acc
     const int lane = threadIdx.x, warp = threadIdx.y, b = blockIdx.y;
     const int slot = blockIdx.x * blockDim.y + warp;
@@ -631,12 +667,16 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
     const float fx = (float)x, fy0 = (float)y0;
     const size_t plane = (size_t)Hp * Wp;
 
-    float2 T[NP], g0[NP], g1[NP], g2[NP], S[NP], ngt[NP];
+    float2 T[NP], g0[NP], g1[NP], g2[NP], S[NP], ngt[NP], gz[DEPTH ? NP : 1];
     int nl[PPT];
     int kmax = 0;
 #pragma unroll
     for (int j = 0; j < PPT; j++) {
         const size_t po = (size_t)(y0 + j) * Wp + x;
+        if (DEPTH) {
+            const float z = d_depth[(size_t)b * plane + po];
+            if (j & 1) gz[j / 2].y = z; else gz[j / 2].x = z;
+        }
         float t = Tfinal[(size_t)b * plane + po];
         float a0 = d_img[((size_t)b * 3 + 0) * plane + po];
         float a1 = d_img[((size_t)b * 3 + 1) * plane + po];
@@ -673,7 +713,8 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
             p0 = add2(p0, p2); p4 = add2(p4, p6);
             p0 = add2(p0, p4);
             const float sum = p0.x + p0.y;
-            const int sp = lane / NV, v = lane - sp * NV;
+            const int sp = lane / NV, row = lane - sp * NV;
+            const int v = (DEPTH && row == NV - 1) ? LGS_GRAD_DEPTH : row;         // gradient slot of the row
             const int pid = s_pid[warp][sp];
             if (DET) {
                 unsigned long long* gq = reinterpret_cast<unsigned long long*>(grad);
@@ -701,7 +742,7 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
             id_cur = id_next;
             id_next = (c >= 2) ? ids[(c - 2) * 32 + lane] : -1;
         }
-        st.template wait<true>(v & 1, more);
+        st.template wait<true, DEPTH>(v & 1, more);
         const SplatRec* chunk = &s_rec[warp][v & 1][0];
         const int nk = min(32, kmax - c * 32);
         for (int kk = nk - 1; kk >= 0; kk--) {
@@ -715,7 +756,8 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
             const float base = a2 * dx * dx, lin = b2 * dx;
             const float2 os2 = bc2(q2.y), o2 = bc2(q1.y), c22 = bc2(c2), lin2 = bc2(lin), base2 = bc2(base);
             const float2 cr2 = bc2(q1.z), cg2 = bc2(q1.w), cb2 = bc2(cb), dy02 = bc2(dy0);
-            float2 s0, s1, s2, dr, dg, db;              // per-(tile, splat) sums: the first pixel pair initialises them
+            const float2 z2 = bc2(DEPTH ? chunk[kk].pad0 : 0.0f);            // view-space z (staged by prescale<DEPTH>)
+            float2 s0, s1, s2, dr, dg, db, dzs;         // per-(tile, splat) sums: the first pixel pair initialises them
             float esq = 0.f, runx = 0.f, runy = 0.f;
             bool any = false;
 #pragma unroll
@@ -738,7 +780,8 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
                 const float2 Tn = mul2(T[p], rc);                                  // transmittance in front of this splat
                 T[p] = Tn;                                                               // (rc = 1 exactly where G was zeroed)
                 const float2 w = mul2(a, Tn);
-                const float2 cgd = fma2(cr2, g0[p], fma2(cg2, g1[p], mul2(cb2, g2[p])));
+                float2 cgd = fma2(cr2, g0[p], fma2(cg2, g1[p], mul2(cb2, g2[p])));
+                if (DEPTH) cgd = fma2(z2, gz[p], cgd);          // added last: g_z = 0 leaves the colour-only value
                 const float2 diff = fma2(S[p], bc2(-1.0f), cgd);                   // (c - R) . g
                 float2 da = mul2(Tn, diff);
                 if (TRANS) da = fma2(ngt[p], rc, da);
@@ -747,9 +790,11 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
                 const float2 td = mul2(dpw, dy);
                 if (p == 0) {
                     dr = mul2(w, g0[p]); dg = mul2(w, g1[p]); db = mul2(w, g2[p]);
+                    if (DEPTH) dzs = mul2(w, gz[p]);
                     s0 = dpw; s1 = td; s2 = mul2(td, dy);
                 } else {
                     dr = fma2(w, g0[p], dr); dg = fma2(w, g1[p], dg); db = fma2(w, g2[p], db);
+                    if (DEPTH) dzs = fma2(w, gz[p], dzs);
                     s0 = add2(s0, dpw);
                     s1 = add2(s1, td);
                     s2 = fma2(td, dy, s2);
@@ -782,8 +827,9 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
                 row[7 * LGS_ROWF] = db.x + db.y;
                 row[8 * LGS_ROWF] = m0;                    // sum s0
                 if (STAT) row[9 * LGS_ROWF] = esq;
+                if (DEPTH) row[(NV - 1) * LGS_ROWF] = dzs.x + dzs.y;     // sum w g_z -> slot LGS_GRAD_DEPTH
                 pend++;
-                if (pend == LGS_RG) flush();
+                if (pend == RG) flush();
             }
         }
         __syncwarp();
@@ -980,15 +1026,20 @@ extern "C" int lgs_pack_params(const float* ndc, const float* cov2d_inv, const f
 
 // sorted_points i32[V,cap]; start_index i32[V,tiles+2]; packed f32[V,N,12]; specific_tiles i32[V,n_sel] or null.
 // img f32[V,3,Hp,Wp]; T f32[V,1,Hp,Wp]; last i16[V,1,Hp,Wp]; fragment_count i32[V,1,N] / weight f32[V,1,N]
-// (must be zero-initialised by the caller when enable_statistic).
+// (must be zero-initialised by the caller when enable_statistic).  depth f32[V,1,Hp,Wp] or NULL: the per-pixel depth D = sum w z
+// of the records' view-space z (default kernel only: refused while bulk staging or the pair forward is forced).
 extern "C" int lgs_rasterize_forward_packed(const int* sorted_points, const int* start_index, const float* packed_params,
                                             const int* specific_tiles, int n_specific, int V, int N, int cap, int img_h, int img_w,
                                             int tile_h, int tile_w, int enable_statistic, int clamp_zero, float* img,
                                             float* transmittance, short* last_contributor, int* fragment_count,
-                                            float* fragment_weight, int* tile_work, void* stream)
+                                            float* fragment_weight, int* tile_work, float* depth, void* stream)
 {
     LGS_REQUIRE(lgs_tile_ok(tile_h, tile_w), "rasterize_forward: tile %dx%d not one of 8x16, 12x16, 16x16, 8x8", tile_h, tile_w);
     LGS_REQUIRE(V >= 1 && img_h > 0 && img_w > 0, "rasterize_forward: bad sizes V=%d H=%d W=%d", V, img_h, img_w);
+    const bool bulk = use_bulk();
+    LGS_REQUIRE(depth == nullptr || !(bulk || (!enable_statistic && forward_pairs())),
+                "rasterize_forward: depth is rendered by the default kernel only, but %s is selected",
+                bulk ? "bulk staging" : "the pixel-pair forward");
     int gx = (img_w + tile_w - 1) / tile_w, gy = (img_h + tile_h - 1) / tile_h;
     int ntile = gx * gy, Hp = gy * tile_h, Wp = gx * tile_w;
     int nrender = specific_tiles ? n_specific : ntile;
@@ -997,16 +1048,22 @@ extern "C" int lgs_rasterize_forward_packed(const int* sorted_points, const int*
     dim3 grid(lgs_cdiv(nrender, wpb), V), block(32, wpb);
     cudaStream_t st = (cudaStream_t)stream;
     const SplatRec* recs = (const SplatRec*)packed_params;
-    const bool bulk = use_bulk();
 #define FWD(S, B) raster_forward_kernel<TH, TW, S, B><<<grid, block, 0, st>>>(sorted_points, start_index, recs, specific_tiles, n_specific, \
-        img, transmittance, (unsigned short*)last_contributor, fragment_count, fragment_weight, tile_work, gx, ntile, cap, N, Hp, Wp, clamp_zero)
+        img, transmittance, (unsigned short*)last_contributor, fragment_count, fragment_weight, tile_work, gx, ntile, cap, N, Hp, Wp, clamp_zero, nullptr)
 #define FWDP() raster_forward_kernel<TH, TW, false, false, true><<<grid, block, 0, st>>>(sorted_points, start_index, recs, specific_tiles, \
-        n_specific, img, transmittance, (unsigned short*)last_contributor, fragment_count, fragment_weight, tile_work, gx, ntile, cap, N, Hp, Wp, clamp_zero)
-    LGS_DISPATCH_TILE(tile_h, tile_w,
-        if (enable_statistic) { if (bulk) FWD(true, true); else FWD(true, false); }
-        else { if (bulk) FWD(false, true); else if (forward_pairs()) FWDP(); else FWD(false, false); })
+        n_specific, img, transmittance, (unsigned short*)last_contributor, fragment_count, fragment_weight, tile_work, gx, ntile, cap, N, Hp, Wp, clamp_zero, nullptr)
+#define FWDD(S) raster_forward_kernel<TH, TW, S, false, false, true><<<grid, block, 0, st>>>(sorted_points, start_index, recs, specific_tiles, \
+        n_specific, img, transmittance, (unsigned short*)last_contributor, fragment_count, fragment_weight, tile_work, gx, ntile, cap, N, Hp, Wp, clamp_zero, depth)
+    if (depth != nullptr) {
+        LGS_DISPATCH_TILE(tile_h, tile_w, if (enable_statistic) FWDD(true); else FWDD(false);)
+    } else {
+        LGS_DISPATCH_TILE(tile_h, tile_w,
+            if (enable_statistic) { if (bulk) FWD(true, true); else FWD(true, false); }
+            else { if (bulk) FWD(false, true); else if (forward_pairs()) FWDP(); else FWD(false, false); })
+    }
 #undef FWD
 #undef FWDP
+#undef FWDD
     LGS_CHECK_LAUNCH("raster_forward_kernel");
     return LGS_OK;
 }
@@ -1018,10 +1075,14 @@ extern "C" int lgs_rasterize_backward(const int* sorted_points, const int* start
                                       const float* clamped_img, const float* grad_inv_scaler, int V, int N, int cap, int img_h,
                                       int img_w, int tile_h,
                                       int tile_w, int enable_statistic, float* packed_grad, float* d_ndc, float* d_cov2d_inv,
-                                      float* d_color, float* d_opacity, float* err_sum, float* err_square_sum, void* stream)
+                                      float* d_color, float* d_opacity, float* err_sum, float* err_square_sum, const float* d_depth,
+                                      void* stream)
 {
     LGS_REQUIRE(lgs_tile_ok(tile_h, tile_w), "rasterize_backward: tile %dx%d not one of 8x16, 12x16, 16x16, 8x8", tile_h, tile_w);
     LGS_REQUIRE(V >= 1 && img_h > 0 && img_w > 0, "rasterize_backward: bad sizes V=%d H=%d W=%d", V, img_h, img_w);
+    LGS_REQUIRE(d_depth == nullptr || deterministic() || (backward_version() == 2 && !use_bulk()),
+                "rasterize_backward: the depth gradient is taken by the pixel-pair kernel only, but %s is selected",
+                use_bulk() ? "bulk staging" : "the scalar (v1) kernel");
     int gx = (img_w + tile_w - 1) / tile_w, gy = (img_h + tile_h - 1) / tile_h;
     int ntile = gx * gy, Hp = gy * tile_h, Wp = gx * tile_w;
     int nrender = specific_tiles ? n_specific : ntile;
@@ -1042,22 +1103,28 @@ extern "C" int lgs_rasterize_backward(const int* sorted_points, const int* start
             long long* q = nullptr;
             LGS_CUDA(cudaMallocAsync((void**)&q, nq * sizeof(long long), st));
             LGS_CUDA(cudaMemsetAsync(q, 0, nq * sizeof(long long), st));
-#define BWD_DET(S, T) raster_backward_v2_kernel<TH, TW, S, T, true><<<grid, block, 0, st>>>(sorted_points, start_index, recs, specific_tiles, \
-        n_specific, final_transmittance, lastu, d_img, d_trans_img, clamped_img, (float*)q, gx, ntile, cap, N, Hp, Wp, g_err_mode)
-            LGS_DISPATCH_TILE(tile_h, tile_w,
-                if (enable_statistic) { if (trans) BWD_DET(true, true); else BWD_DET(true, false); }
-                else { if (trans) BWD_DET(false, true); else BWD_DET(false, false); })
+#define BWD_DET(S, T, Z) raster_backward_v2_kernel<TH, TW, S, T, true, Z><<<grid, block, 0, st>>>(sorted_points, start_index, recs, \
+        specific_tiles, n_specific, final_transmittance, lastu, d_img, d_trans_img, clamped_img, (float*)q, gx, ntile, cap, N, Hp, Wp, g_err_mode, \
+        d_depth)
+#define BWD_DET_Z(Z) LGS_DISPATCH_TILE(tile_h, tile_w,                                                                    \
+                if (enable_statistic) { if (trans) BWD_DET(true, true, Z); else BWD_DET(true, false, Z); }                  \
+                else { if (trans) BWD_DET(false, true, Z); else BWD_DET(false, false, Z); })
+            if (d_depth != nullptr) { BWD_DET_Z(true) } else { BWD_DET_Z(false) }
+#undef BWD_DET_Z
 #undef BWD_DET
             LGS_CHECK_LAUNCH("raster_backward_v2_kernel<DET>");
             det_to_float_kernel<<<lgs_cdiv((long long)nq, 256), 256, 0, st>>>(q, packed_grad, nq);
             LGS_CHECK_LAUNCH("det_to_float_kernel");
             LGS_CUDA(cudaFreeAsync(q, st));
         } else if (backward_version() == 2 && !bulk) {
-#define BW2(S, T) raster_backward_v2_kernel<TH, TW, S, T><<<grid, block, 0, st>>>(sorted_points, start_index, recs, specific_tiles, n_specific, \
-        final_transmittance, lastu, d_img, d_trans_img, clamped_img, packed_grad, gx, ntile, cap, N, Hp, Wp, g_err_mode)
-            LGS_DISPATCH_TILE(tile_h, tile_w,
-                if (enable_statistic) { if (trans) BW2(true, true); else BW2(true, false); }
-                else { if (trans) BW2(false, true); else BW2(false, false); })
+#define BW2(S, T, Z) raster_backward_v2_kernel<TH, TW, S, T, false, Z><<<grid, block, 0, st>>>(sorted_points, start_index, recs, \
+        specific_tiles, n_specific, final_transmittance, lastu, d_img, d_trans_img, clamped_img, packed_grad, gx, ntile, cap, N, Hp, Wp, \
+        g_err_mode, d_depth)
+#define BW2_Z(Z) LGS_DISPATCH_TILE(tile_h, tile_w,                                                                         \
+                if (enable_statistic) { if (trans) BW2(true, true, Z); else BW2(true, false, Z); }                          \
+                else { if (trans) BW2(false, true, Z); else BW2(false, false, Z); })
+            if (d_depth != nullptr) { BW2_Z(true) } else { BW2_Z(false) }
+#undef BW2_Z
 #undef BW2
             LGS_CHECK_LAUNCH("raster_backward_v2_kernel");
         } else {

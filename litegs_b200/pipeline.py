@@ -64,6 +64,7 @@ class ViewState:
     tile_order: Optional[torch.Tensor] = None   # i32[1,tiles]: tile ids, heaviest backward work first
     antialiased: bool = False        # antialiased mode (DESIGN.md section 1): the backward must use the forward's setting
     filter_3d: Optional[torch.Tensor] = None    # 3D smoothing filter f32[1,C,S] the forward used (DESIGN.md section 1), or None
+    depth: Optional[torch.Tensor] = None        # f32[1,1,Hp,Wp] per-pixel depth D (render_depth, DESIGN.md section 1), or None
 
 
 class _Pinned:
@@ -76,6 +77,15 @@ class _Pinned:
         if b is None:
             b = cls._bufs[dev] = torch.zeros(4, dtype=_I32).pin_memory()
         return b
+
+
+def _padded(g: torch.Tensor, shape) -> torch.Tensor:
+    """A per-pixel gradient f32[1,1,H,W] or [1,1,Hp,Wp] as a contiguous f32[1,1,Hp,Wp] (zeros in the padding)."""
+    if not (g.is_cuda and g.dtype == _F32 and g.dim() == 4 and g.shape[:2] == (1, 1)):
+        raise RuntimeError("per-pixel gradients must be float32 CUDA tensors of shape [1,1,H,W]")
+    if tuple(g.shape) != tuple(shape):
+        g = torch.nn.functional.pad(g, (0, shape[-1] - g.shape[-1], 0, shape[-2] - g.shape[-2]))
+    return g if g.is_contiguous() else g.contiguous()
 
 
 def check_filter_3d(filter_3d: Optional[torch.Tensor], xyz: torch.Tensor) -> Optional[torch.Tensor]:
@@ -92,7 +102,7 @@ def check_filter_3d(filter_3d: Optional[torch.Tensor], xyz: torch.Tensor) -> Opt
 def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_extend: torch.Tensor, frustumplane: torch.Tensor,
                         view_matrix: torch.Tensor, proj_matrix: torch.Tensor, sh_degree: int, hw: tuple, tile: tuple,
                         enable_statistic: bool = False, specific_tiles: Optional[torch.Tensor] = None, clamp_zero: bool = False,
-                        antialiased: bool = False, filter_3d: Optional[torch.Tensor] = None):
+                        antialiased: bool = False, filter_3d: Optional[torch.Tensor] = None, render_depth: bool = False):
     """Forward of one view.  params: xyz[3,C,S] scale[3,C,S] rot[4,C,S] sh_0[1,3,C,S] sh_rest[R,3,C,S]
     opacity[1,C,S] (raw, clustered; float32 CUDA, contiguous).  Returns (img f32[1,3,Hp,Wp] padded to whole
     tiles, ViewState, (fragment_count, fragment_weight) or None).
@@ -102,7 +112,10 @@ def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_exte
 
     filter_3d: Mip-Splatting's 3D smoothing filter f32[1,C,S] (scene.filter_3d_device), or None.  Each Gaussian is drawn with
     the scale sqrt(s^2 + f^2) and its opacity scaled by the matching volume ratio (DESIGN.md section 1); the state keeps the
-    tensor for the backward, which must see the same values."""
+    tensor for the backward, which must see the same values.
+
+    render_depth: also render the per-pixel depth D = sum_i w_i z_i (w_i the colour's blend weights, z_i the view-space z; not
+    clamped; DESIGN.md section 1, "Depth") into state.depth f32[1,1,Hp,Wp].  The expected depth is D / (1 - T)."""
     xyz = params["xyz"]
     dev = xyz.device
     filter_3d = check_filter_3d(filter_3d, xyz)
@@ -184,10 +197,13 @@ def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_exte
         img = torch.empty((1, 3, Hp, Wp), dtype=_F32, device=dev)
         T = torch.empty((1, 1, Hp, Wp), dtype=_F32, device=dev)
         last = torch.empty((1, 1, Hp, Wp), dtype=torch.int16, device=dev)
+        depth = torch.empty((1, 1, Hp, Wp), dtype=_F32, device=dev) if render_depth else None
         n_sel = 0
         if specific_tiles is not None:
             n_sel = specific_tiles.shape[1]
             img.zero_(); T.fill_(1.0); last.zero_()
+            if depth is not None:
+                depth.zero_()
         stats = None
         fc = fw = None
         if enable_statistic:
@@ -199,21 +215,22 @@ def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_exte
         work = torch.empty((1, ntile), dtype=_I32, device=dev) if (CONFIG["tile_order"] and specific_tiles is None and D > 0) else None
         _lib.call("lgs_rasterize_forward_packed", _ptr(sorted_pid), _ptr(ranges), _ptr(packed), _ptr(specific_tiles), n_sel, 1,
                   Nmax, sorted_pid.shape[1], H, W, th, tw, int(bool(enable_statistic)), int(bool(clamp_zero)), _ptr(img), _ptr(T),
-                  _ptr(last), _ptr(fc), _ptr(fw), _ptr(work), st)
+                  _ptr(last), _ptr(fc), _ptr(fw), _ptr(work), _ptr(depth), st)
         if work is not None:
             order = torch.empty((1, ntile), dtype=_I32, device=dev)
             _lib.call("lgs_tile_order", _ptr(work), 1, ntile, _ptr(order), st)
     state = ViewState(sh_degree=int(sh_degree), hw=(H, W), tile=(th, tw), n_chunks_visible=nvis, n_pairs=D, chunk_ids=ids,
                       counters=counters, view=view_matrix, proj=proj_matrix, packed=packed, tile_count=tcount,
                       sorted_pid=sorted_pid, ranges=ranges, T=T, last=last, tile_order=order, antialiased=bool(antialiased),
-                      filter_3d=filter_3d)
+                      filter_3d=filter_3d, depth=depth)
     return img, state, stats
 
 
 def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_trans: Optional[torch.Tensor] = None,
                          enable_statistic: bool = False, specific_tiles: Optional[torch.Tensor] = None,
                          accumulate_into: Optional[dict] = None, clamped_img: Optional[torch.Tensor] = None,
-                         camera_grad: Optional[torch.Tensor] = None, exact_grad: bool = False):
+                         camera_grad: Optional[torch.Tensor] = None, exact_grad: bool = False,
+                         d_depth: Optional[torch.Tensor] = None):
     """Backward of one view: d_img f32[1,3,Hp,Wp] (padded) -> compacted parameter gradients
     (xyz[3,A,S], scale[3,A,S], rot[4,A,S], sh_0[1,3,A,S], sh_rest[R,3,A,S], opacity[1,A,S]) with
     A = state.n_chunks_visible, plus packed_grad (whose slot 9 carries the statistics term).
@@ -226,7 +243,10 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
     J and the SH view direction held constant (DESIGN.md section 1).  It is assigned, not accumulated.
 
     exact_grad: exact gradient mode (DESIGN.md section 1): the xyz gradient and camera_grad also carry the terms through the
-    ray-space Jacobian J and through the SH view direction.  The other gradients and the forward do not depend on it."""
+    ray-space Jacobian J and through the SH view direction.  The other gradients and the forward do not depend on it.
+
+    d_depth: dL/dD f32[1,1,H,W] or [1,1,Hp,Wp] of the depth the forward rendered (render_depth=True), or None.  It reaches every
+    parameter through the blend weights and the positions and camera through the view-space z."""
     xyz = params["xyz"]
     dev = xyz.device
     C, S = xyz.shape[-2:]
@@ -240,6 +260,10 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
     d_img = d_img if d_img.is_contiguous() else d_img.contiguous()
     if d_trans is not None:
         d_trans = d_trans if d_trans.is_contiguous() else d_trans.contiguous()
+    if d_depth is not None:
+        if state.depth is None:
+            raise RuntimeError("d_depth is given, but the forward of this view did not render depth (render_depth=False)")
+        d_depth = _padded(d_depth, state.T.shape)
     if camera_grad is not None and not (camera_grad.is_cuda and camera_grad.dtype == _F32 and camera_grad.is_contiguous()
                                         and tuple(camera_grad.shape) == (2, 4, 4)):
         raise RuntimeError("camera_grad must be a contiguous float32 CUDA tensor of shape [2,4,4]")
@@ -255,7 +279,8 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
         _lib.call("lgs_rasterize_backward", _ptr(state.sorted_pid), _ptr(state.ranges), _ptr(state.packed), _ptr(specific_tiles), n_sel,
                   _ptr(state.T), _ptr(state.last), _ptr(d_img), _ptr(d_trans), _ptr(clamped_img), None, 1, Nmax, state.sorted_pid.shape[1],
                   H, W, th, tw,
-                  int(bool(enable_statistic)), _ptr(pg), None, None, None, None, None, None, st)
+                  int(bool(enable_statistic)), _ptr(pg), None, None, None, None, None, None, _ptr(d_depth), st)
+        depth_arg = int(d_depth is not None)            # the record gradient carries the depth slot
         if accumulate_into is not None:
             for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity"):
                 t = accumulate_into[k]
@@ -267,7 +292,7 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
                           _ptr(state.view), _ptr(state.proj), _ptr(xyz), _ptr(params["scale"]), _ptr(params["rot"]),
                           _ptr(params["opacity"]), C, S, A, R, H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(pg), None, 2,
                           _ptr(d["xyz"]), _ptr(d["scale"]), _ptr(d["rot"]), _ptr(d["sh_0"]), _ptr(d["sh_rest"]), _ptr(d["opacity"]),
-                          _ptr(d.get("_touched")), *cam_args, _ptr(state.filter_3d), int(state.antialiased), *exact_args, st)   # "_touched": chunk marks for the fused optimizer step
+                          _ptr(d.get("_touched")), *cam_args, _ptr(state.filter_3d), int(state.antialiased), *exact_args, depth_arg, st)   # "_touched": chunk marks for the fused optimizer step
             elif camera_grad is not None:
                 camera_grad.zero_()
             return None, pg
@@ -282,7 +307,7 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
             _lib.call("lgs_project_backward", state.sh_degree, _ptr(state.chunk_ids), ctypes.c_void_p(state.counters.data_ptr()),
                       _ptr(state.view), _ptr(state.proj), _ptr(xyz), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["opacity"]),
                       C, S, A, R, H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(pg), None, 0, _ptr(g_pos), _ptr(g_sc), _ptr(g_rot),
-                      _ptr(g_s0), _ptr(g_sr), _ptr(g_op), None, *cam_args, _ptr(state.filter_3d), int(state.antialiased), *exact_args, st)
+                      _ptr(g_s0), _ptr(g_sr), _ptr(g_op), None, *cam_args, _ptr(state.filter_3d), int(state.antialiased), *exact_args, depth_arg, st)
         elif camera_grad is not None:
             camera_grad.zero_()
     return [g_pos, g_sc, g_rot, g_s0, g_sr, g_op], pg
@@ -340,6 +365,8 @@ class ViewWorkspace:
         self.work, self.tile_order = e((1, self.ntile), _I32), e((1, self.ntile), _I32)
         self.pg = e((1, N, 12), _F32)
         self.d_img = e((1, 3, self.Hp, self.Wp), _F32)
+        self.depth = self.d_depth = self.d_trans = None     # f32[1,1,Hp,Wp] each, allocated on first use (depth mode, d_trans)
+        self.rendered_depth = False                          # whether the last forward on this workspace rendered depth
         self.cam_view, self.cam_proj, self.cam_planes = e((1, 4, 4), _F32), e((1, 4, 4), _F32), e((1, 6, 4), _F32)
         self.cam_partials, self.d_cam = e((C, 32), _F32), e((2, 4, 4), _F32)     # camera gradient: per-chunk rows, their sum
         nb = max(_query_bytes("lgs_sort_pairs_u32_workspace_bytes", _round_up(N, 1 << 16)),
@@ -354,7 +381,13 @@ class ViewWorkspace:
         self.views_done = 0
 
     # -- enqueue ---------------------------------------------------------------------------------------------------
-    def _forward_kernels(self, params, cluster_origin, cluster_extend, sh_degree, clamp_zero, antialiased, filter_3d):
+    def _plane(self, name):
+        """The f32[1,1,Hp,Wp] buffer `name`, allocated the first time it is asked for (its pointer then stays fixed)."""
+        if getattr(self, name) is None:
+            setattr(self, name, torch.zeros((1, 1, self.Hp, self.Wp), dtype=_F32, device=self.dev))
+        return getattr(self, name)
+
+    def _forward_kernels(self, params, cluster_origin, cluster_extend, sh_degree, clamp_zero, antialiased, filter_3d, render_depth):
         dev, st = self.dev, _stream(self.dev)
         H, W = self.hw
         th, tw = self.tile
@@ -383,19 +416,22 @@ class ViewWorkspace:
                   int(CONFIG["fix_last_tile"]), _ptr(self.ranges), st)
         order = CONFIG["tile_order"]
         _lib.call("lgs_rasterize_forward_packed", _ptr(self.sorted_pid), _ptr(self.ranges), _ptr(self.packed), None, 0, 1, N, D, H, W, th, tw,
-                  0, int(bool(clamp_zero)), _ptr(self.img), _ptr(self.T), _ptr(self.last), None, None, _ptr(self.work) if order else None, st)
+                  0, int(bool(clamp_zero)), _ptr(self.img), _ptr(self.T), _ptr(self.last), None, None, _ptr(self.work) if order else None,
+                  _ptr(self.depth) if render_depth else None, st)
         if order:
             _lib.call("lgs_tile_order", _ptr(self.work), 1, self.ntile, _ptr(self.tile_order), st)
 
-    def _backward_kernels(self, params, sh_degree, accumulate_into, use_clamp, camera_grad, antialiased, filter_3d, exact_grad):
+    def _backward_kernels(self, params, sh_degree, accumulate_into, use_clamp, camera_grad, antialiased, filter_3d, exact_grad, depth,
+                          trans):
         st = _stream(self.dev)
         H, W = self.hw
         th, tw = self.tile
         C, S, N, D = self.C, self.S, self.Nmax, self.cap
         tiles = self.tile_order if CONFIG["tile_order"] else None
         _lib.call("lgs_rasterize_backward", _ptr(self.sorted_pid), _ptr(self.ranges), _ptr(self.packed), _ptr(tiles),
-                  self.ntile if tiles is not None else 0, _ptr(self.T), _ptr(self.last), _ptr(self.d_img), None,
-                  _ptr(self.img) if use_clamp else None, None, 1, N, D, H, W, th, tw, 0, _ptr(self.pg), None, None, None, None, None, None, st)
+                  self.ntile if tiles is not None else 0, _ptr(self.T), _ptr(self.last), _ptr(self.d_img), _ptr(self.d_trans) if trans else None,
+                  _ptr(self.img) if use_clamp else None, None, 1, N, D, H, W, th, tw, 0, _ptr(self.pg), None, None, None, None, None, None,
+                  _ptr(self.d_depth) if depth else None, st)
         d = accumulate_into
         R = params["sh_rest"].shape[0]
         # A = all chunks: project_backward returns at once for chunks past the (device) visible count
@@ -404,7 +440,7 @@ class ViewWorkspace:
                   H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(self.pg), None, 2, _ptr(d["xyz"]), _ptr(d["scale"]), _ptr(d["rot"]),
                   _ptr(d["sh_0"]), _ptr(d["sh_rest"]), _ptr(d["opacity"]), _ptr(d.get("_touched")),
                   _ptr(self.cam_partials) if camera_grad else None, _ptr(self.d_cam) if camera_grad else None, _ptr(filter_3d),
-                  int(antialiased), _ptr(params["sh_0"]), _ptr(params["sh_rest"]), int(exact_grad), st)
+                  int(antialiased), _ptr(params["sh_0"]), _ptr(params["sh_rest"]), int(exact_grad), int(depth), st)
 
     def _run(self, kind, sig, fn):
         """Eager the first time a pointer signature is seen, captured into a CUDA graph the second time, replayed afterwards."""
@@ -427,30 +463,40 @@ class ViewWorkspace:
         self._graphs[key] = g
         g.replay()
 
-    def forward(self, params, cluster_origin, cluster_extend, cam, sh_degree, clamp_zero=True, antialiased=False, filter_3d=None):
+    def forward(self, params, cluster_origin, cluster_extend, cam, sh_degree, clamp_zero=True, antialiased=False, filter_3d=None,
+                render_depth=False):
         """cam: dict(view, proj, frustumplane) of device tensors.  Returns the padded image (a view of the workspace).
+        render_depth: also render the per-pixel depth D into ``self.depth`` (f32[1,1,Hp,Wp], DESIGN.md section 1); the transmittance
+        is ``self.T``.
         antialiased: antialiased mode (DESIGN.md section 1); the backward of this view must be given the same value.
         filter_3d: 3D smoothing filter f32[1,C,S] or None; the backward of this view must be given the same tensor.  Its data
         pointer is part of the graph signature: a replayed graph reads whatever the tensor holds, so recomputing it in place
         (scene.filter_3d_device(..., out=)) needs no new capture."""
         filter_3d = check_filter_3d(filter_3d, params["xyz"])
+        if render_depth:
+            self._plane("depth")
         self.cam_view.copy_(cam["view"], non_blocking=True)
         self.cam_proj.copy_(cam["proj"], non_blocking=True)
         self.cam_planes.copy_(cam["frustumplane"], non_blocking=True)
         sig = (tuple(params[k].data_ptr() for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")), cluster_origin.data_ptr(),
                cluster_extend.data_ptr(), int(sh_degree), bool(clamp_zero), bool(CONFIG["tile_order"]),
                0 if filter_3d is None else filter_3d.data_ptr(), bool(antialiased))
+        if render_depth:
+            sig += ("depth",)
         self._run("fwd", sig, lambda: self._forward_kernels(params, cluster_origin, cluster_extend, sh_degree, clamp_zero, antialiased,
-                                                            filter_3d))
+                                                            filter_3d, bool(render_depth)))
+        self.rendered_depth = bool(render_depth)
         self.views_done += 1
         return self.img
 
     def backward(self, params, d_img, sh_degree, accumulate_into, use_clamp=True, camera_grad=None, antialiased=False, filter_3d=None,
-                 exact_grad=False):
+                 exact_grad=False, d_depth=None, d_trans=None):
         """d_img f32[1,3,H,W] or [1,3,Hp,Wp]: gradient of the loss w.r.t. the (clamped) image.  camera_grad (optional f32[2,4,4]
         CUDA tensor) receives (d view_matrix, d proj_matrix) of this view, copied on the stream after the backward.
         antialiased, filter_3d: the values the forward of this view was given.  exact_grad: exact gradient mode (DESIGN.md
-        section 1); a backward-only choice, so it is part of the backward graph's signature and of nothing else."""
+        section 1); a backward-only choice, so it is part of the backward graph's signature and of nothing else.
+        d_depth, d_trans: f32[1,1,H,W] or [1,1,Hp,Wp] gradients of the depth (the forward must have rendered it) and of the
+        transmittance, or None; whether each is given is part of the backward graph's signature."""
         filter_3d = check_filter_3d(filter_3d, params["xyz"])
         if camera_grad is not None and not (camera_grad.is_cuda and camera_grad.dtype == _F32 and tuple(camera_grad.shape) == (2, 4, 4)):
             raise RuntimeError("camera_grad must be a float32 CUDA tensor of shape [2,4,4]")
@@ -461,14 +507,28 @@ class ViewWorkspace:
             if self.Hp != H or self.Wp != W:
                 self.d_img.zero_()
             self.d_img[..., :H, :W].copy_(d_img, non_blocking=True)
+        if d_depth is not None and not self.rendered_depth:
+            raise RuntimeError("d_depth is given, but the last forward on this workspace did not render depth (render_depth=False)")
+        for name, g in (("d_depth", d_depth), ("d_trans", d_trans)):
+            if g is None:
+                continue
+            plane = self._plane(name)
+            if g.shape[-2:] == (self.Hp, self.Wp):
+                plane.copy_(g, non_blocking=True)
+            else:
+                if self.Hp != H or self.Wp != W:
+                    plane.zero_()
+                plane[..., :H, :W].copy_(g, non_blocking=True)
         sig = (tuple(params[k].data_ptr() for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")),
                tuple(accumulate_into[k].data_ptr() for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")),
                0 if accumulate_into.get("_touched") is None else accumulate_into["_touched"].data_ptr(), int(sh_degree), bool(use_clamp),
                bool(CONFIG["tile_order"]), bool(antialiased), 0 if filter_3d is None else filter_3d.data_ptr(), bool(exact_grad),
                camera_grad is not None)
+        if d_depth is not None or d_trans is not None:
+            sig += (("depth", d_depth is not None, d_trans is not None),)
         cam = camera_grad is not None
         self._run("bwd", sig, lambda: self._backward_kernels(params, sh_degree, accumulate_into, use_clamp, cam, antialiased, filter_3d,
-                                                             bool(exact_grad)))
+                                                             bool(exact_grad), d_depth is not None, d_trans is not None))
         if cam:
             camera_grad.copy_(self.d_cam, non_blocking=True)
 

@@ -7,6 +7,7 @@ Level B is what ``bench.py`` measures.
 """
 from __future__ import annotations
 
+import copy
 import math
 import os
 from typing import Optional
@@ -69,7 +70,7 @@ def render(view_matrix, proj_matrix, xyz, scale, rot, color, opacity,
            valid_length, feedback_binning_allocate_size, idx_tensor,
            actived_sh_degree: int, output_shape, pp):
     """Projection -> binning -> rasterisation; returns (img, transmittance, depth, normal, primitive_visible)
-    as render/__init__.py:50-94.  The antialiased and exact gradient modes exist on the fused path only (render_view,
+    as render/__init__.py:50-94.  The antialiased, exact gradient and depth modes exist on the fused path only (render_view,
     render_views)."""
     if getattr(pp, "antialiased", False):
         raise RuntimeError("pp.antialiased is set, but the op-by-op render() has no antialiased mode and would draw every splat "
@@ -77,6 +78,9 @@ def render(view_matrix, proj_matrix, xyz, scale, rot, color, opacity,
     if getattr(pp, "exact_grad", False):
         raise RuntimeError("pp.exact_grad is set, but the op-by-op render() has no exact gradient mode and would return position "
                            "gradients with J and the SH direction held constant; render through render_view or render_views instead")
+    if getattr(pp, "render_depth", False):
+        raise RuntimeError("pp.render_depth is set, but the op-by-op render() has no depth mode (its depth slot keeps the reference's "
+                           "enable_depth contract); render through render_view or render_views instead")
     nvtx.range_push("Proj")
     view_pos, ndc_pos = wrapper.MVPTransform.apply(xyz, view_matrix, proj_matrix, valid_length)
     transform_matrix = wrapper.CreateTransformMatrix.call_fused(scale, rot, valid_length)
@@ -138,14 +142,14 @@ class _RenderViewFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, xyz, scale, rot, sh_0, sh_rest, opacity, cluster_origin, cluster_extend, frustumplane,
                 view_matrix, proj_matrix, sh_degree, H, W, th, tw, sparse_grad, enable_transmitance, accumulate_into, antialiased,
-                filter_3d, exact_grad):
+                filter_3d, exact_grad, render_depth):
         params = dict(xyz=xyz, scale=scale, rot=rot, sh_0=sh_0, sh_rest=sh_rest, opacity=opacity)
         stat = bool(StatisticsHelperInst.bStart)
         ctx.set_materialize_grads(False)       # an unused transmittance output must not cost a zero-filled gradient image
         # the kernel writes clamp(c,0,1) directly (render/__init__.py:87 does it as a separate pass) ...
         img, state, stats = pipeline.render_view_forward(params, cluster_origin, cluster_extend, frustumplane, view_matrix,
                                                          proj_matrix, sh_degree, (H, W), (th, tw), enable_statistic=stat, clamp_zero=True,
-                                                         antialiased=antialiased, filter_3d=filter_3d)
+                                                         antialiased=antialiased, filter_3d=filter_3d, render_depth=render_depth)
         ctx.state = state
         ctx.stats = stats
         ctx.stat = stat
@@ -155,10 +159,10 @@ class _RenderViewFn(torch.autograd.Function):
         ctx.exact_grad = bool(exact_grad)           # backward only: the forward does not depend on it
         ctx.save_for_backward(xyz, scale, rot, sh_0, sh_rest, opacity, img)
         ctx.mark_non_differentiable(state.last)
-        return img, state.T, state.last
+        return img, state.T, state.last, state.depth          # depth: None unless render_depth
 
     @staticmethod
-    def backward(ctx, g_img, g_T, _g_last):
+    def backward(ctx, g_img, g_T, _g_last, g_depth):
         xyz, scale, rot, sh_0, sh_rest, opacity, img_out = ctx.saved_tensors
         params = dict(xyz=xyz, scale=scale, rot=rot, sh_0=sh_0, sh_rest=sh_rest, opacity=opacity)
         state = ctx.state
@@ -172,7 +176,7 @@ class _RenderViewFn(torch.autograd.Function):
         grads, pg = pipeline.render_view_backward(params, state, g_img, g_T if (ctx.trans and g_T is not None) else None,
                                                   enable_statistic=ctx.stat,
                                                   accumulate_into=ctx.accumulate_into, clamped_img=img_out, camera_grad=cam,
-                                                  exact_grad=ctx.exact_grad)
+                                                  exact_grad=ctx.exact_grad, d_depth=g_depth)
         if ctx.stat:
             _feed_statistics(state, ctx.stats, pg, state.tile)
         g_view = g_proj = None
@@ -181,7 +185,7 @@ class _RenderViewFn(torch.autograd.Function):
             g_proj = cam[1].reshape(state.proj.shape) if ctx.needs_input_grad[10] else None
         if grads is None:          # gradients went straight into the caller's dense buffers
             ctx.state = None
-            return (None,) * 9 + (g_view, g_proj) + (None,) * 11
+            return (None,) * 9 + (g_view, g_proj) + (None,) * 12
         C, S = xyz.shape[-2:]
         ids = state.chunk_ids[: state.n_chunks_visible]
         out = []
@@ -189,7 +193,7 @@ class _RenderViewFn(torch.autograd.Function):
             ct = CompactedTensor((*g.shape[:-2], C, S), ids, g)
             out.append(ct if ctx.sparse else ct.to_dense())
         ctx.state = None
-        return (*out, None, None, None, g_view, g_proj, None, None, None, None, None, None, None, None, None, None, None)
+        return (*out, None, None, None, g_view, g_proj, None, None, None, None, None, None, None, None, None, None, None, None)
 
 
 def render_view(cluster_origin, cluster_extend, frustumplane, view_matrix, proj_matrix,
@@ -204,19 +208,22 @@ def render_view(cluster_origin, cluster_extend, frustumplane, view_matrix, proj_
     data-parallel training).  ``pp.antialiased`` (absent = False) selects the antialiased mode (DESIGN.md section 1).
     ``pp.exact_grad`` (absent = False) selects the exact gradient mode (DESIGN.md section 1): the xyz and camera gradients also
     carry the terms through the ray-space Jacobian J and the SH view direction.
+    ``pp.render_depth`` (absent = False) also renders the per-pixel depth D = sum_i w_i z_i (DESIGN.md section 1, "Depth") and
+    returns it, differentiable, in the depth slot as [1,1,H,W]; the expected depth is D / (1 - transmittance).  ``pp.enable_depth``
+    keeps the reference's meaning.
     ``filter_3d`` (f32[1,C,S] or None): Mip-Splatting's 3D smoothing filter (scene.filter_3d_device, DESIGN.md section 1); it is
     an input without a gradient."""
     if not pp.cluster_size:
         raise RuntimeError("render_view needs the clustered layout (cluster_size > 0); use render_preprocess + render otherwise")
     H, W = int(output_shape[0]), int(output_shape[1])
     th, tw = int(pp.tile_size[0]), int(pp.tile_size[1])
-    img, T, last = _RenderViewFn.apply(xyz, scale, rot, sh_0, sh_rest, opacity, cluster_origin, cluster_extend, frustumplane,
-                                       view_matrix, proj_matrix, int(actived_sh_degree), H, W, th, tw, pp.sparse_grad,
-                                       pp.enable_transmitance, accumulate_into, bool(getattr(pp, "antialiased", False)), filter_3d,
-                                       bool(getattr(pp, "exact_grad", False)))
+    img, T, last, depth = _RenderViewFn.apply(xyz, scale, rot, sh_0, sh_rest, opacity, cluster_origin, cluster_extend, frustumplane,
+                                              view_matrix, proj_matrix, int(actived_sh_degree), H, W, th, tw, pp.sparse_grad,
+                                              pp.enable_transmitance, accumulate_into, bool(getattr(pp, "antialiased", False)),
+                                              filter_3d, bool(getattr(pp, "exact_grad", False)), bool(getattr(pp, "render_depth", False)))
     img = img[..., :H, :W]          # already clamped to [0,1] by the kernel
     trans = T[..., :H, :W] if pp.enable_transmitance else None
-    return img, trans, None, None, last
+    return img, trans, None if depth is None else depth[..., :H, :W], None, last
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -257,7 +264,12 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
     ``camera_grads`` (optional contiguous f32[n_views,2,4,4] CUDA tensor): slot i receives (d view_matrix, d proj_matrix) of view i
     (pipeline.render_view_backward), on every path; it is complete when this function returns (the current stream waits).
 
-    ``filter_3d`` (f32[1,C,S] or None): the 3D smoothing filter every view of the batch is drawn with (see render_view)."""
+    ``filter_3d`` (f32[1,C,S] or None): the 3D smoothing filter every view of the batch is drawn with (see render_view).
+
+    ``pp.render_depth`` (absent = False): every view also renders its depth (see render_view), and the callbacks take it with the
+    transmittance: ``loss_fn(i, img, depth, trans)`` -> scalar (autograd over the three [1,C,H,W] inputs) or ``(loss, d_img,
+    d_depth, d_trans)``, and ``loss_and_grad_fn(i, img, depth, trans) -> (loss, d_img, d_depth, d_trans)``, where d_depth and
+    d_trans may be None.  An expected-depth loss uses depth / (1 - trans).  Without the flag both callbacks are called as above."""
     dev = xyz.device
     filter_3d = pipeline.check_filter_3d(filter_3d, xyz)
     if camera_grads is not None and not (camera_grads.is_cuda and camera_grads.dtype == torch.float32 and camera_grads.is_contiguous()
@@ -269,6 +281,7 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
     th, tw = int(pp.tile_size[0]), int(pp.tile_size[1])
     aa = bool(getattr(pp, "antialiased", False))
     exact = bool(getattr(pp, "exact_grad", False))
+    dep = bool(getattr(pp, "render_depth", False))
     direct = loss_and_grad_fn is not None or _DIRECT_VIEWS
     if direct:
         params = dict(xyz=xyz.detach(), scale=scale.detach(), rot=rot.detach(), sh_0=sh_0.detach(), sh_rest=sh_rest.detach(),
@@ -279,8 +292,11 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
         cam = camera_fn(i)
         img_p, state, stats = pipeline.render_view_forward(params, cluster_origin, cluster_extend, cam["frustumplane"], cam["view"],
                                                            cam["proj"], int(actived_sh_degree), (H, W), (th, tw), enable_statistic=stat,
-                                                           clamp_zero=True, antialiased=aa, filter_3d=filter_3d)
-        if loss_and_grad_fn is not None:
+                                                           clamp_zero=True, antialiased=aa, filter_3d=filter_3d, render_depth=dep)
+        d_depth = d_trans = None
+        if dep:
+            loss, d_img, d_depth, d_trans = _depth_loss(i, img_p, state.depth, state.T, H, W)
+        elif loss_and_grad_fn is not None:
             loss, d_img = loss_and_grad_fn(i, img_p[..., :H, :W])
         else:                          # autograd only through the user's loss, never through the render kernels
             leaf = img_p[..., :H, :W].detach().requires_grad_(True)
@@ -291,10 +307,12 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
                 (d_img,) = torch.autograd.grad(loss, leaf)
         if d_img.shape[-2:] != img_p.shape[-2:]:                        # image padded to whole tiles: pad the gradient with zeros
             d_img = torch.nn.functional.pad(d_img, (0, img_p.shape[-1] - W, 0, img_p.shape[-2] - H))
+        if d_trans is not None:
+            d_trans = pipeline._padded(d_trans, state.T.shape)
         if wait_ev is not None:
             torch.cuda.current_stream(dev).wait_event(wait_ev)
-        _, pg_ = pipeline.render_view_backward(params, state, d_img, None, enable_statistic=stat, accumulate_into=accumulate_into,
-                                               clamped_img=img_p, camera_grad=slot(i), exact_grad=exact)
+        _, pg_ = pipeline.render_view_backward(params, state, d_img, d_trans, enable_statistic=stat, accumulate_into=accumulate_into,
+                                               clamped_img=img_p, camera_grad=slot(i), exact_grad=exact, d_depth=d_depth)
         if stat:
             _feed_statistics(state, stats, pg_, (th, tw))
         losses.append(loss.detach())
@@ -304,12 +322,21 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
         view, proj = cam["view"], cam["proj"]
         if camera_grads is not None:              # leaves of this call: their .grad is view i's camera gradient
             view, proj = view.detach().requires_grad_(True), proj.detach().requires_grad_(True)
-        img = render_view(cluster_origin, cluster_extend, cam["frustumplane"], view, proj, xyz, scale, rot, sh_0, sh_rest,
-                          opacity, actived_sh_degree, output_shape, pp, accumulate_into=accumulate_into, filter_3d=filter_3d)[0]
-        loss = loss_fn(i, img)
+        pp_i = pp
+        if dep and not pp.enable_transmitance:    # the depth callbacks take the transmittance
+            pp_i = copy.copy(pp)
+            pp_i.enable_transmitance = True
+        out = render_view(cluster_origin, cluster_extend, cam["frustumplane"], view, proj, xyz, scale, rot, sh_0, sh_rest,
+                          opacity, actived_sh_degree, output_shape, pp_i, accumulate_into=accumulate_into, filter_3d=filter_3d)
+        img = out[0]
+        loss = loss_fn(i, img, out[2], out[1]) if dep else loss_fn(i, img)
         if wait_ev is not None:          # the previous view's accumulate (other stream) must have landed
             torch.cuda.current_stream(dev).wait_event(wait_ev)
-        if isinstance(loss, tuple):
+        if isinstance(loss, tuple) and dep:
+            loss, *gs = loss
+            pairs = [(t, g) for t, g in zip((img, out[2], out[1]), gs) if g is not None]
+            torch.autograd.backward([t for t, _ in pairs], [g for _, g in pairs])
+        elif isinstance(loss, tuple):
             loss, d_img = loss
             img.backward(d_img)
         else:
@@ -331,8 +358,11 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
     def one_ws(i, wait_ev, ws):
         cam = camera_fn(i)
         img_p = ws.forward(params, cluster_origin, cluster_extend, cam, int(actived_sh_degree), clamp_zero=True, antialiased=aa,
-                           filter_3d=filter_3d)
-        if loss_and_grad_fn is not None:
+                           filter_3d=filter_3d, render_depth=dep)
+        d_depth = d_trans = None
+        if dep:
+            loss, d_img, d_depth, d_trans = _depth_loss(i, img_p, ws.depth, ws.T, H, W)
+        elif loss_and_grad_fn is not None:
             loss, d_img = loss_and_grad_fn(i, img_p[..., :H, :W])
         else:
             leaf = img_p[..., :H, :W].detach().requires_grad_(True)
@@ -344,8 +374,20 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
         if wait_ev is not None:
             torch.cuda.current_stream(dev).wait_event(wait_ev)
         ws.backward(params, d_img, int(actived_sh_degree), accumulate_into, use_clamp=True, camera_grad=slot(i), antialiased=aa,
-                    filter_3d=filter_3d, exact_grad=exact)
+                    filter_3d=filter_3d, exact_grad=exact, d_depth=d_depth, d_trans=d_trans)
         losses.append(loss.detach())
+
+    def _depth_loss(i, img_p, depth_p, T_p, H, W):
+        """The depth-mode callbacks on the padded outputs of one view -> (loss, d_img, d_depth or None, d_trans or None)."""
+        img, depth, trans = img_p[..., :H, :W], depth_p[..., :H, :W], T_p[..., :H, :W]
+        if loss_and_grad_fn is not None:
+            return tuple(loss_and_grad_fn(i, img, depth, trans))
+        leaves = [t.detach().requires_grad_(True) for t in (img, depth, trans)]
+        loss = loss_fn(i, *leaves)
+        if isinstance(loss, tuple):
+            return tuple(loss)
+        d_img, d_depth, d_trans = torch.autograd.grad(loss, leaves, allow_unused=True)
+        return loss, (torch.zeros_like(img) if d_img is None else d_img), d_depth, d_trans
 
     def one_probe(i, wait_ev):
         n0 = len(pipeline.LAST_VIEW_SIZES)
