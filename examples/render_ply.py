@@ -8,7 +8,8 @@
 Cameras: the poses of a COLMAP model when --colmap is given, else the Fibonacci lattice of scene.make_camera.  Forward only
 (the reference's example_metrics.py path): project -> bin -> sort -> composite, no gradients kept.  With --depth each view also
 writes <name>_depth.npy (D = sum w z, the accumulated view-space depth, f32[H,W]) and <name>_alpha.npy (1 - T, f32[H,W]); the
-expected depth is D / alpha where alpha > 0.
+expected depth is D / alpha where alpha > 0.  With --normal each view also writes <name>_normal.npy, the expected view-space
+normal N / (1 - T) (f32[3,H,W], zero where nothing was blended; DESIGN.md section 1, "Normals").
 """
 import argparse
 import os
@@ -38,6 +39,7 @@ def main():
     ap.add_argument("--filter-3d", action="store_true",
                     help="apply the file's filter_3D property (Mip-Splatting's 3D smoothing filter); the file must have it")
     ap.add_argument("--depth", action="store_true", help="also write the accumulated depth D and 1 - T of each view as .npy")
+    ap.add_argument("--normal", action="store_true", help="also write the expected view-space normal N / (1 - T) of each view as .npy")
     a = ap.parse_args()
     path = a.ply
     if a.make:
@@ -66,17 +68,22 @@ def main():
         cams = [(scene.make_camera(i, a.views, a.width, a.height), (a.height, a.width), f"view_{i:04d}.png") for i in range(a.views)]
     import PIL.Image
     os.makedirs(a.out, exist_ok=True)
-    imgs, depths = [], []
+    imgs, depths, normals = [], [], []
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     with torch.no_grad():
         for cam, hw, _ in cams:
             c = {k: torch.from_numpy(v).to(dev) for k, v in cam.items()}
             img, st, _ = pipeline.render_view_forward(P, A[0], A[1], c["frustumplane"], c["view"], c["proj"], a.sh_degree, hw, (8, 16),
-                                                      clamp_zero=True, antialiased=a.antialiased, filter_3d=filt, render_depth=a.depth)
+                                                      clamp_zero=True, antialiased=a.antialiased, filter_3d=filt, render_depth=a.depth,
+                                                      render_normal=a.normal)
             imgs.append(img[0, :, : hw[0], : hw[1]])
             if a.depth:
                 depths.append((st.depth[0, 0, : hw[0], : hw[1]], 1.0 - st.T[0, 0, : hw[0], : hw[1]]))
+            if a.normal:
+                alpha = 1.0 - st.T[0, :, : hw[0], : hw[1]]
+                nrm = st.normal[0, :, : hw[0], : hw[1]]
+                normals.append(torch.where(alpha > 0, nrm / alpha.clamp_min(1e-12), torch.zeros_like(nrm)))
     torch.cuda.synchronize()
     dt = time.perf_counter() - t0
     for (cam, hw, name), img in zip(cams, imgs):
@@ -85,6 +92,8 @@ def main():
     for (_, _, name), (d, alpha) in zip(cams, depths):
         np.save(os.path.join(a.out, os.path.splitext(name)[0] + "_depth.npy"), d.cpu().numpy())
         np.save(os.path.join(a.out, os.path.splitext(name)[0] + "_alpha.npy"), alpha.cpu().numpy())
+    for (_, _, name), en in zip(cams, normals):
+        np.save(os.path.join(a.out, os.path.splitext(name)[0] + "_normal.npy"), en.cpu().numpy())
     print(f"{g['n_points']} Gaussians, {len(cams)} views rendered in {dt * 1e3:.1f} ms ({len(cams) / dt:.0f} views/s forward only) -> {a.out}")
 
 

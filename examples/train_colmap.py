@@ -5,6 +5,7 @@
     python examples/train_colmap.py --make /tmp/noisy --pose-noise 1 0.02 --refine-poses     # learn the camera poses too
     python examples/train_colmap.py --make /tmp/noisy --pose-noise 1 0.02 --refine-poses --exact-grad   # ... with the J and SH terms
     python examples/train_colmap.py --make /tmp/synth_depth --depth-weight 0.1     # also supervise the expected depth
+    python examples/train_colmap.py --make /tmp/synth_normal --normal-weight 0.1   # also supervise the rendered normals
 
 Reads ``sparse/0/{cameras,images,points3D}.bin`` and ``images/*`` (litegs_b200.colmap; same files and conventions as the
 reference's ``litegs/io_manager/colmap.py`` + ``litegs/data.py``), initialises Gaussians from the SfM points the way
@@ -13,6 +14,9 @@ No densification (that policy is out of scope, SURVEY 2.1): the point count stay
 With ``--depth-weight W`` and a ``depths/`` directory beside ``images/`` (``depths/<image stem>.npy``, f32[H,W] expected depth,
 NaN where unknown -- ``--make`` writes the hidden scene's), the loss gains W * mean |ED - target| over the known pixels, with
 ED = D / (1 - T) from the depth mode (DESIGN.md section 1, "Depth").
+With ``--normal-weight W`` and a ``normals/`` directory (``normals/<image stem>.npy``, f32[3,H,W] unit view-space normal, NaN
+where unknown -- ``--make`` writes the hidden scene's N / |N|), the loss gains W * mean(1 - cos(N / |N|, target)) over the known
+pixels, with N from the normal mode (DESIGN.md section 1, "Normals"); it composes with ``--depth-weight``.
 """
 import argparse
 import os
@@ -37,21 +41,23 @@ def make_dataset(root, n_gaussians=60_000, n_views=24, hw=(270, 480), n_points=2
     axis and a translation of that fraction of the camera's distance, as noisy SfM poses are; the images stay exact."""
     dev = dev or torch.device("cuda:0")
     H, W = hw
-    pp = PipelineParams(tile_size=(8, 16), sparse_grad=True, render_depth=True, enable_transmitance=True)
+    pp = PipelineParams(tile_size=(8, 16), sparse_grad=True, render_depth=True, enable_transmitance=True, render_normal=True)
     truth = scene.make_scene(n_gaussians, sh_degree=3, seed=seed, log_scale_range=log_scale_range)
     T = {k: torch.from_numpy(truth[k]).to(dev) for k in PARAM_ORDER}
     A = [torch.from_numpy(truth[k]).to(dev) for k in ("cluster_origin", "cluster_extend")]
 
-    eds = {}
+    eds, nrms = {}, {}
 
     def render_fn(i, cam):
         c = {k: torch.from_numpy(v).to(dev) for k, v in cam.items()}
         with torch.no_grad():
-            img, trans, depth, _, _ = render.render_view(A[0], A[1], c["frustumplane"], c["view"], c["proj"], T["xyz"], T["scale"], T["rot"],
-                                                         T["sh_0"], T["sh_rest"], T["opacity"], 3, (H, W), pp)
+            img, trans, depth, normal, _ = render.render_view(A[0], A[1], c["frustumplane"], c["view"], c["proj"], T["xyz"], T["scale"],
+                                                              T["rot"], T["sh_0"], T["sh_rest"], T["opacity"], 3, (H, W), pp)
             alpha = 1.0 - trans[0, 0]
-            # the hidden scene's expected depth where it is mostly opaque, unknown elsewhere
+            # the hidden scene's expected depth and unit normal where it is mostly opaque, unknown elsewhere
             eds[i] = torch.where(alpha > 0.5, depth[0, 0] / alpha.clamp_min(0.5), torch.full_like(alpha, float("nan"))).cpu().numpy()
+            un = normal[0] / normal[0].norm(dim=0, keepdim=True).clamp_min(1e-12)
+            nrms[i] = torch.where(alpha[None] > 0.5, un, torch.full_like(un, float("nan"))).cpu().numpy()
         return (img[0].permute(1, 2, 0) * 255.0 + 0.5).clamp(0, 255).to(torch.uint8).cpu().numpy()
 
     rng = np.random.default_rng(seed + 7)
@@ -62,6 +68,9 @@ def make_dataset(root, n_gaussians=60_000, n_views=24, hw=(270, 480), n_points=2
     os.makedirs(os.path.join(root, "depths"), exist_ok=True)
     for i, name in enumerate(names):
         np.save(os.path.join(root, "depths", os.path.splitext(name)[0] + ".npy"), eds[i].astype(np.float32))
+    os.makedirs(os.path.join(root, "normals"), exist_ok=True)
+    for i, name in enumerate(names):
+        np.save(os.path.join(root, "normals", os.path.splitext(name)[0] + ".npy"), nrms[i].astype(np.float32))
     if pose_noise is not None:
         deg, frac = pose_noise
         cams, images, pts = colmap.read_model(root)
@@ -97,10 +106,10 @@ def load_dataset(root, image_dir="images", dev=None):
     return frames, np.stack([p.xyz for p in P]), np.stack([p.rgb for p in P])
 
 
-def load_depths(root, dev=None):
+def load_depths(root, dev=None, sub="depths"):
     """Expected-depth targets f32[1,1,H,W] (NaN = unknown) aligned with load_dataset's frames, from root/depths/<image stem>.npy;
-    None when the dataset has no depths directory."""
-    if not os.path.isdir(os.path.join(root, "depths")):
+    None when the dataset has no depths directory.  sub="normals": the unit-normal targets f32[1,3,H,W] of root/normals."""
+    if not os.path.isdir(os.path.join(root, sub)):
         return None
     dev = dev or torch.device("cuda:0")
     cams, images, _ = colmap.read_model(root)
@@ -108,9 +117,26 @@ def load_depths(root, dev=None):
     for im in sorted(images.values(), key=lambda v: v.name):
         if cams[im.camera_id].model != "PINHOLE":
             continue
-        d = np.load(os.path.join(root, "depths", os.path.splitext(im.name)[0] + ".npy")).astype(np.float32)
-        out.append(torch.from_numpy(d).to(dev)[None, None].contiguous())
+        d = np.load(os.path.join(root, sub, os.path.splitext(im.name)[0] + ".npy")).astype(np.float32)
+        d = d[None] if d.ndim == 2 else d
+        out.append(torch.from_numpy(d).to(dev)[None].contiguous())
     return out
+
+
+def normal_loss_and_grad(normal, target, weight, upstream=1.0):
+    """weight * mean(1 - cos(N / |N|, target)) over the pixels with a finite target and |N| > 1e-6 -> (loss, d_normal) with the
+    gradient scaled by upstream; also the mean angle in degrees (for the evaluation)."""
+    norm = normal.norm(dim=1, keepdim=True)
+    valid = torch.isfinite(target[:, :1]) & (norm > 1e-6)
+    n = valid.sum().clamp_min(1)
+    nn = norm.clamp_min(1e-6)
+    u = normal / nn
+    t = torch.nan_to_num(target)
+    cos = (u * t).sum(1, keepdim=True)
+    loss = weight * torch.where(valid, 1.0 - cos, torch.zeros_like(cos)).sum() / n
+    g = torch.where(valid, -(t - u * cos) / nn, torch.zeros_like(u)) * (weight * upstream / n)
+    angle = torch.where(valid, torch.rad2deg(torch.arccos(cos.clamp(-1, 1))), torch.zeros_like(cos)).sum() / n
+    return loss, g, angle
 
 
 def depth_loss_and_grad(depth, trans, target, weight, upstream=1.0):
@@ -128,17 +154,19 @@ def depth_loss_and_grad(depth, trans, target, weight, upstream=1.0):
 
 
 def train(root, iters=300, views_per_step=8, log=print, refine_poses=False, antialiased=False, filter_3d=False, exact_grad=False,
-          depth_weight=0.0, metrics=None):
-    """Returns (loss history, PSNR).  depth_weight > 0 adds the expected-depth term (the dataset must have depths/).
-    metrics (a dict, optional) receives "ed_error": mean |ED - target| over the known pixels of 8 training views, when the
-    dataset has depths."""
+          depth_weight=0.0, metrics=None, normal_weight=0.0):
+    """Returns (loss history, PSNR).  depth_weight > 0 adds the expected-depth term (the dataset must have depths/), normal_weight
+    > 0 the normal term (the dataset must have normals/).  metrics (a dict, optional) receives "ed_error": mean |ED - target| over
+    the known pixels of 8 training views, when the dataset has depths, and "normal_angle": their mean angle in degrees between
+    N / |N| and the target, when it has normals."""
     from litegs_b200 import fused
     if refine_poses and int(os.environ.get("WORLD_SIZE", "1")) > 1:
         raise ValueError("--refine-poses runs on one GPU: multi-GPU pose refinement is not supported")
     keep = fused.CONFIG["true_sigmoid_grad"]
     fused.CONFIG["true_sigmoid_grad"] = True               # our own loops train with the true sigmoid derivative (SURVEY Q15)
     try:
-        return _train(root, iters, views_per_step, log, refine_poses, antialiased, filter_3d, exact_grad, depth_weight, metrics)
+        return _train(root, iters, views_per_step, log, refine_poses, antialiased, filter_3d, exact_grad, depth_weight, metrics,
+                      normal_weight)
     finally:
         fused.CONFIG["true_sigmoid_grad"] = keep
 
@@ -176,7 +204,7 @@ class _Poses:
 
 
 def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=False, filter_3d=False, exact_grad=False,
-           depth_weight=0.0, metrics=None):
+           depth_weight=0.0, metrics=None, normal_weight=0.0):
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", 0)))
     torch.cuda.set_device(dev)
     frames, xyz, rgb = load_dataset(root, dev=dev)
@@ -184,13 +212,18 @@ def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=Fal
     if depth_weight > 0 and targets is None:
         raise ValueError(f"--depth-weight needs expected-depth targets in {os.path.join(root, 'depths')}")
     use_depth = depth_weight > 0
+    ntargets = load_depths(root, dev=dev, sub="normals")
+    if normal_weight > 0 and ntargets is None:
+        raise ValueError(f"--normal-weight needs unit-normal targets in {os.path.join(root, 'normals')}")
+    use_normal = normal_weight > 0
     H, W = frames[0][2]
     poses = _Poses(frames, (H, W), dev) if refine_poses else None
     extr0 = poses.extr.detach().clone() if poses else None
     cgrads = torch.empty((views_per_step, 2, 4, 4), dtype=torch.float32, device=dev) if poses else None
     g = colmap.gaussians_from_points(xyz, rgb, sh_degree=3)
     P = {k: torch.from_numpy(g[k]).to(dev) for k in PARAM_ORDER}
-    pp = PipelineParams(tile_size=(8, 16), sparse_grad=True, antialiased=antialiased, exact_grad=exact_grad, render_depth=use_depth)
+    pp = PipelineParams(tile_size=(8, 16), sparse_grad=True, antialiased=antialiased, exact_grad=exact_grad, render_depth=use_depth,
+                        render_normal=use_normal)
     acc = lgs_dist.GradAccumulator(P)
     extent = float(np.linalg.norm(xyz.max(0) - xyz.min(0)) * 0.5)
     opt, sched = optimizer.get_optimizer(P, spatial_lr_scale=extent)
@@ -219,10 +252,18 @@ def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=Fal
             ld, d_depth, d_trans = depth_loss_and_grad(depth, trans, targets[idx[i]], depth_weight, upstream=1.0 / views_per_step)
             return loss + ld, d_img, d_depth, d_trans
 
+        def with_normal_loss(i, img, depth, trans, normal):
+            if use_depth:
+                loss, d_img, d_depth, d_trans = colour_and_depth_loss(i, img, depth, trans)
+            else:
+                (loss, d_img), d_depth, d_trans = colour_loss(i, img), None, None
+            ln, d_normal, _ = normal_loss_and_grad(normal, ntargets[idx[i]], normal_weight, upstream=1.0 / views_per_step)
+            return loss + ln, d_img, d_depth, d_trans, d_normal
+
+        fn = with_normal_loss if use_normal else (colour_and_depth_loss if use_depth else colour_loss)
         losses = render.render_views(views_per_step, lambda i: cams[i], None, A[0], A[1], P["xyz"], P["scale"], P["rot"],
                                      P["sh_0"], P["sh_rest"], P["opacity"], 3, (H, W), pp, acc.grads(),
-                                     loss_and_grad_fn=colour_and_depth_loss if use_depth else colour_loss,
-                                     camera_grads=cgrads, filter_3d=filt)
+                                     loss_and_grad_fn=fn, camera_grads=cgrads, filter_3d=filt)
         opt.step(acc)
         if poses:
             poses.step(idx, cgrads)
@@ -233,21 +274,28 @@ def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=Fal
     torch.cuda.synchronize(dev)
     dt = time.perf_counter() - t0
     pp_eval = PipelineParams(tile_size=(8, 16), sparse_grad=True, antialiased=antialiased, render_depth=targets is not None,
-                             enable_transmitance=targets is not None)
+                             enable_transmitance=targets is not None, render_normal=ntargets is not None)
     with torch.no_grad():
-        mse, ed_err = [], []
+        mse, ed_err, n_err = [], [], []
         for j, (cam, gt, _) in enumerate(frames[:8]):
             cam = poses.cameras([j])[0] if poses else cam
-            img, trans, depth, _, _ = render.render_view(A[0], A[1], cam["frustumplane"], cam["view"], cam["proj"], P["xyz"], P["scale"],
-                                                         P["rot"], P["sh_0"], P["sh_rest"], P["opacity"], 3, (H, W), pp_eval, filter_3d=filt)
+            img, trans, depth, normal, _ = render.render_view(A[0], A[1], cam["frustumplane"], cam["view"], cam["proj"], P["xyz"],
+                                                              P["scale"], P["rot"], P["sh_0"], P["sh_rest"], P["opacity"], 3, (H, W),
+                                                              pp_eval, filter_3d=filt)
             mse.append(float(((img - gt) ** 2).mean()))
             if targets is not None:
                 ed_err.append(float(depth_loss_and_grad(depth, trans, targets[j], 1.0)[0]))
+            if ntargets is not None:
+                n_err.append(float(normal_loss_and_grad(normal, ntargets[j], 1.0)[2]))
     psnr = -10.0 * np.log10(np.mean(mse))
     if ed_err:
         log(f"expected-depth error over 8 training views: {np.mean(ed_err):.4f}")
         if metrics is not None:
             metrics["ed_error"] = float(np.mean(ed_err))
+    if n_err:
+        log(f"mean angle between N / |N| and the target normals over 8 training views: {np.mean(n_err):.2f} degrees")
+        if metrics is not None:
+            metrics["normal_angle"] = float(np.mean(n_err))
     log(f"{iters} iterations x {views_per_step} views in {dt:.1f} s ({iters * views_per_step / dt:.0f} views/s incl. loss + optimizer); "
         f"{xyz.shape[0]} Gaussians, PSNR over 8 training views {psnr:.2f} dB")
     if poses:
@@ -269,6 +317,9 @@ if __name__ == "__main__":
                     help="exact position and camera gradients: also through the ray-space Jacobian and the SH view direction")
     ap.add_argument("--depth-weight", type=float, default=0.0,
                     help="weight of the mean |expected depth - target| term (needs depths/<image stem>.npy, written by --make)")
+    ap.add_argument("--normal-weight", type=float, default=0.0,
+                    help="weight of the mean (1 - cos) term between N / |N| and the target normals (needs normals/<image stem>.npy, "
+                         "written by --make)")
     ap.add_argument("--pose-noise", type=float, nargs=2, default=None, metavar=("DEG", "FRAC"),
                     help="with --make: perturb the written poses by DEG degrees and FRAC of the camera distance")
     a = ap.parse_args()
@@ -278,5 +329,5 @@ if __name__ == "__main__":
     if root is None:
         ap.error("give --data or --make")
     h, _ = train(root, a.iters, refine_poses=a.refine_poses, antialiased=a.antialiased, filter_3d=a.filter_3d,
-                 exact_grad=a.exact_grad, depth_weight=a.depth_weight)
+                 exact_grad=a.exact_grad, depth_weight=a.depth_weight, normal_weight=a.normal_weight)
     assert h[-1] < h[0]

@@ -19,3 +19,5 @@ class PipelineParams:
     # ours as well: per-pixel depth on the fused path (DESIGN.md section 1, "Depth"), read as getattr(pp, "render_depth", False);
     # enable_depth above keeps the reference's meaning
     render_depth: bool = False
+    # ours as well: per-pixel normals on the fused path (DESIGN.md section 1, "Normals"), read as getattr(pp, "render_normal", False)
+    render_normal: bool = False

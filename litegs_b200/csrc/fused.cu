@@ -161,6 +161,41 @@ __device__ __forceinline__ void project_chain(const float* __restrict__ Vm, cons
     t.inv[0] = c11 * dr; t.inv[1] = -c01 * dr; t.inv[2] = c00 * dr;
 }
 
+// d qn of a gradient dR of fused_quat_R's rows (its derivative; the same formulas as the quaternion backward of
+// project_backward_kernel, which keeps its own inline copy).
+__device__ __forceinline__ void fused_quat_R_backward(float r, float x, float y, float z, const float* dT, float* dq)
+{
+    dq[0] = 2 * z * (dT[1] - dT[3]) + 2 * y * (dT[6] - dT[2]) + 2 * x * (dT[5] - dT[7]);
+    dq[1] = 2 * y * (dT[3] + dT[1]) + 2 * z * (dT[6] + dT[2]) + 2 * r * (dT[5] - dT[7]) - 4 * x * (dT[8] + dT[4]);
+    dq[2] = 2 * x * (dT[3] + dT[1]) + 2 * r * (dT[6] - dT[2]) + 2 * z * (dT[5] + dT[7]) - 4 * y * (dT[8] + dT[0]);
+    dq[3] = 2 * r * (dT[1] - dT[3]) + 2 * x * (dT[6] + dT[2]) + 2 * y * (dT[5] + dT[7]) - 4 * z * (dT[4] + dT[0]);
+}
+
+// Normals (DESIGN.md section 1, "Normals"): the view-space normal of the shortest scale axis, turned to face the camera.
+// ax = argmin of the RAW log-scales (first index wins a tie; the 3D filter never changes it), n_w = row ax of R,
+// n_c[j] = (n_w0 V[0][j] + n_w1 V[1][j]) + n_w2 V[2][j], sg = -1 if (n_c0 v0 + n_c1 v1) + n_c2 v2 > 0 else +1; n = sg n_c.
+// n_c and the facing test are single-rounded ops in this order, so that tests/normal_oracle.py reproduces sg bit for bit.
+// R is indexed with selects: a dynamic index would put the array in local memory.
+struct NormalFrame {
+    float nw[3], nc[3], sg;
+    int ax;
+};
+
+__device__ __forceinline__ void normal_frame(const float* s_raw, const float* R, const float* __restrict__ Vm, const float* v,
+                                             NormalFrame& f)
+{
+    int ax = (s_raw[1] < s_raw[0]) ? 1 : 0;
+    ax = (s_raw[2] < (ax == 1 ? s_raw[1] : s_raw[0])) ? 2 : ax;
+    f.ax = ax;
+#pragma unroll
+    for (int k = 0; k < 3; k++) f.nw[k] = (ax == 0) ? R[k] : ((ax == 1) ? R[3 + k] : R[6 + k]);
+#pragma unroll
+    for (int j = 0; j < 3; j++)
+        f.nc[j] = __fadd_rn(__fadd_rn(__fmul_rn(f.nw[0], Vm[j]), __fmul_rn(f.nw[1], Vm[4 + j])), __fmul_rn(f.nw[2], Vm[8 + j]));
+    const float dv = __fadd_rn(__fadd_rn(__fmul_rn(f.nc[0], v[0]), __fmul_rn(f.nc[1], v[1])), __fmul_rn(f.nc[2], v[2]));
+    f.sg = (dv > 0.0f) ? -1.0f : 1.0f;
+}
+
 // Antialiased mode (DESIGN.md section 1): the opacity compensation of the 2D low-pass filter,
 // rho = sqrt(det(M^T M) / det(M^T M + 0.3 I)).  Every step is one correctly rounded op in a fixed order, so that the
 // opacity the tile decision sees is the oracle's bit for bit.
@@ -187,14 +222,16 @@ __device__ __forceinline__ void antialias_factor(const float* M, AAFactor& f)
 // grid = allocated chunks (all M: chunks >= *visible_num write an invisible record), block = chunk size
 // AA: the record's opacity is sigma(o_raw) * rho (antialiased mode); everything downstream reads it from the record.
 // F3D: the 3D smoothing filter filter_3d[src] widens the scale and scales the opacity by rho3 before AA sees either.
-template <int DEG, int TH, int TW, bool AA, bool F3D>
+// NORMAL: also the camera-facing view-space normal n of the shortest axis (normal_frame) into normal_rec f32[A*S,4] as
+// (n0, n1, n2, 0); slots of chunks at or past the visible count get zeros, as their record does.
+template <int DEG, int TH, int TW, bool AA, bool F3D, bool NORMAL = false>
 __global__ void project_forward_kernel(
     const int64_t* __restrict__ chunk_ids, const int* __restrict__ visible_num, const float* __restrict__ view,
     const float* __restrict__ proj, const float* __restrict__ pos, const float* __restrict__ scale,
     const float* __restrict__ rot, const float* __restrict__ sh0, const float* __restrict__ shr,
     const float* __restrict__ opac, int C, int S, int H, int W, int gx, int gy, SplatRec* __restrict__ recs,
     unsigned* __restrict__ depth_key, unsigned* __restrict__ iota, int* __restrict__ tile_count, int* __restrict__ totals,
-    const float* __restrict__ filter_3d)
+    const float* __restrict__ filter_3d, float4* __restrict__ normal_rec)
 {
     const int a = blockIdx.x, s = threadIdx.x;
     const size_t dst = (size_t)a * S + s;
@@ -202,6 +239,7 @@ __global__ void project_forward_kernel(
     unsigned key = 0xFFFFFFFFu;
     SplatRec r;
     r.px = r.py = 0.f; r.A = r.B = r.C = 0.f; r.o = 0.f; r.r = r.g = r.b = 0.f; r.depth = 0.f; r.pad0 = r.pad1 = 0.f;
+    float4 nrm = make_float4(0.f, 0.f, 0.f, 0.f);
     if (a < visible_num[0]) {
         const size_t CS = (size_t)C * S;
         const size_t src = (size_t)chunk_ids[a] * S + s;
@@ -219,6 +257,11 @@ __global__ void project_forward_kernel(
             AAFactor f;
             antialias_factor(t.M, f);
             t.o = __fmul_rn(t.o, f.rho);
+        }
+        if constexpr (NORMAL) {
+            NormalFrame nf;
+            normal_frame(sr_, t.R, view, t.v, nf);
+            nrm = make_float4(nf.sg * nf.nc[0], nf.sg * nf.nc[1], nf.sg * nf.nc[2], 0.f);
         }
         // colour (GR/compact.cu:573-653), no clamp on this path (SURVEY Q13)
         constexpr int K = (DEG + 1) * (DEG + 1);
@@ -244,6 +287,7 @@ __global__ void project_forward_kernel(
         (void)ndcz;
     }
     recs[dst] = r;
+    if constexpr (NORMAL) normal_rec[dst] = nrm;
     depth_key[dst] = key;
     iota[dst] = (unsigned)dst;
     tile_count[dst] = count;
@@ -273,12 +317,25 @@ __global__ void project_forward_kernel(
     }
 }
 
-extern "C" int lgs_project_forward(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
-                                   const float* view_matrix, const float* proj_matrix, const float* position,
-                                   const float* scale, const float* rotation, const float* sh_base, const float* sh_rest,
-                                   const float* opacity, int C, int S, int A, int img_h, int img_w, int tile_h, int tile_w,
-                                   float* packed_params, unsigned* depth_key, unsigned* iota, int* tile_count, int* totals,
-                                   const float* filter_3d, int antialiased, void* stream)
+// Largest block a NORMAL instantiation of project_forward_kernel can be launched with: the heaviest use 72 registers, which
+// allows 896 threads instead of 1024 (DESIGN.md section 1, "Normals").  Read once per instantiation, on its first (eager) use.
+template <int DEG, int TH, int TW, bool AA, bool F3D>
+static int project_forward_normal_max_threads()
+{
+    static const int n = [] {
+        cudaFuncAttributes a;
+        return cudaFuncGetAttributes(&a, project_forward_kernel<DEG, TH, TW, AA, F3D, true>) == cudaSuccess ? a.maxThreadsPerBlock : 0;
+    }();
+    return n;
+}
+
+// normal_rec f32[A*S,4] or NULL: normal mode, the camera-facing view-space normal of each record (DESIGN.md section 1, "Normals").
+extern "C" int lgs_project_forward_normal(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
+                                          const float* view_matrix, const float* proj_matrix, const float* position,
+                                          const float* scale, const float* rotation, const float* sh_base, const float* sh_rest,
+                                          const float* opacity, int C, int S, int A, int img_h, int img_w, int tile_h, int tile_w,
+                                          float* packed_params, unsigned* depth_key, unsigned* iota, int* tile_count, int* totals,
+                                          const float* filter_3d, int antialiased, float* normal_rec, void* stream)
 {
     LGS_REQUIRE(sh_degree >= 0 && sh_degree <= 3, "project_forward: sh_degree %d not in 0..3", sh_degree);
     LGS_REQUIRE(lgs_tile_ok(tile_h, tile_w), "project_forward: tile %dx%d not one of 8x16, 12x16, 16x16, 8x8", tile_h, tile_w);
@@ -287,20 +344,42 @@ extern "C" int lgs_project_forward(int sh_degree, const int64_t* visible_chunk_i
     LGS_CUDA(cudaMemsetAsync(totals, 0, 3 * sizeof(int), st));
     if (A == 0) return LGS_OK;
     int gx = (img_w + tile_w - 1) / tile_w, gy = (img_h + tile_h - 1) / tile_h;
-#define PF(D, AA, F3) project_forward_kernel<D, TH, TW, AA, F3><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num, view_matrix,  \
-        proj_matrix, position, scale, rotation, sh_base, sh_rest, opacity, C, S, img_h, img_w, gx, gy, (SplatRec*)packed_params,     \
-        depth_key, iota, tile_count, totals, filter_3d)
-#define PF_DEG(AA, F3) LGS_DISPATCH_TILE(tile_h, tile_w,                                                                            \
-        switch (sh_degree) { case 0: PF(0, AA, F3); break; case 1: PF(1, AA, F3); break; case 2: PF(2, AA, F3); break; default: PF(3, AA, F3); })
-    if (filter_3d != nullptr) {
-        if (antialiased) { PF_DEG(true, true) } else { PF_DEG(false, true) }
-    } else {
-        if (antialiased) { PF_DEG(true, false) } else { PF_DEG(false, false) }
+#define PF(D, AA, F3, NM) {                                                                                                         \
+        if constexpr (NM) {                                                                                                         \
+            const int mt = project_forward_normal_max_threads<D, TH, TW, AA, F3>();                                                 \
+            LGS_REQUIRE(S <= mt, "project_forward: normals with this configuration support chunk sizes up to %d, got %d", mt, S); \
+        }                                                                                                                           \
+        project_forward_kernel<D, TH, TW, AA, F3, NM><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num,                        \
+        view_matrix, proj_matrix, position, scale, rotation, sh_base, sh_rest, opacity, C, S, img_h, img_w, gx, gy,                  \
+        (SplatRec*)packed_params, depth_key, iota, tile_count, totals, filter_3d, (float4*)normal_rec); }
+#define PF_DEG(AA, F3, NM) LGS_DISPATCH_TILE(tile_h, tile_w,                                                                        \
+        switch (sh_degree) { case 0: PF(0, AA, F3, NM); break; case 1: PF(1, AA, F3, NM); break; case 2: PF(2, AA, F3, NM); break;   \
+                             default: PF(3, AA, F3, NM); })
+#define PF_MODE(NM)                                                                                                                 \
+    if (filter_3d != nullptr) {                                                                                                     \
+        if (antialiased) { PF_DEG(true, true, NM) } else { PF_DEG(false, true, NM) }                                                \
+    } else {                                                                                                                        \
+        if (antialiased) { PF_DEG(true, false, NM) } else { PF_DEG(false, false, NM) }                                              \
     }
+    if (normal_rec != nullptr) { PF_MODE(true) } else { PF_MODE(false) }
+#undef PF_MODE
 #undef PF_DEG
 #undef PF
     LGS_CHECK_LAUNCH("project_forward_kernel");
     return LGS_OK;
+}
+
+// The form without normals: lgs_project_forward_normal with normal_rec = NULL.
+extern "C" int lgs_project_forward(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
+                                   const float* view_matrix, const float* proj_matrix, const float* position,
+                                   const float* scale, const float* rotation, const float* sh_base, const float* sh_rest,
+                                   const float* opacity, int C, int S, int A, int img_h, int img_w, int tile_h, int tile_w,
+                                   float* packed_params, unsigned* depth_key, unsigned* iota, int* tile_count, int* totals,
+                                   const float* filter_3d, int antialiased, void* stream)
+{
+    return lgs_project_forward_normal(sh_degree, visible_chunk_id, visible_chunks_num, view_matrix, proj_matrix, position, scale,
+                                      rotation, sh_base, sh_rest, opacity, C, S, A, img_h, img_w, tile_h, tile_w, packed_params,
+                                      depth_key, iota, tile_count, totals, filter_3d, antialiased, nullptr, stream);
 }
 
 // (tile+1, splat) emission in depth order from the packed record.    replaces GR/binning.cu:33-110
@@ -494,7 +573,11 @@ __device__ __forceinline__ float warp_sum32_transposed(float* v)
 // active degree).  The other gradients are the same instructions as without it.
 // DEPTH: depth mode.  Record slot LGS_GRAD_DEPTH (d view-space z) joins dv.z: it reaches d xyz through V and the camera gradient as
 // dV[k][2] += p~_k dz, and nothing reaches d proj.  A Gaussian whose only gradient is that slot is not skipped.
-template <int DEG, bool CAM, bool AA, bool F3D, bool EXACT, bool DEPTH>
+// NORMAL: normal mode.  grad_normal f32[A*S,4] (dL/dn from the raster backward) gives dn_c = sg dn and dn_w = V3x3 dn_c, which is
+// added to row ax of the rotation-matrix gradient (dT after its product with s) and so reaches rot; with CAM,
+// dV[k][j] += n_w[k] dn_c[j] (k, j < 3).  Nothing reaches xyz, the scales or d proj; ax and sg are held constant.  A Gaussian
+// whose only gradient is a normal row is not skipped.
+template <int DEG, bool CAM, bool AA, bool F3D, bool EXACT, bool DEPTH, bool NORMAL = false>
 __global__ void project_backward_kernel(
     const int64_t* __restrict__ chunk_ids, const int* __restrict__ visible_num, const float* __restrict__ view,
     const float* __restrict__ proj, const float* __restrict__ pos, const float* __restrict__ scale,
@@ -502,7 +585,7 @@ __global__ void project_backward_kernel(
     int true_sigmoid, int accumulate, const float* __restrict__ grad /*[A*S,12]*/, const float* __restrict__ inv_scaler,
     float* __restrict__ g_pos, float* __restrict__ g_scale, float* __restrict__ g_rot, float* __restrict__ g_sh0,
     float* __restrict__ g_shr, float* __restrict__ g_opac, float* __restrict__ touched, float* __restrict__ cam_partials,
-    const float* __restrict__ filter_3d, const float* __restrict__ shr)
+    const float* __restrict__ filter_3d, const float* __restrict__ shr, const float4* __restrict__ grad_normal)
 {
     const int a = blockIdx.x, s = threadIdx.x;
     if (a >= visible_num[0]) {
@@ -518,8 +601,10 @@ __global__ void project_backward_kernel(
     const float sc = inv_scaler ? inv_scaler[0] : 1.0f;
     const float4* g4 = reinterpret_cast<const float4*>(grad + dst * LGS_GRAD_FLOATS);
     const float4 ga = g4[0], gb = g4[1], gc = g4[2];
+    const float4 gn = NORMAL ? grad_normal[dst] : make_float4(0.f, 0.f, 0.f, 0.f);
     const bool any = (ga.x != 0.f) | (ga.y != 0.f) | (ga.z != 0.f) | (ga.w != 0.f) | (gb.x != 0.f) | (gb.y != 0.f) |
-                     (gb.z != 0.f) | (gb.w != 0.f) | (gc.x != 0.f) | (DEPTH && gc.z != 0.f);
+                     (gb.z != 0.f) | (gb.w != 0.f) | (gc.x != 0.f) | (DEPTH && gc.z != 0.f) |
+                     (NORMAL && ((gn.x != 0.f) | (gn.y != 0.f) | (gn.z != 0.f)));
     float o_pos[3] = { 0.f, 0.f, 0.f }, o_sc[3] = { 0.f, 0.f, 0.f }, o_q[4] = { 0.f, 0.f, 0.f, 0.f }, o_op = 0.f;
     float shb[16], dcol3[3] = { 0.f, 0.f, 0.f };       // SH basis and colour gradient: d sh[k][c] = shb[k] * dcol3[c]
 #pragma unroll
@@ -592,6 +677,23 @@ __global__ void project_backward_kernel(
             ds[r] = t.R[r * 3] * dT[r * 3] + t.R[r * 3 + 1] * dT[r * 3 + 1] + t.R[r * 3 + 2] * dT[r * 3 + 2];
             dT[r * 3] *= t.s[r]; dT[r * 3 + 1] *= t.s[r]; dT[r * 3 + 2] *= t.s[r];
         }
+        NormalFrame nf;
+        float dnc[3], dqn[4];
+        if constexpr (NORMAL) {
+            // the rotation-matrix gradient of the normal term: row ax is dn_w[k] = sum_j V[k][j] dn_c[j] with dn_c = sg dn, the
+            // other rows zero.  It goes through its own quaternion backward and is added to the rot gradient at the end: by
+            // linearity the same as adding it to dT here, and the other terms keep their instructions (g_N = 0 leaves their bits).
+            normal_frame(sr_, t.R, view, t.v, nf);
+            dnc[0] = nf.sg * (gn.x * sc); dnc[1] = nf.sg * (gn.y * sc); dnc[2] = nf.sg * (gn.z * sc);
+            float dRn[9];
+#pragma unroll
+            for (int k = 0; k < 3; k++) {
+                const float dnw = view[k * 4] * dnc[0] + view[k * 4 + 1] * dnc[1] + view[k * 4 + 2] * dnc[2];
+#pragma unroll
+                for (int r = 0; r < 3; r++) dRn[r * 3 + k] = (r == nf.ax) ? dnw : 0.0f;
+            }
+            fused_quat_R_backward(t.qn[0], t.qn[1], t.qn[2], t.qn[3], dRn, dqn);
+        }
         const float r_ = t.qn[0], x = t.qn[1], y = t.qn[2], z = t.qn[3];
         float dq[4];
         dq[0] = 2 * z * (dT[1] - dT[3]) + 2 * y * (dT[6] - dT[2]) + 2 * x * (dT[5] - dT[7]);
@@ -613,6 +715,11 @@ __global__ void project_backward_kernel(
         const float dot = dq[0] * t.qn[0] + dq[1] * t.qn[1] + dq[2] * t.qn[2] + dq[3] * t.qn[3];
 #pragma unroll
         for (int k = 0; k < 4; k++) o_q[k] = t.rn * (dq[k] - dot * t.qn[k]);
+        if constexpr (NORMAL) {
+            const float dotn = dqn[0] * t.qn[0] + dqn[1] * t.qn[1] + dqn[2] * t.qn[2] + dqn[3] * t.qn[3];
+#pragma unroll
+            for (int k = 0; k < 4; k++) o_q[k] = __fadd_rn(o_q[k], t.rn * (dqn[k] - dotn * t.qn[k]));   // no contraction into o_q
+        }
         const float sig = 1.0f - 1.0f / (1.0f + expf(o_raw));
         o_op = d_o * (true_sigmoid ? sig * (1.0f - sig) : sig);
         // MVP backward (GR/transform.cu:517-558) with d_ndc.z = d_ndc.w = 0 and no view-space gradient
@@ -665,6 +772,13 @@ __global__ void project_backward_kernel(
                     dVJ[c] = t.R[r] * t.s[0] * dM[c] + t.R[3 + r] * t.s[1] * dM[2 + c] + t.R[6 + r] * t.s[2] * dM[4 + c];
 #pragma unroll
                 for (int k = 0; k < 3; k++) cam[r * 4 + k] += dVJ[0] * J[k * 2] + dVJ[1] * J[k * 2 + 1];
+            }
+            if constexpr (NORMAL) {
+                // n_c[j] = sum_k n_w[k] V[k][j]  ->  dV[k][j] += n_w[k] dn_c[j]
+#pragma unroll
+                for (int k = 0; k < 3; k++)
+#pragma unroll
+                    for (int j = 0; j < 3; j++) cam[k * 4 + j] = __fmaf_rn(nf.nw[k], dnc[j], cam[k * 4 + j]);
             }
         }
         // SH coefficients (GR/compact.cu:655-823); the direction is treated as constant
@@ -782,15 +896,16 @@ __global__ void __launch_bounds__(1024) camera_grad_sum_kernel(const float* __re
     }
 }
 
-// Largest block an EXACT instantiation can be launched with.  The kernel has no launch bounds (the default instantiations
-// must keep their code), and the heaviest EXACT ones use up to 168 registers, which allows 384 threads instead of 1024
-// (DESIGN.md section 1, "Exact gradient mode").  Read once per instantiation, on its first (eager) use.
-template <int DEG, bool CAM, bool AA, bool F3D, bool DEPTH>
-static int project_backward_exact_max_threads()
+// Largest block an EXACT or NORMAL instantiation can be launched with.  The kernel has no launch bounds (the default
+// instantiations must keep their code), and the heaviest EXACT ones use up to 168 registers, which allows 384 threads instead of
+// 1024 (DESIGN.md section 1, "Exact gradient mode"); NORMAL instantiations use up to 138 without EXACT (DESIGN.md section 1,
+// "Normals").  Read once per instantiation, on its first (eager) use.
+template <int DEG, bool CAM, bool AA, bool F3D, bool EXACT, bool DEPTH, bool NORMAL>
+static int project_backward_max_threads()
 {
     static const int n = [] {
         cudaFuncAttributes a;
-        return cudaFuncGetAttributes(&a, project_backward_kernel<DEG, CAM, AA, F3D, true, DEPTH>) == cudaSuccess ? a.maxThreadsPerBlock : 0;
+        return cudaFuncGetAttributes(&a, project_backward_kernel<DEG, CAM, AA, F3D, EXACT, DEPTH, NORMAL>) == cudaSuccess ? a.maxThreadsPerBlock : 0;
     }();
     return n;
 }
@@ -799,14 +914,16 @@ static int project_backward_exact_max_threads()
 // sh_rest rows above the active degree must read as zero); mode 2: outputs are the DENSE [..,C,S] gradient tensors and
 // this view's gradients are accumulated into them (the multi-view / data-parallel path: no compacted round trip).
 // depth: 1 = the record gradient carries a depth slot (lgs_rasterize_backward was given d_depth), 0 = it does not.
-extern "C" int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
-                                    const float* view_matrix, const float* proj_matrix, const float* position,
-                                    const float* scale, const float* rotation, const float* opacity, int C, int S, int A,
-                                    int rest_dim, int img_h, int img_w, int true_sigmoid_grad, const float* packed_grad,
-                                    const float* grad_inv_scaler, int zero_outputs, float* g_position, float* g_scale,
-                                    float* g_rotation, float* g_sh_base, float* g_sh_rest, float* g_opacity, float* touched,
-                                    float* cam_partials, float* d_cam, const float* filter_3d, int antialiased,
-                                    const float* sh_base, const float* sh_rest, int exact_grad, int depth, void* stream)
+// grad_normal: f32[A*S,4] normal gradient of lgs_rasterize_backward (normal mode), or NULL = no normal term.
+extern "C" int lgs_project_backward_normal(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
+                                           const float* view_matrix, const float* proj_matrix, const float* position,
+                                           const float* scale, const float* rotation, const float* opacity, int C, int S, int A,
+                                           int rest_dim, int img_h, int img_w, int true_sigmoid_grad, const float* packed_grad,
+                                           const float* grad_inv_scaler, int zero_outputs, float* g_position, float* g_scale,
+                                           float* g_rotation, float* g_sh_base, float* g_sh_rest, float* g_opacity, float* touched,
+                                           float* cam_partials, float* d_cam, const float* filter_3d, int antialiased,
+                                           const float* sh_base, const float* sh_rest, int exact_grad, int depth,
+                                           const float* grad_normal, void* stream)
 {
     LGS_REQUIRE(sh_degree >= 0 && sh_degree <= 3, "project_backward: sh_degree %d not in 0..3", sh_degree);
     LGS_REQUIRE(rest_dim >= (sh_degree + 1) * (sh_degree + 1) - 1, "project_backward: sh_rest has %d rows, degree %d needs %d", rest_dim,
@@ -833,29 +950,32 @@ extern "C" int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_
         LGS_CUDA(cudaMemsetAsync(g_sh_rest, 0, sizeof(float) * (size_t)rest_dim * 3 * AS, st));
         LGS_CUDA(cudaMemsetAsync(g_opacity, 0, sizeof(float) * AS, st));
     }
-#define PB(D, K, AA, F3, EX, Z) {                                                                                                   \
-        if constexpr (EX) {                                                                                                         \
-            const int mt = project_backward_exact_max_threads<D, K, AA, F3, Z>();                                                   \
-            LGS_REQUIRE(S <= mt, "project_backward: exact_grad with this configuration supports chunk sizes up to %d, got %d", mt, S); \
+#define PB(D, K, AA, F3, EX, Z, NM) {                                                                                               \
+        if constexpr (EX || NM) {                                                                                                   \
+            const int mt = project_backward_max_threads<D, K, AA, F3, EX, Z, NM>();                                                 \
+            LGS_REQUIRE(S <= mt, "project_backward: %s with this configuration supports chunk sizes up to %d, got %d",            \
+                        EX ? "exact_grad" : "the normal gradient", mt, S);                                                          \
         }                                                                                                                           \
-        project_backward_kernel<D, K, AA, F3, EX, Z><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num,                         \
+        project_backward_kernel<D, K, AA, F3, EX, Z, NM><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num,                     \
         view_matrix, proj_matrix, position, scale, rotation, opacity, C, S, A, rest_dim, img_h, img_w, true_sigmoid_grad, accumulate,  \
         packed_grad, grad_inv_scaler, g_position, g_scale, g_rotation, g_sh_base, g_sh_rest, g_opacity, touched, cam_partials,        \
-        filter_3d, sh_rest); }
-#define PB_DEG(K, AA, F3, EX, Z) switch (sh_degree) { case 0: PB(0, K, AA, F3, EX, Z); break; case 1: PB(1, K, AA, F3, EX, Z); break; \
-                                                      case 2: PB(2, K, AA, F3, EX, Z); break; default: PB(3, K, AA, F3, EX, Z); }
-#define PB_CAM(AA, F3, EX, Z) if (cam) { PB_DEG(true, AA, F3, EX, Z) } else { PB_DEG(false, AA, F3, EX, Z) }
-#define PB_MODE(EX, Z)                                                                                                              \
+        filter_3d, sh_rest, (const float4*)grad_normal); }
+#define PB_DEG(K, AA, F3, EX, Z, NM) switch (sh_degree) { case 0: PB(0, K, AA, F3, EX, Z, NM); break; case 1: PB(1, K, AA, F3, EX, Z, NM); break; \
+                                                          case 2: PB(2, K, AA, F3, EX, Z, NM); break; default: PB(3, K, AA, F3, EX, Z, NM); }
+#define PB_CAM(AA, F3, EX, Z, NM) if (cam) { PB_DEG(true, AA, F3, EX, Z, NM) } else { PB_DEG(false, AA, F3, EX, Z, NM) }
+#define PB_MODE(EX, Z, NM)                                                                                                          \
     if (filter_3d != nullptr) {                                                                                                     \
-        if (antialiased) { PB_CAM(true, true, EX, Z) } else { PB_CAM(false, true, EX, Z) }                                          \
+        if (antialiased) { PB_CAM(true, true, EX, Z, NM) } else { PB_CAM(false, true, EX, Z, NM) }                                  \
     } else {                                                                                                                        \
-        if (antialiased) { PB_CAM(true, false, EX, Z) } else { PB_CAM(false, false, EX, Z) }                                        \
+        if (antialiased) { PB_CAM(true, false, EX, Z, NM) } else { PB_CAM(false, false, EX, Z, NM) }                                \
     }
-    if (depth) {
-        if (exact_grad) { PB_MODE(true, true) } else { PB_MODE(false, true) }
+#define PB_DEPTH(EX, NM) if (depth) { PB_MODE(EX, true, NM) } else { PB_MODE(EX, false, NM) }
+    if (grad_normal != nullptr) {
+        if (exact_grad) { PB_DEPTH(true, true) } else { PB_DEPTH(false, true) }
     } else {
-        if (exact_grad) { PB_MODE(true, false) } else { PB_MODE(false, false) }
+        if (exact_grad) { PB_DEPTH(true, false) } else { PB_DEPTH(false, false) }
     }
+#undef PB_DEPTH
 #undef PB_MODE
 #undef PB_CAM
 #undef PB_DEG
@@ -866,6 +986,23 @@ extern "C" int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_
         LGS_CHECK_LAUNCH("camera_grad_sum_kernel");
     }
     return LGS_OK;
+}
+
+// The form without normals: lgs_project_backward_normal with grad_normal = NULL.
+extern "C" int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
+                                    const float* view_matrix, const float* proj_matrix, const float* position,
+                                    const float* scale, const float* rotation, const float* opacity, int C, int S, int A,
+                                    int rest_dim, int img_h, int img_w, int true_sigmoid_grad, const float* packed_grad,
+                                    const float* grad_inv_scaler, int zero_outputs, float* g_position, float* g_scale,
+                                    float* g_rotation, float* g_sh_base, float* g_sh_rest, float* g_opacity, float* touched,
+                                    float* cam_partials, float* d_cam, const float* filter_3d, int antialiased,
+                                    const float* sh_base, const float* sh_rest, int exact_grad, int depth, void* stream)
+{
+    return lgs_project_backward_normal(sh_degree, visible_chunk_id, visible_chunks_num, view_matrix, proj_matrix, position, scale,
+                                       rotation, opacity, C, S, A, rest_dim, img_h, img_w, true_sigmoid_grad, packed_grad,
+                                       grad_inv_scaler, zero_outputs, g_position, g_scale, g_rotation, g_sh_base, g_sh_rest, g_opacity,
+                                       touched, cam_partials, d_cam, filter_3d, antialiased, sh_base, sh_rest, exact_grad, depth,
+                                       nullptr, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -93,6 +93,53 @@ __device__ __forceinline__ void blend_pixel_depth(float a, float cr, float cg, f
         : "+f"(Ts), "+f"(Cr), "+f"(Cg), "+f"(Cb), "+f"(D), "+f"(nf)
         : "f"(a), "f"(cr), "f"(cg), "f"(cb), "f"(ts_min), "f"(a_min), "f"(neg_ki), "f"(z));
 }
+// blend_pixel plus the normal channels (DESIGN.md section 1, "Normals"): N += n w, three more predicated FMAs, before the
+// transmittance update; with DEPTH the depth FMA comes first, as in blend_pixel_depth.
+template <bool DEPTH>
+__device__ __forceinline__ void blend_pixel_normal(float a, float cr, float cg, float cb, float z, float n0, float n1, float n2,
+                                                   float& Ts, float& Cr, float& Cg, float& Cb, float& D, float& N0, float& N1,
+                                                   float& N2, float& nf, float ts_min, float a_min, float neg_ki)
+{
+    if (DEPTH) {
+        asm("{\n"
+            ".reg .pred pa, pk;\n"
+            ".reg .f32 w;\n"
+            "setp.gt.f32 pa, %0, %13;\n"
+            "@pa add.f32 %8, %8, 0f3F800000;\n"
+            "setp.ge.and.f32 pk, %9, %14, pa;\n"
+            "mul.f32 w, %9, %0;\n"
+            "@pk fma.rn.f32 %1, %10, w, %1;\n"
+            "@pk fma.rn.f32 %2, %11, w, %2;\n"
+            "@pk fma.rn.f32 %3, %12, w, %3;\n"
+            "@pk fma.rn.f32 %4, %16, w, %4;\n"
+            "@pk fma.rn.f32 %5, %17, w, %5;\n"
+            "@pk fma.rn.f32 %6, %18, w, %6;\n"
+            "@pk fma.rn.f32 %7, %19, w, %7;\n"
+            "@pk fma.rn.f32 %0, %15, w, %0;\n"
+            "}\n"
+            : "+f"(Ts), "+f"(Cr), "+f"(Cg), "+f"(Cb), "+f"(D), "+f"(N0), "+f"(N1), "+f"(N2), "+f"(nf)
+            : "f"(a), "f"(cr), "f"(cg), "f"(cb), "f"(ts_min), "f"(a_min), "f"(neg_ki), "f"(z), "f"(n0), "f"(n1), "f"(n2));
+    } else {
+        asm("{\n"
+            ".reg .pred pa, pk;\n"
+            ".reg .f32 w;\n"
+            "setp.gt.f32 pa, %0, %12;\n"
+            "@pa add.f32 %7, %7, 0f3F800000;\n"
+            "setp.ge.and.f32 pk, %8, %13, pa;\n"
+            "mul.f32 w, %8, %0;\n"
+            "@pk fma.rn.f32 %1, %9, w, %1;\n"
+            "@pk fma.rn.f32 %2, %10, w, %2;\n"
+            "@pk fma.rn.f32 %3, %11, w, %3;\n"
+            "@pk fma.rn.f32 %4, %15, w, %4;\n"
+            "@pk fma.rn.f32 %5, %16, w, %5;\n"
+            "@pk fma.rn.f32 %6, %17, w, %6;\n"
+            "@pk fma.rn.f32 %0, %14, w, %0;\n"
+            "}\n"
+            : "+f"(Ts), "+f"(Cr), "+f"(Cg), "+f"(Cb), "+f"(N0), "+f"(N1), "+f"(N2), "+f"(nf)
+            : "f"(a), "f"(cr), "f"(cg), "f"(cb), "f"(ts_min), "f"(a_min), "f"(neg_ki), "f"(n0), "f"(n1), "f"(n2));
+    }
+    (void)z; (void)D;
+}
 
 // ---- asynchronous staging primitives -------------------------------------------------------------
 __device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
@@ -155,8 +202,12 @@ struct Stager {
         }
     }
     // lane `lane` stages record `id` (or nothing when id < 0) into slot `lane` of buffer `which`.
-    __device__ __forceinline__ void issue(int which, const SplatRec* __restrict__ recs, int id)
+    // NORMAL (cp.async only): also the 16-byte side row nrec[id] into slot `lane` of nbuf[which], in the same group.
+    template <bool NORMAL = false>
+    __device__ __forceinline__ void issue(int which, const SplatRec* __restrict__ recs, int id, const float4* __restrict__ nrec = nullptr,
+                                          float4* nbuf = nullptr)
     {
+        static_assert(!(NORMAL && BULK), "the normal rows are staged with cp.async only");
         SplatRec* dst = buf + which * 32 + lane;
         if (BULK) {
             unsigned live = __ballot_sync(FULL_MASK, id >= 0);
@@ -170,6 +221,7 @@ struct Stager {
                 cp_async16((char*)dst, src);
                 cp_async16((char*)dst + 16, src + 16);
                 cp_async16((char*)dst + 32, src + 32);
+                if (NORMAL) cp_async16(nbuf + which * 32 + lane, nrec + id);
             }
             cp_async_commit();
         }
@@ -240,16 +292,20 @@ __global__ void pack_kernel(const float* __restrict__ ndc, const float* __restri
 // PAIRS: blend the lane's pixels two at a time (add2/mul2/fma2; A/B switch, lgs_set_forward_pairs / env LGS_FWD_PAIRS).
 // DEPTH: also D = sum w z (the record's view-space z, DESIGN.md section 1 "Depth") into depth_out f32[V,1,Hp,Wp], unclamped;
 // built on the default form only (scalar body, cp.async staging).
-template <int TH, int TW, bool STAT, bool BULK, bool PAIRS = false, bool DEPTH = false>
+// NORMAL: also N = sum w n (DESIGN.md section 1 "Normals") into normal_out f32[V,3,Hp,Wp], unclamped and not normalised; n is the
+// side row nrec f32[V*N,4] of each record, staged with one more cp.async beside it.  Default form only, as DEPTH.
+template <int TH, int TW, bool STAT, bool BULK, bool PAIRS = false, bool DEPTH = false, bool NORMAL = false>
 __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_forward_kernel(
     const int* __restrict__ sorted, const int* __restrict__ start_index, const SplatRec* __restrict__ recs,
     const int* __restrict__ tiles, int n_sel, float* __restrict__ img, float* __restrict__ Tout, unsigned short* __restrict__ last,
     int* __restrict__ frag_count, float* __restrict__ frag_weight, int* __restrict__ tile_work, int gx, int ntile, int cap, int N,
-    int Hp, int Wp, int clamp_zero, float* __restrict__ depth_out)
+    int Hp, int Wp, int clamp_zero, float* __restrict__ depth_out, const float4* __restrict__ nrec, float* __restrict__ normal_out)
 {
     static_assert(!DEPTH || (!BULK && !PAIRS), "the depth channel exists on the default forward only");
+    static_assert(!NORMAL || (!BULK && !PAIRS), "the normal channels exist on the default forward only");
     constexpr int PPT = TH * TW / 32;
     __shared__ __align__(128) SplatRec s_rec[WARPS_PER_BLOCK][2][32];
+    __shared__ __align__(16) float4 s_nrm[NORMAL ? WARPS_PER_BLOCK : 1][NORMAL ? 2 : 1][NORMAL ? 32 : 1];
     __shared__ __align__(8) uint64_t s_bar[WARPS_PER_BLOCK][2];
     const int lane = threadIdx.x, warp = threadIdx.y, b = blockIdx.y;
     const int slot = blockIdx.x * blockDim.y + warp;
@@ -275,11 +331,17 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_forward_kernel(
     constexpr float KS = 256.0f / 255.0f, KI = 255.0f / 256.0f;
     constexpr float TS_MIN = T_MIN * KI, A_MIN_S = ALPHA_MIN * KS;
     float Ts[PPT], Cr[PPT], Cg[PPT], Cb[PPT], nf[PPT], Dz[DEPTH ? PPT : 1];
+    float N0[NORMAL ? PPT : 1], N1[NORMAL ? PPT : 1], N2[NORMAL ? PPT : 1];
 #pragma unroll
     for (int j = 0; j < PPT; j++) { Ts[j] = KI; Cr[j] = Cg[j] = Cb[j] = 0.0f; nf[j] = 0.0f; }
     if (DEPTH) {
 #pragma unroll
         for (int j = 0; j < PPT; j++) Dz[j] = 0.0f;
+    }
+    if (NORMAL) {
+#pragma unroll
+        for (int j = 0; j < PPT; j++) N0[j] = N1[j] = N2[j] = 0.0f;
+        nrec += (size_t)b * N;
     }
 
     if (count > 0) {
@@ -287,13 +349,14 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_forward_kernel(
         st.init(&s_rec[warp][0][0], &s_bar[warp][0], lane);
         const int nchunks = (count + 31) >> 5;
         int id_cur = (lane < count) ? ids[lane] : -1;
-        st.issue(0, recs, id_cur);
+        float4* nbuf = NORMAL ? &s_nrm[warp][0][0] : nullptr;
+        st.template issue<NORMAL>(0, recs, id_cur, nrec, nbuf);
         int id_next = (32 + lane < count) ? ids[32 + lane] : -1;
         bool done = false;
         for (int c = 0; c < nchunks && !done; c++) {
             const bool more = (c + 1 < nchunks);
             if (more) {
-                st.issue((c + 1) & 1, recs, id_next);
+                st.template issue<NORMAL>((c + 1) & 1, recs, id_next, nrec, nbuf);
                 int nn = (c + 2) * 32 + lane;
                 id_next = (nn < count) ? ids[nn] : -1;
             }
@@ -321,6 +384,7 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_forward_kernel(
                 const float a2 = q0.z, b2 = q0.w, c2 = q1.x;
                 const float base = a2 * dx * dx, lin = b2 * dx;
                 const float os = q2.y;
+                const float4 nk4 = NORMAL ? s_nrm[warp][c & 1][k] : make_float4(0.f, 0.f, 0.f, 0.f);   // n of this splat
                 int fcount = 0; float wsum = 0.f;
                 if (PAIRS && !STAT) {
                     // pair form (add2/mul2/fma2): the two pixels of a pair run the same chain side by side;
@@ -357,7 +421,10 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_forward_kernel(
                         const bool ok = (Ts[j] > TS_MIN) && (a >= A_MIN_S);
                         if (ok) { fcount++; wsum += a * Ts[j]; }
                     }
-                    if (DEPTH) blend_pixel_depth(a, q1.z, q1.w, cb, chunk[k].pad0, Ts[j], Cr[j], Cg[j], Cb[j], Dz[j], nf[j], TS_MIN, A_MIN_S, -KI);
+                    if (NORMAL) blend_pixel_normal<DEPTH>(a, q1.z, q1.w, cb, DEPTH ? chunk[k].pad0 : 0.0f, nk4.x, nk4.y, nk4.z, Ts[j], Cr[j],
+                                                          Cg[j], Cb[j], Dz[DEPTH ? j : 0], N0[j], N1[j], N2[j], nf[j], TS_MIN,
+                                                          A_MIN_S, -KI);
+                    else if (DEPTH) blend_pixel_depth(a, q1.z, q1.w, cb, chunk[k].pad0, Ts[j], Cr[j], Cg[j], Cb[j], Dz[j], nf[j], TS_MIN, A_MIN_S, -KI);
                     else blend_pixel(a, q1.z, q1.w, cb, Ts[j], Cr[j], Cg[j], Cb[j], nf[j], TS_MIN, A_MIN_S, -KI);
                 }
                 }
@@ -390,6 +457,11 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_forward_kernel(
         img[((size_t)b * 3 + 2) * plane + po] = fmaxf(fminf(Cb[j], 1.0f), lo);
         Tout[(size_t)b * plane + po] = Ts[j] * KS;
         if (DEPTH) depth_out[(size_t)b * plane + po] = Dz[j];
+        if (NORMAL) {
+            normal_out[((size_t)b * 3 + 0) * plane + po] = N0[j];
+            normal_out[((size_t)b * 3 + 1) * plane + po] = N1[j];
+            normal_out[((size_t)b * 3 + 2) * plane + po] = N2[j];
+        }
         // the contributor count is a 16-bit tensor in the reference contract (read back as unsigned short,
         // GR/raster.cu:683-686): saturate instead of wrapping when a pixel stays active past 65535 list entries
         last[(size_t)b * plane + po] = (unsigned short)__float2uint_rn(fminf(nf[j], 65535.0f));
@@ -633,19 +705,29 @@ __device__ __forceinline__ float2 bc2(float a) { return make_float2(a, a); }
 // DEPTH: d_depth f32[V,1,Hp,Wp] = dL/dD is one more colour channel with "colour" z (the staged pad0): z g_z joins the (c - R) . g
 // dot product, and sum w g_z is reduced into slot LGS_GRAD_DEPTH.  That value is the last row of a parked splat; with STAT it makes
 // 11 rows, so only 2 splats are parked per flush (RG * NV <= 32 lanes).
-template <int TH, int TW, bool STAT, bool TRANS, bool DET = false, bool DEPTH = false>
+// NORMAL: d_normal f32[V,3,Hp,Wp] = dL/dN is three more colour channels with "colour" n (the side row nrec[id], staged beside the
+// record): n . g_N joins the dot product after the depth term, and sum w g_N is reduced as the last three rows of a parked splat,
+// which go to grad_normal f32[V*N,4] (i64 in DET) instead of the record gradient.  NV = 9 + STAT + DEPTH + 3 <= 14, so 2 splats
+// are parked per flush.  g_N is not held in registers (30 more live floats at 16x16 would exceed the register budget): each lane
+// parks its pixel pairs' g_N in shared memory once and reads them back per splat (conflict-free LDS.64).
+template <int TH, int TW, bool STAT, bool TRANS, bool DET = false, bool DEPTH = false, bool NORMAL = false>
 __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kernel(
     const int* __restrict__ sorted, const int* __restrict__ start_index, const SplatRec* __restrict__ recs,
     const int* __restrict__ tiles, int n_sel, const float* __restrict__ Tfinal, const unsigned short* __restrict__ last,
     const float* __restrict__ d_img, const float* __restrict__ d_trans, const float* __restrict__ clamped_img,
-    float* __restrict__ grad, int gx, int ntile, int cap, int N, int Hp, int Wp, int err_mode, const float* __restrict__ d_depth)
+    float* __restrict__ grad, int gx, int ntile, int cap, int N, int Hp, int Wp, int err_mode, const float* __restrict__ d_depth,
+    const float4* __restrict__ nrec, const float* __restrict__ d_normal, float* __restrict__ grad_normal)
 {
     constexpr int PPT = TH * TW / 32, NP = PPT / 2;
     static_assert(PPT % 2 == 0, "pixels per lane must pair up");
-    constexpr int NV = 9 + (STAT ? 1 : 0) + (DEPTH ? 1 : 0);   // values reduced per (tile, splat)
+    constexpr int NV = 9 + (STAT ? 1 : 0) + (DEPTH ? 1 : 0) + (NORMAL ? 3 : 0);   // values reduced per (tile, splat)
+    constexpr int ROW_N = NV - 3;                              // first normal row (NORMAL)
+    constexpr int ROW_Z = NV - 1 - (NORMAL ? 3 : 0);           // depth row (DEPTH)
     constexpr int RG = (LGS_RG * NV <= 32) ? LGS_RG : 2;      // splats parked per flush
     constexpr float KS = 256.0f / 255.0f, A_MIN_S = ALPHA_MIN * KS;
     __shared__ __align__(128) SplatRec s_rec[WARPS_PER_BLOCK][2][32];
+    __shared__ __align__(16) float4 s_nrm[NORMAL ? WARPS_PER_BLOCK : 1][NORMAL ? 2 : 1][NORMAL ? 32 : 1];
+    __shared__ __align__(16) float2 s_gn[NORMAL ? WARPS_PER_BLOCK : 1][NORMAL ? 3 * NP : 1][NORMAL ? 32 : 1];   // g_N per pixel pair
     __shared__ __align__(8) uint64_t s_bar[WARPS_PER_BLOCK][2];
     __shared__ __align__(16) float s_acc[WARPS_PER_BLOCK][RG * NV][LGS_ROWF];
     __shared__ int s_pid[WARPS_PER_BLOCK][4];               // ids of the splats parked in s_acc
@@ -660,6 +742,10 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
     if (start < 0) return;
     recs += (size_t)b * N;
     grad += (size_t)b * N * LGS_GRAD_FLOATS * (DET ? 2 : 1);          // DET: 64-bit slots
+    if (NORMAL) {
+        nrec += (size_t)b * N;
+        grad_normal += (size_t)b * N * 4 * (DET ? 2 : 1);
+    }
     const int* ids = sorted + (size_t)b * cap + start;
 
     const int x = ((tile_id - 1) % gx) * TW + lane % TW;
@@ -676,6 +762,13 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
         if (DEPTH) {
             const float z = d_depth[(size_t)b * plane + po];
             if (j & 1) gz[j / 2].y = z; else gz[j / 2].x = z;
+        }
+        if (NORMAL) {
+#pragma unroll
+            for (int ch = 0; ch < 3; ch++) {
+                float* e = reinterpret_cast<float*>(&s_gn[warp][ch * NP + j / 2][lane]);
+                e[j & 1] = d_normal[((size_t)b * 3 + ch) * plane + po];
+            }
         }
         float t = Tfinal[(size_t)b * plane + po];
         float a0 = d_img[((size_t)b * 3 + 0) * plane + po];
@@ -714,9 +807,16 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
             p0 = add2(p0, p4);
             const float sum = p0.x + p0.y;
             const int sp = lane / NV, row = lane - sp * NV;
-            const int v = (DEPTH && row == NV - 1) ? LGS_GRAD_DEPTH : row;         // gradient slot of the row
+            const int v = (DEPTH && row == ROW_Z) ? LGS_GRAD_DEPTH : row;         // gradient slot of the row
             const int pid = s_pid[warp][sp];
-            if (DET) {
+            if (NORMAL && row >= ROW_N) {                                            // normal rows -> the side array
+                if (DET) {
+                    unsigned long long* gq = reinterpret_cast<unsigned long long*>(grad_normal);
+                    atomicAdd(&gq[(size_t)pid * 4 + (row - ROW_N)], (unsigned long long)__double2ll_rn((double)sum * LGS_DET_SCALE));
+                } else {
+                    atomicAdd(&grad_normal[(size_t)pid * 4 + (row - ROW_N)], sum);
+                }
+            } else if (DET) {
                 unsigned long long* gq = reinterpret_cast<unsigned long long*>(grad);
                 atomicAdd(&gq[(size_t)pid * LGS_GRAD_FLOATS + v], (unsigned long long)__double2ll_rn((double)sum * LGS_DET_SCALE));
             } else {
@@ -731,14 +831,15 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
     const int nchunks = (kmax + 31) >> 5;
     int c0 = nchunks - 1;
     int id_cur = (c0 * 32 + lane < kmax) ? ids[c0 * 32 + lane] : -1;
-    st.issue(0, recs, id_cur);
+    float4* nbuf = NORMAL ? &s_nrm[warp][0][0] : nullptr;
+    st.template issue<NORMAL>(0, recs, id_cur, nrec, nbuf);
     int id_next = (c0 >= 1) ? ids[(c0 - 1) * 32 + lane] : -1;
     for (int v = 0; v < nchunks; v++) {
         const int c = nchunks - 1 - v;
         const bool more = (c >= 1);
         const int id_this = id_cur;
         if (more) {
-            st.issue((v + 1) & 1, recs, id_next);
+            st.template issue<NORMAL>((v + 1) & 1, recs, id_next, nrec, nbuf);
             id_cur = id_next;
             id_next = (c >= 2) ? ids[(c - 2) * 32 + lane] : -1;
         }
@@ -757,7 +858,10 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
             const float2 os2 = bc2(q2.y), o2 = bc2(q1.y), c22 = bc2(c2), lin2 = bc2(lin), base2 = bc2(base);
             const float2 cr2 = bc2(q1.z), cg2 = bc2(q1.w), cb2 = bc2(cb), dy02 = bc2(dy0);
             const float2 z2 = bc2(DEPTH ? chunk[kk].pad0 : 0.0f);            // view-space z (staged by prescale<DEPTH>)
+            const float4 nk4 = NORMAL ? s_nrm[warp][v & 1][kk] : make_float4(0.f, 0.f, 0.f, 0.f);   // n of this splat
+            const float2 n02 = bc2(nk4.x), n12 = bc2(nk4.y), n22 = bc2(nk4.z);
             float2 s0, s1, s2, dr, dg, db, dzs;         // per-(tile, splat) sums: the first pixel pair initialises them
+            float2 dn0, dn1, dn2;
             float esq = 0.f, runx = 0.f, runy = 0.f;
             bool any = false;
 #pragma unroll
@@ -782,6 +886,11 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
                 const float2 w = mul2(a, Tn);
                 float2 cgd = fma2(cr2, g0[p], fma2(cg2, g1[p], mul2(cb2, g2[p])));
                 if (DEPTH) cgd = fma2(z2, gz[p], cgd);          // added last: g_z = 0 leaves the colour-only value
+                float2 u0, u1, u2;                                                       // g_N of the pair (NORMAL)
+                if (NORMAL) {
+                    u0 = s_gn[warp][p][lane]; u1 = s_gn[warp][NP + p][lane]; u2 = s_gn[warp][2 * NP + p][lane];
+                    cgd = fma2(n22, u2, fma2(n12, u1, fma2(n02, u0, cgd)));       // after depth: g_N = 0 leaves it
+                }
                 const float2 diff = fma2(S[p], bc2(-1.0f), cgd);                   // (c - R) . g
                 float2 da = mul2(Tn, diff);
                 if (TRANS) da = fma2(ngt[p], rc, da);
@@ -791,10 +900,12 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
                 if (p == 0) {
                     dr = mul2(w, g0[p]); dg = mul2(w, g1[p]); db = mul2(w, g2[p]);
                     if (DEPTH) dzs = mul2(w, gz[p]);
+                    if (NORMAL) { dn0 = mul2(w, u0); dn1 = mul2(w, u1); dn2 = mul2(w, u2); }
                     s0 = dpw; s1 = td; s2 = mul2(td, dy);
                 } else {
                     dr = fma2(w, g0[p], dr); dg = fma2(w, g1[p], dg); db = fma2(w, g2[p], db);
                     if (DEPTH) dzs = fma2(w, gz[p], dzs);
+                    if (NORMAL) { dn0 = fma2(w, u0, dn0); dn1 = fma2(w, u1, dn1); dn2 = fma2(w, u2, dn2); }
                     s0 = add2(s0, dpw);
                     s1 = add2(s1, td);
                     s2 = fma2(td, dy, s2);
@@ -827,7 +938,12 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
                 row[7 * LGS_ROWF] = db.x + db.y;
                 row[8 * LGS_ROWF] = m0;                    // sum s0
                 if (STAT) row[9 * LGS_ROWF] = esq;
-                if (DEPTH) row[(NV - 1) * LGS_ROWF] = dzs.x + dzs.y;     // sum w g_z -> slot LGS_GRAD_DEPTH
+                if (DEPTH) row[ROW_Z * LGS_ROWF] = dzs.x + dzs.y;        // sum w g_z -> slot LGS_GRAD_DEPTH
+                if (NORMAL) {                                            // sum w g_N -> grad_normal
+                    row[ROW_N * LGS_ROWF] = dn0.x + dn0.y;
+                    row[(ROW_N + 1) * LGS_ROWF] = dn1.x + dn1.y;
+                    row[(ROW_N + 2) * LGS_ROWF] = dn2.x + dn2.y;
+                }
                 pend++;
                 if (pend == RG) flush();
             }
@@ -1028,17 +1144,24 @@ extern "C" int lgs_pack_params(const float* ndc, const float* cov2d_inv, const f
 // img f32[V,3,Hp,Wp]; T f32[V,1,Hp,Wp]; last i16[V,1,Hp,Wp]; fragment_count i32[V,1,N] / weight f32[V,1,N]
 // (must be zero-initialised by the caller when enable_statistic).  depth f32[V,1,Hp,Wp] or NULL: the per-pixel depth D = sum w z
 // of the records' view-space z (default kernel only: refused while bulk staging or the pair forward is forced).
-extern "C" int lgs_rasterize_forward_packed(const int* sorted_points, const int* start_index, const float* packed_params,
-                                            const int* specific_tiles, int n_specific, int V, int N, int cap, int img_h, int img_w,
-                                            int tile_h, int tile_w, int enable_statistic, int clamp_zero, float* img,
-                                            float* transmittance, short* last_contributor, int* fragment_count,
-                                            float* fragment_weight, int* tile_work, float* depth, void* stream)
+// normal_rec f32[V,N,4] and normal f32[V,3,Hp,Wp], both or neither: the per-pixel normal N = sum w n of the side rows n
+// (lgs_project_forward's normal_rec; default kernel only, as depth).
+extern "C" int lgs_rasterize_forward_packed_normal(const int* sorted_points, const int* start_index, const float* packed_params,
+                                                   const int* specific_tiles, int n_specific, int V, int N, int cap, int img_h,
+                                                   int img_w, int tile_h, int tile_w, int enable_statistic, int clamp_zero, float* img,
+                                                   float* transmittance, short* last_contributor, int* fragment_count,
+                                                   float* fragment_weight, int* tile_work, float* depth, const float* normal_rec,
+                                                   float* normal, void* stream)
 {
     LGS_REQUIRE(lgs_tile_ok(tile_h, tile_w), "rasterize_forward: tile %dx%d not one of 8x16, 12x16, 16x16, 8x8", tile_h, tile_w);
     LGS_REQUIRE(V >= 1 && img_h > 0 && img_w > 0, "rasterize_forward: bad sizes V=%d H=%d W=%d", V, img_h, img_w);
     const bool bulk = use_bulk();
     LGS_REQUIRE(depth == nullptr || !(bulk || (!enable_statistic && forward_pairs())),
                 "rasterize_forward: depth is rendered by the default kernel only, but %s is selected",
+                bulk ? "bulk staging" : "the pixel-pair forward");
+    LGS_REQUIRE((normal_rec == nullptr) == (normal == nullptr), "rasterize_forward: normal_rec and normal are both given or both NULL");
+    LGS_REQUIRE(normal == nullptr || !(bulk || (!enable_statistic && forward_pairs())),
+                "rasterize_forward: normals are rendered by the default kernel only, but %s is selected",
                 bulk ? "bulk staging" : "the pixel-pair forward");
     int gx = (img_w + tile_w - 1) / tile_w, gy = (img_h + tile_h - 1) / tile_h;
     int ntile = gx * gy, Hp = gy * tile_h, Wp = gx * tile_w;
@@ -1049,12 +1172,22 @@ extern "C" int lgs_rasterize_forward_packed(const int* sorted_points, const int*
     cudaStream_t st = (cudaStream_t)stream;
     const SplatRec* recs = (const SplatRec*)packed_params;
 #define FWD(S, B) raster_forward_kernel<TH, TW, S, B><<<grid, block, 0, st>>>(sorted_points, start_index, recs, specific_tiles, n_specific, \
-        img, transmittance, (unsigned short*)last_contributor, fragment_count, fragment_weight, tile_work, gx, ntile, cap, N, Hp, Wp, clamp_zero, nullptr)
+        img, transmittance, (unsigned short*)last_contributor, fragment_count, fragment_weight, tile_work, gx, ntile, cap, N, Hp, Wp, clamp_zero, nullptr, \
+        nullptr, nullptr)
 #define FWDP() raster_forward_kernel<TH, TW, false, false, true><<<grid, block, 0, st>>>(sorted_points, start_index, recs, specific_tiles, \
-        n_specific, img, transmittance, (unsigned short*)last_contributor, fragment_count, fragment_weight, tile_work, gx, ntile, cap, N, Hp, Wp, clamp_zero, nullptr)
+        n_specific, img, transmittance, (unsigned short*)last_contributor, fragment_count, fragment_weight, tile_work, gx, ntile, cap, N, Hp, Wp, clamp_zero, nullptr, \
+        nullptr, nullptr)
 #define FWDD(S) raster_forward_kernel<TH, TW, S, false, false, true><<<grid, block, 0, st>>>(sorted_points, start_index, recs, specific_tiles, \
-        n_specific, img, transmittance, (unsigned short*)last_contributor, fragment_count, fragment_weight, tile_work, gx, ntile, cap, N, Hp, Wp, clamp_zero, depth)
-    if (depth != nullptr) {
+        n_specific, img, transmittance, (unsigned short*)last_contributor, fragment_count, fragment_weight, tile_work, gx, ntile, cap, N, Hp, Wp, clamp_zero, depth, \
+        nullptr, nullptr)
+#define FWDN(S, Z) raster_forward_kernel<TH, TW, S, false, false, Z, true><<<grid, block, 0, st>>>(sorted_points, start_index, recs,    \
+        specific_tiles, n_specific, img, transmittance, (unsigned short*)last_contributor, fragment_count, fragment_weight, tile_work, gx, \
+        ntile, cap, N, Hp, Wp, clamp_zero, depth, (const float4*)normal_rec, normal)
+    if (normal != nullptr) {
+        LGS_DISPATCH_TILE(tile_h, tile_w,
+            if (depth != nullptr) { if (enable_statistic) FWDN(true, true); else FWDN(false, true); }
+            else { if (enable_statistic) FWDN(true, false); else FWDN(false, false); })
+    } else if (depth != nullptr) {
         LGS_DISPATCH_TILE(tile_h, tile_w, if (enable_statistic) FWDD(true); else FWDD(false);)
     } else {
         LGS_DISPATCH_TILE(tile_h, tile_w,
@@ -1064,24 +1197,45 @@ extern "C" int lgs_rasterize_forward_packed(const int* sorted_points, const int*
 #undef FWD
 #undef FWDP
 #undef FWDD
+#undef FWDN
     LGS_CHECK_LAUNCH("raster_forward_kernel");
     return LGS_OK;
 }
 
+// The form without normals: lgs_rasterize_forward_packed_normal with normal_rec = normal = NULL.
+extern "C" int lgs_rasterize_forward_packed(const int* sorted_points, const int* start_index, const float* packed_params,
+                                            const int* specific_tiles, int n_specific, int V, int N, int cap, int img_h, int img_w,
+                                            int tile_h, int tile_w, int enable_statistic, int clamp_zero, float* img,
+                                            float* transmittance, short* last_contributor, int* fragment_count,
+                                            float* fragment_weight, int* tile_work, float* depth, void* stream)
+{
+    return lgs_rasterize_forward_packed_normal(sorted_points, start_index, packed_params, specific_tiles, n_specific, V, N, cap, img_h,
+                                               img_w, tile_h, tile_w, enable_statistic, clamp_zero, img, transmittance, last_contributor,
+                                               fragment_count, fragment_weight, tile_work, depth, nullptr, nullptr, stream);
+}
+
 // packed_grad: f32[V,N,12] scratch, zeroed here.  d_trans may be null.  Outputs as GR/raster.cu:1021-1036.
-extern "C" int lgs_rasterize_backward(const int* sorted_points, const int* start_index, const float* packed_params,
-                                      const int* specific_tiles, int n_specific, const float* final_transmittance,
-                                      const short* last_contributor, const float* d_img, const float* d_trans_img,
-                                      const float* clamped_img, const float* grad_inv_scaler, int V, int N, int cap, int img_h,
-                                      int img_w, int tile_h,
-                                      int tile_w, int enable_statistic, float* packed_grad, float* d_ndc, float* d_cov2d_inv,
-                                      float* d_color, float* d_opacity, float* err_sum, float* err_square_sum, const float* d_depth,
-                                      void* stream)
+// normal_rec f32[V,N,4], d_normal f32[V,3,Hp,Wp] and grad_normal f32[V,N,4] (zeroed here), all or none: dL/dN joins the alpha
+// gradient as three more colour channels with colour n, and grad_normal receives sum_pixels w g_N = dL/dn.
+extern "C" int lgs_rasterize_backward_normal(const int* sorted_points, const int* start_index, const float* packed_params,
+                                             const int* specific_tiles, int n_specific, const float* final_transmittance,
+                                             const short* last_contributor, const float* d_img, const float* d_trans_img,
+                                             const float* clamped_img, const float* grad_inv_scaler, int V, int N, int cap, int img_h,
+                                             int img_w, int tile_h, int tile_w, int enable_statistic, float* packed_grad, float* d_ndc,
+                                             float* d_cov2d_inv, float* d_color, float* d_opacity, float* err_sum,
+                                             float* err_square_sum, const float* d_depth, const float* normal_rec,
+                                             const float* d_normal, float* grad_normal, void* stream)
 {
     LGS_REQUIRE(lgs_tile_ok(tile_h, tile_w), "rasterize_backward: tile %dx%d not one of 8x16, 12x16, 16x16, 8x8", tile_h, tile_w);
     LGS_REQUIRE(V >= 1 && img_h > 0 && img_w > 0, "rasterize_backward: bad sizes V=%d H=%d W=%d", V, img_h, img_w);
     LGS_REQUIRE(d_depth == nullptr || deterministic() || (backward_version() == 2 && !use_bulk()),
                 "rasterize_backward: the depth gradient is taken by the pixel-pair kernel only, but %s is selected",
+                use_bulk() ? "bulk staging" : "the scalar (v1) kernel");
+    const bool nrm = d_normal != nullptr;
+    LGS_REQUIRE((normal_rec != nullptr) == nrm && (grad_normal != nullptr) == nrm,
+                "rasterize_backward: normal_rec, d_normal and grad_normal are all given or all NULL");
+    LGS_REQUIRE(!nrm || deterministic() || (backward_version() == 2 && !use_bulk()),
+                "rasterize_backward: the normal gradient is taken by the pixel-pair kernel only, but %s is selected",
                 use_bulk() ? "bulk staging" : "the scalar (v1) kernel");
     int gx = (img_w + tile_w - 1) / tile_w, gy = (img_h + tile_h - 1) / tile_h;
     int ntile = gx * gy, Hp = gy * tile_h, Wp = gx * tile_w;
@@ -1089,6 +1243,7 @@ extern "C" int lgs_rasterize_backward(const int* sorted_points, const int* start
     cudaStream_t st = (cudaStream_t)stream;
     if (N == 0) return LGS_OK;
     LGS_CUDA(cudaMemsetAsync(packed_grad, 0, sizeof(float) * (size_t)V * N * LGS_GRAD_FLOATS, st));
+    if (nrm) LGS_CUDA(cudaMemsetAsync(grad_normal, 0, sizeof(float) * (size_t)V * N * 4, st));
     if (nrender > 0) {
         const int wpb = warps_per_block();
         dim3 grid(lgs_cdiv(nrender, wpb), V), block(32, wpb);
@@ -1099,31 +1254,44 @@ extern "C" int lgs_rasterize_backward(const int* sorted_points, const int* start
         const unsigned short* lastu = (const unsigned short*)last_contributor;
         if (deterministic()) {
             // integer accumulation in a stream-ordered scratch buffer, converted into packed_grad afterwards
-            const size_t nq = (size_t)V * N * LGS_GRAD_FLOATS;
+            // (normal mode: the normal rows follow in the same buffer, V*N*4 more slots)
+            const size_t nq = (size_t)V * N * LGS_GRAD_FLOATS, nqn = nrm ? (size_t)V * N * 4 : 0;
             long long* q = nullptr;
-            LGS_CUDA(cudaMallocAsync((void**)&q, nq * sizeof(long long), st));
-            LGS_CUDA(cudaMemsetAsync(q, 0, nq * sizeof(long long), st));
-#define BWD_DET(S, T, Z) raster_backward_v2_kernel<TH, TW, S, T, true, Z><<<grid, block, 0, st>>>(sorted_points, start_index, recs, \
-        specific_tiles, n_specific, final_transmittance, lastu, d_img, d_trans_img, clamped_img, (float*)q, gx, ntile, cap, N, Hp, Wp, g_err_mode, \
-        d_depth)
-#define BWD_DET_Z(Z) LGS_DISPATCH_TILE(tile_h, tile_w,                                                                    \
-                if (enable_statistic) { if (trans) BWD_DET(true, true, Z); else BWD_DET(true, false, Z); }                  \
-                else { if (trans) BWD_DET(false, true, Z); else BWD_DET(false, false, Z); })
-            if (d_depth != nullptr) { BWD_DET_Z(true) } else { BWD_DET_Z(false) }
+            LGS_CUDA(cudaMallocAsync((void**)&q, (nq + nqn) * sizeof(long long), st));
+            LGS_CUDA(cudaMemsetAsync(q, 0, (nq + nqn) * sizeof(long long), st));
+#define BWD_DET(S, T, Z, NM) raster_backward_v2_kernel<TH, TW, S, T, true, Z, NM><<<grid, block, 0, st>>>(sorted_points, start_index, \
+        recs, specific_tiles, n_specific, final_transmittance, lastu, d_img, d_trans_img, clamped_img, (float*)q, gx, ntile, cap, N, Hp, Wp, \
+        g_err_mode, d_depth, (const float4*)normal_rec, d_normal, (float*)(q + nq))
+#define BWD_DET_Z(Z, NM) LGS_DISPATCH_TILE(tile_h, tile_w,                                                                \
+                if (enable_statistic) { if (trans) BWD_DET(true, true, Z, NM); else BWD_DET(true, false, Z, NM); }          \
+                else { if (trans) BWD_DET(false, true, Z, NM); else BWD_DET(false, false, Z, NM); })
+            if (nrm) {
+                if (d_depth != nullptr) { BWD_DET_Z(true, true) } else { BWD_DET_Z(false, true) }
+            } else {
+                if (d_depth != nullptr) { BWD_DET_Z(true, false) } else { BWD_DET_Z(false, false) }
+            }
 #undef BWD_DET_Z
 #undef BWD_DET
             LGS_CHECK_LAUNCH("raster_backward_v2_kernel<DET>");
             det_to_float_kernel<<<lgs_cdiv((long long)nq, 256), 256, 0, st>>>(q, packed_grad, nq);
             LGS_CHECK_LAUNCH("det_to_float_kernel");
+            if (nrm) {
+                det_to_float_kernel<<<lgs_cdiv((long long)nqn, 256), 256, 0, st>>>(q + nq, grad_normal, nqn);
+                LGS_CHECK_LAUNCH("det_to_float_kernel");
+            }
             LGS_CUDA(cudaFreeAsync(q, st));
         } else if (backward_version() == 2 && !bulk) {
-#define BW2(S, T, Z) raster_backward_v2_kernel<TH, TW, S, T, false, Z><<<grid, block, 0, st>>>(sorted_points, start_index, recs, \
-        specific_tiles, n_specific, final_transmittance, lastu, d_img, d_trans_img, clamped_img, packed_grad, gx, ntile, cap, N, Hp, Wp, \
-        g_err_mode, d_depth)
-#define BW2_Z(Z) LGS_DISPATCH_TILE(tile_h, tile_w,                                                                         \
-                if (enable_statistic) { if (trans) BW2(true, true, Z); else BW2(true, false, Z); }                          \
-                else { if (trans) BW2(false, true, Z); else BW2(false, false, Z); })
-            if (d_depth != nullptr) { BW2_Z(true) } else { BW2_Z(false) }
+#define BW2(S, T, Z, NM) raster_backward_v2_kernel<TH, TW, S, T, false, Z, NM><<<grid, block, 0, st>>>(sorted_points, start_index, \
+        recs, specific_tiles, n_specific, final_transmittance, lastu, d_img, d_trans_img, clamped_img, packed_grad, gx, ntile, cap, N, Hp, \
+        Wp, g_err_mode, d_depth, (const float4*)normal_rec, d_normal, grad_normal)
+#define BW2_Z(Z, NM) LGS_DISPATCH_TILE(tile_h, tile_w,                                                                     \
+                if (enable_statistic) { if (trans) BW2(true, true, Z, NM); else BW2(true, false, Z, NM); }                  \
+                else { if (trans) BW2(false, true, Z, NM); else BW2(false, false, Z, NM); })
+            if (nrm) {
+                if (d_depth != nullptr) { BW2_Z(true, true) } else { BW2_Z(false, true) }
+            } else {
+                if (d_depth != nullptr) { BW2_Z(true, false) } else { BW2_Z(false, false) }
+            }
 #undef BW2_Z
 #undef BW2
             LGS_CHECK_LAUNCH("raster_backward_v2_kernel");
@@ -1147,4 +1315,20 @@ extern "C" int lgs_rasterize_backward(const int* sorted_points, const int* start
         LGS_CHECK_LAUNCH("unpack_kernel");
     }
     return LGS_OK;
+}
+
+// The form without normals: lgs_rasterize_backward_normal with normal_rec = d_normal = grad_normal = NULL.
+extern "C" int lgs_rasterize_backward(const int* sorted_points, const int* start_index, const float* packed_params,
+                                      const int* specific_tiles, int n_specific, const float* final_transmittance,
+                                      const short* last_contributor, const float* d_img, const float* d_trans_img,
+                                      const float* clamped_img, const float* grad_inv_scaler, int V, int N, int cap, int img_h,
+                                      int img_w, int tile_h,
+                                      int tile_w, int enable_statistic, float* packed_grad, float* d_ndc, float* d_cov2d_inv,
+                                      float* d_color, float* d_opacity, float* err_sum, float* err_square_sum, const float* d_depth,
+                                      void* stream)
+{
+    return lgs_rasterize_backward_normal(sorted_points, start_index, packed_params, specific_tiles, n_specific, final_transmittance,
+                                         last_contributor, d_img, d_trans_img, clamped_img, grad_inv_scaler, V, N, cap, img_h, img_w,
+                                         tile_h, tile_w, enable_statistic, packed_grad, d_ndc, d_cov2d_inv, d_color, d_opacity, err_sum,
+                                         err_square_sum, d_depth, nullptr, nullptr, nullptr, stream);
 }

@@ -65,6 +65,8 @@ class ViewState:
     antialiased: bool = False        # antialiased mode (DESIGN.md section 1): the backward must use the forward's setting
     filter_3d: Optional[torch.Tensor] = None    # 3D smoothing filter f32[1,C,S] the forward used (DESIGN.md section 1), or None
     depth: Optional[torch.Tensor] = None        # f32[1,1,Hp,Wp] per-pixel depth D (render_depth, DESIGN.md section 1), or None
+    normal: Optional[torch.Tensor] = None       # f32[1,3,Hp,Wp] per-pixel normal N (render_normal, DESIGN.md section 1), or None
+    normal_rec: Optional[torch.Tensor] = None   # f32[Nv,4] each record's camera-facing view-space normal (render_normal), or None
 
 
 class _Pinned:
@@ -80,9 +82,9 @@ class _Pinned:
 
 
 def _padded(g: torch.Tensor, shape) -> torch.Tensor:
-    """A per-pixel gradient f32[1,1,H,W] or [1,1,Hp,Wp] as a contiguous f32[1,1,Hp,Wp] (zeros in the padding)."""
-    if not (g.is_cuda and g.dtype == _F32 and g.dim() == 4 and g.shape[:2] == (1, 1)):
-        raise RuntimeError("per-pixel gradients must be float32 CUDA tensors of shape [1,1,H,W]")
+    """A per-pixel gradient f32[1,c,H,W] or [1,c,Hp,Wp] as a contiguous f32[1,c,Hp,Wp] (zeros in the padding), c = shape[1]."""
+    if not (g.is_cuda and g.dtype == _F32 and g.dim() == 4 and tuple(g.shape[:2]) == tuple(shape[:2])):
+        raise RuntimeError(f"per-pixel gradients must be float32 CUDA tensors of shape [1,{shape[1]},H,W]")
     if tuple(g.shape) != tuple(shape):
         g = torch.nn.functional.pad(g, (0, shape[-1] - g.shape[-1], 0, shape[-2] - g.shape[-2]))
     return g if g.is_contiguous() else g.contiguous()
@@ -102,7 +104,8 @@ def check_filter_3d(filter_3d: Optional[torch.Tensor], xyz: torch.Tensor) -> Opt
 def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_extend: torch.Tensor, frustumplane: torch.Tensor,
                         view_matrix: torch.Tensor, proj_matrix: torch.Tensor, sh_degree: int, hw: tuple, tile: tuple,
                         enable_statistic: bool = False, specific_tiles: Optional[torch.Tensor] = None, clamp_zero: bool = False,
-                        antialiased: bool = False, filter_3d: Optional[torch.Tensor] = None, render_depth: bool = False):
+                        antialiased: bool = False, filter_3d: Optional[torch.Tensor] = None, render_depth: bool = False,
+                        render_normal: bool = False):
     """Forward of one view.  params: xyz[3,C,S] scale[3,C,S] rot[4,C,S] sh_0[1,3,C,S] sh_rest[R,3,C,S]
     opacity[1,C,S] (raw, clustered; float32 CUDA, contiguous).  Returns (img f32[1,3,Hp,Wp] padded to whole
     tiles, ViewState, (fragment_count, fragment_weight) or None).
@@ -115,7 +118,11 @@ def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_exte
     tensor for the backward, which must see the same values.
 
     render_depth: also render the per-pixel depth D = sum_i w_i z_i (w_i the colour's blend weights, z_i the view-space z; not
-    clamped; DESIGN.md section 1, "Depth") into state.depth f32[1,1,Hp,Wp].  The expected depth is D / (1 - T)."""
+    clamped; DESIGN.md section 1, "Depth") into state.depth f32[1,1,Hp,Wp].  The expected depth is D / (1 - T).
+
+    render_normal: also render the per-pixel normal N = sum_i w_i n_i (n_i the camera-facing view-space normal of Gaussian i's
+    shortest axis; neither clamped nor normalised; DESIGN.md section 1, "Normals") into state.normal f32[1,3,Hp,Wp], and keep
+    the per-record normals in state.normal_rec for the backward.  The expected normal is N / (1 - T), the unit normal N / |N|."""
     xyz = params["xyz"]
     dev = xyz.device
     filter_3d = check_filter_3d(filter_3d, xyz)
@@ -144,10 +151,13 @@ def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_exte
         dkey = torch.empty(Nmax, dtype=_I32, device=dev)
         iota = torch.empty(Nmax, dtype=_I32, device=dev)
         tcount = torch.empty(Nmax, dtype=_I32, device=dev)
-        _lib.call("lgs_project_forward", int(sh_degree), _ptr(ids), ctypes.c_void_p(counters.data_ptr()), _ptr(view_matrix),
+        normal_rec = torch.empty((Nmax, 4), dtype=_F32, device=dev) if render_normal else None
+        _lib.call("lgs_project_forward_normal" if render_normal else "lgs_project_forward", int(sh_degree), _ptr(ids),
+                  ctypes.c_void_p(counters.data_ptr()), _ptr(view_matrix),
                   _ptr(proj_matrix), _ptr(xyz), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["sh_0"]),
                   _ptr(params["sh_rest"]), _ptr(params["opacity"]), C, S, M, H, W, th, tw, _ptr(packed), _ptr(dkey), _ptr(iota),
-                  _ptr(tcount), ctypes.c_void_p(counters.data_ptr() + 4), _ptr(filter_3d), int(bool(antialiased)), st)
+                  _ptr(tcount), ctypes.c_void_p(counters.data_ptr() + 4), _ptr(filter_3d), int(bool(antialiased)),
+                  *((_ptr(normal_rec),) if render_normal else ()), st)
         pinned = _Pinned.get(dev)
         pinned.copy_(counters, non_blocking=True)
         torch.cuda.current_stream(dev).synchronize()
@@ -198,12 +208,15 @@ def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_exte
         T = torch.empty((1, 1, Hp, Wp), dtype=_F32, device=dev)
         last = torch.empty((1, 1, Hp, Wp), dtype=torch.int16, device=dev)
         depth = torch.empty((1, 1, Hp, Wp), dtype=_F32, device=dev) if render_depth else None
+        normal = torch.empty((1, 3, Hp, Wp), dtype=_F32, device=dev) if render_normal else None
         n_sel = 0
         if specific_tiles is not None:
             n_sel = specific_tiles.shape[1]
             img.zero_(); T.fill_(1.0); last.zero_()
             if depth is not None:
                 depth.zero_()
+            if normal is not None:
+                normal.zero_()
         stats = None
         fc = fw = None
         if enable_statistic:
@@ -213,16 +226,17 @@ def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_exte
         # per-tile trip count of the backward (deepest list position any pixel consumed) -> heaviest-first tile order
         order = None
         work = torch.empty((1, ntile), dtype=_I32, device=dev) if (CONFIG["tile_order"] and specific_tiles is None and D > 0) else None
-        _lib.call("lgs_rasterize_forward_packed", _ptr(sorted_pid), _ptr(ranges), _ptr(packed), _ptr(specific_tiles), n_sel, 1,
+        _lib.call("lgs_rasterize_forward_packed_normal" if render_normal else "lgs_rasterize_forward_packed", _ptr(sorted_pid),
+                  _ptr(ranges), _ptr(packed), _ptr(specific_tiles), n_sel, 1,
                   Nmax, sorted_pid.shape[1], H, W, th, tw, int(bool(enable_statistic)), int(bool(clamp_zero)), _ptr(img), _ptr(T),
-                  _ptr(last), _ptr(fc), _ptr(fw), _ptr(work), _ptr(depth), st)
+                  _ptr(last), _ptr(fc), _ptr(fw), _ptr(work), _ptr(depth), *((_ptr(normal_rec), _ptr(normal)) if render_normal else ()), st)
         if work is not None:
             order = torch.empty((1, ntile), dtype=_I32, device=dev)
             _lib.call("lgs_tile_order", _ptr(work), 1, ntile, _ptr(order), st)
     state = ViewState(sh_degree=int(sh_degree), hw=(H, W), tile=(th, tw), n_chunks_visible=nvis, n_pairs=D, chunk_ids=ids,
                       counters=counters, view=view_matrix, proj=proj_matrix, packed=packed, tile_count=tcount,
                       sorted_pid=sorted_pid, ranges=ranges, T=T, last=last, tile_order=order, antialiased=bool(antialiased),
-                      filter_3d=filter_3d, depth=depth)
+                      filter_3d=filter_3d, depth=depth, normal=normal, normal_rec=normal_rec)
     return img, state, stats
 
 
@@ -230,7 +244,7 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
                          enable_statistic: bool = False, specific_tiles: Optional[torch.Tensor] = None,
                          accumulate_into: Optional[dict] = None, clamped_img: Optional[torch.Tensor] = None,
                          camera_grad: Optional[torch.Tensor] = None, exact_grad: bool = False,
-                         d_depth: Optional[torch.Tensor] = None):
+                         d_depth: Optional[torch.Tensor] = None, d_normal: Optional[torch.Tensor] = None):
     """Backward of one view: d_img f32[1,3,Hp,Wp] (padded) -> compacted parameter gradients
     (xyz[3,A,S], scale[3,A,S], rot[4,A,S], sh_0[1,3,A,S], sh_rest[R,3,A,S], opacity[1,A,S]) with
     A = state.n_chunks_visible, plus packed_grad (whose slot 9 carries the statistics term).
@@ -246,7 +260,11 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
     ray-space Jacobian J and through the SH view direction.  The other gradients and the forward do not depend on it.
 
     d_depth: dL/dD f32[1,1,H,W] or [1,1,Hp,Wp] of the depth the forward rendered (render_depth=True), or None.  It reaches every
-    parameter through the blend weights and the positions and camera through the view-space z."""
+    parameter through the blend weights and the positions and camera through the view-space z.
+
+    d_normal: dL/dN f32[1,3,H,W] or [1,3,Hp,Wp] of the normal the forward rendered (render_normal=True), or None.  It reaches
+    every parameter through the blend weights, and the rotations and the camera through the normals (the shortest axis and the
+    facing sign held constant)."""
     xyz = params["xyz"]
     dev = xyz.device
     C, S = xyz.shape[-2:]
@@ -264,6 +282,10 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
         if state.depth is None:
             raise RuntimeError("d_depth is given, but the forward of this view did not render depth (render_depth=False)")
         d_depth = _padded(d_depth, state.T.shape)
+    if d_normal is not None:
+        if state.normal is None:
+            raise RuntimeError("d_normal is given, but the forward of this view did not render normals (render_normal=False)")
+        d_normal = _padded(d_normal, state.normal.shape)
     if camera_grad is not None and not (camera_grad.is_cuda and camera_grad.dtype == _F32 and camera_grad.is_contiguous()
                                         and tuple(camera_grad.shape) == (2, 4, 4)):
         raise RuntimeError("camera_grad must be a contiguous float32 CUDA tensor of shape [2,4,4]")
@@ -276,11 +298,17 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
         if specific_tiles is None:
             specific_tiles = state.tile_order          # every tile, longest lists first (None = index order)
         n_sel = 0 if specific_tiles is None else specific_tiles.shape[1]
-        _lib.call("lgs_rasterize_backward", _ptr(state.sorted_pid), _ptr(state.ranges), _ptr(state.packed), _ptr(specific_tiles), n_sel,
+        nrm = d_normal is not None
+        gn = torch.empty((Nmax, 4), dtype=_F32, device=dev) if nrm else None     # dL/dn per record (zeroed by the raster backward)
+        _lib.call("lgs_rasterize_backward_normal" if nrm else "lgs_rasterize_backward", _ptr(state.sorted_pid), _ptr(state.ranges),
+                  _ptr(state.packed), _ptr(specific_tiles), n_sel,
                   _ptr(state.T), _ptr(state.last), _ptr(d_img), _ptr(d_trans), _ptr(clamped_img), None, 1, Nmax, state.sorted_pid.shape[1],
                   H, W, th, tw,
-                  int(bool(enable_statistic)), _ptr(pg), None, None, None, None, None, None, _ptr(d_depth), st)
+                  int(bool(enable_statistic)), _ptr(pg), None, None, None, None, None, None, _ptr(d_depth),
+                  *((_ptr(state.normal_rec), _ptr(d_normal), _ptr(gn)) if nrm else ()), st)
         depth_arg = int(d_depth is not None)            # the record gradient carries the depth slot
+        pb = "lgs_project_backward_normal" if nrm else "lgs_project_backward"
+        pb_tail = (_ptr(gn),) if nrm else ()
         if accumulate_into is not None:
             for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity"):
                 t = accumulate_into[k]
@@ -288,11 +316,12 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
                     raise RuntimeError(f"accumulate_into['{k}'] must be a contiguous float32 CUDA tensor shaped like the parameter")
             if A > 0:
                 d = accumulate_into
-                _lib.call("lgs_project_backward", state.sh_degree, _ptr(state.chunk_ids), ctypes.c_void_p(state.counters.data_ptr()),
+                _lib.call(pb, state.sh_degree, _ptr(state.chunk_ids), ctypes.c_void_p(state.counters.data_ptr()),
                           _ptr(state.view), _ptr(state.proj), _ptr(xyz), _ptr(params["scale"]), _ptr(params["rot"]),
                           _ptr(params["opacity"]), C, S, A, R, H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(pg), None, 2,
                           _ptr(d["xyz"]), _ptr(d["scale"]), _ptr(d["rot"]), _ptr(d["sh_0"]), _ptr(d["sh_rest"]), _ptr(d["opacity"]),
-                          _ptr(d.get("_touched")), *cam_args, _ptr(state.filter_3d), int(state.antialiased), *exact_args, depth_arg, st)   # "_touched": chunk marks for the fused optimizer step
+                          _ptr(d.get("_touched")), *cam_args, _ptr(state.filter_3d), int(state.antialiased), *exact_args, depth_arg,
+                          *pb_tail, st)   # "_touched": chunk marks for the fused optimizer step
             elif camera_grad is not None:
                 camera_grad.zero_()
             return None, pg
@@ -304,10 +333,11 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
         g_sr = torch.zeros((R, 3, A, S), dtype=_F32, device=dev) if R > K - 1 else torch.empty((R, 3, A, S), dtype=_F32, device=dev)
         g_op = torch.empty((1, A, S), dtype=_F32, device=dev)
         if A > 0:
-            _lib.call("lgs_project_backward", state.sh_degree, _ptr(state.chunk_ids), ctypes.c_void_p(state.counters.data_ptr()),
+            _lib.call(pb, state.sh_degree, _ptr(state.chunk_ids), ctypes.c_void_p(state.counters.data_ptr()),
                       _ptr(state.view), _ptr(state.proj), _ptr(xyz), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["opacity"]),
                       C, S, A, R, H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(pg), None, 0, _ptr(g_pos), _ptr(g_sc), _ptr(g_rot),
-                      _ptr(g_s0), _ptr(g_sr), _ptr(g_op), None, *cam_args, _ptr(state.filter_3d), int(state.antialiased), *exact_args, depth_arg, st)
+                      _ptr(g_s0), _ptr(g_sr), _ptr(g_op), None, *cam_args, _ptr(state.filter_3d), int(state.antialiased), *exact_args, depth_arg,
+                      *pb_tail, st)
         elif camera_grad is not None:
             camera_grad.zero_()
     return [g_pos, g_sc, g_rot, g_s0, g_sr, g_op], pg
@@ -367,6 +397,9 @@ class ViewWorkspace:
         self.d_img = e((1, 3, self.Hp, self.Wp), _F32)
         self.depth = self.d_depth = self.d_trans = None     # f32[1,1,Hp,Wp] each, allocated on first use (depth mode, d_trans)
         self.rendered_depth = False                          # whether the last forward on this workspace rendered depth
+        self.normal = self.d_normal = None                   # f32[1,3,Hp,Wp] each, allocated on first use (normal mode)
+        self.normal_rec = self.grad_normal = None            # f32[N,4] each, allocated on first use (normal mode)
+        self.rendered_normal = False                         # whether the last forward on this workspace rendered normals
         self.cam_view, self.cam_proj, self.cam_planes = e((1, 4, 4), _F32), e((1, 4, 4), _F32), e((1, 6, 4), _F32)
         self.cam_partials, self.d_cam = e((C, 32), _F32), e((2, 4, 4), _F32)     # camera gradient: per-chunk rows, their sum
         nb = max(_query_bytes("lgs_sort_pairs_u32_workspace_bytes", _round_up(N, 1 << 16)),
@@ -381,13 +414,15 @@ class ViewWorkspace:
         self.views_done = 0
 
     # -- enqueue ---------------------------------------------------------------------------------------------------
-    def _plane(self, name):
-        """The f32[1,1,Hp,Wp] buffer `name`, allocated the first time it is asked for (its pointer then stays fixed)."""
+    def _plane(self, name, shape=None):
+        """The f32 buffer `name` (default shape [1,1,Hp,Wp]), allocated the first time it is asked for (its pointer then stays
+        fixed)."""
         if getattr(self, name) is None:
-            setattr(self, name, torch.zeros((1, 1, self.Hp, self.Wp), dtype=_F32, device=self.dev))
+            setattr(self, name, torch.zeros(shape or (1, 1, self.Hp, self.Wp), dtype=_F32, device=self.dev))
         return getattr(self, name)
 
-    def _forward_kernels(self, params, cluster_origin, cluster_extend, sh_degree, clamp_zero, antialiased, filter_3d, render_depth):
+    def _forward_kernels(self, params, cluster_origin, cluster_extend, sh_degree, clamp_zero, antialiased, filter_3d, render_depth,
+                         render_normal=False):
         dev, st = self.dev, _stream(self.dev)
         H, W = self.hw
         th, tw = self.tile
@@ -396,10 +431,11 @@ class ViewWorkspace:
         vp = self.vparams.data_ptr()
         _lib.call("lgs_frustum_culling_aabb", _ptr(cluster_origin), _ptr(cluster_extend), _ptr(self.cam_planes), C, 1, _ptr(self.vis),
                   ctypes.c_void_p(cnt), _ptr(self.chunk_ids), st)
-        _lib.call("lgs_project_forward", int(sh_degree), _ptr(self.chunk_ids), ctypes.c_void_p(cnt), _ptr(self.cam_view), _ptr(self.cam_proj),
+        _lib.call("lgs_project_forward_normal" if render_normal else "lgs_project_forward", int(sh_degree), _ptr(self.chunk_ids),
+                  ctypes.c_void_p(cnt), _ptr(self.cam_view), _ptr(self.cam_proj),
                   _ptr(params["xyz"]), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["sh_0"]), _ptr(params["sh_rest"]),
                   _ptr(params["opacity"]), C, S, C, H, W, th, tw, _ptr(self.packed), _ptr(self.dkey), _ptr(self.iota), _ptr(self.tcount),
-                  ctypes.c_void_p(cnt + 4), _ptr(filter_3d), int(antialiased), st)
+                  ctypes.c_void_p(cnt + 4), _ptr(filter_3d), int(antialiased), *((_ptr(self.normal_rec),) if render_normal else ()), st)
         _lib.call("lgs_view_params", ctypes.c_void_p(cnt), S, D, self.planned_bits, ctypes.c_void_p(vp), _ptr(self.sticky), st)
         n_dev, d_dev, bias_dev = ctypes.c_void_p(vp), ctypes.c_void_p(vp + 4), ctypes.c_void_p(vp + 8)
         wsz = ctypes.c_size_t(self.ws_bytes)
@@ -415,32 +451,37 @@ class ViewWorkspace:
         _lib.call("lgs_tile_range_u16_dev" if self.u16 else "lgs_tile_range_dev", _ptr(self.keys_s), D, d_dev, self.ntile,
                   int(CONFIG["fix_last_tile"]), _ptr(self.ranges), st)
         order = CONFIG["tile_order"]
-        _lib.call("lgs_rasterize_forward_packed", _ptr(self.sorted_pid), _ptr(self.ranges), _ptr(self.packed), None, 0, 1, N, D, H, W, th, tw,
+        _lib.call("lgs_rasterize_forward_packed_normal" if render_normal else "lgs_rasterize_forward_packed", _ptr(self.sorted_pid),
+                  _ptr(self.ranges), _ptr(self.packed), None, 0, 1, N, D, H, W, th, tw,
                   0, int(bool(clamp_zero)), _ptr(self.img), _ptr(self.T), _ptr(self.last), None, None, _ptr(self.work) if order else None,
-                  _ptr(self.depth) if render_depth else None, st)
+                  _ptr(self.depth) if render_depth else None, *((_ptr(self.normal_rec), _ptr(self.normal)) if render_normal else ()), st)
         if order:
             _lib.call("lgs_tile_order", _ptr(self.work), 1, self.ntile, _ptr(self.tile_order), st)
 
     def _backward_kernels(self, params, sh_degree, accumulate_into, use_clamp, camera_grad, antialiased, filter_3d, exact_grad, depth,
-                          trans):
+                          trans, normal=False):
         st = _stream(self.dev)
         H, W = self.hw
         th, tw = self.tile
         C, S, N, D = self.C, self.S, self.Nmax, self.cap
         tiles = self.tile_order if CONFIG["tile_order"] else None
-        _lib.call("lgs_rasterize_backward", _ptr(self.sorted_pid), _ptr(self.ranges), _ptr(self.packed), _ptr(tiles),
+        _lib.call("lgs_rasterize_backward_normal" if normal else "lgs_rasterize_backward", _ptr(self.sorted_pid), _ptr(self.ranges),
+                  _ptr(self.packed), _ptr(tiles),
                   self.ntile if tiles is not None else 0, _ptr(self.T), _ptr(self.last), _ptr(self.d_img), _ptr(self.d_trans) if trans else None,
                   _ptr(self.img) if use_clamp else None, None, 1, N, D, H, W, th, tw, 0, _ptr(self.pg), None, None, None, None, None, None,
-                  _ptr(self.d_depth) if depth else None, st)
+                  _ptr(self.d_depth) if depth else None,
+                  *((_ptr(self.normal_rec), _ptr(self.d_normal), _ptr(self.grad_normal)) if normal else ()), st)
         d = accumulate_into
         R = params["sh_rest"].shape[0]
         # A = all chunks: project_backward returns at once for chunks past the (device) visible count
-        _lib.call("lgs_project_backward", int(sh_degree), _ptr(self.chunk_ids), ctypes.c_void_p(self.counters.data_ptr()), _ptr(self.cam_view),
+        _lib.call("lgs_project_backward_normal" if normal else "lgs_project_backward", int(sh_degree), _ptr(self.chunk_ids),
+                  ctypes.c_void_p(self.counters.data_ptr()), _ptr(self.cam_view),
                   _ptr(self.cam_proj), _ptr(params["xyz"]), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["opacity"]), C, S, C, R,
                   H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(self.pg), None, 2, _ptr(d["xyz"]), _ptr(d["scale"]), _ptr(d["rot"]),
                   _ptr(d["sh_0"]), _ptr(d["sh_rest"]), _ptr(d["opacity"]), _ptr(d.get("_touched")),
                   _ptr(self.cam_partials) if camera_grad else None, _ptr(self.d_cam) if camera_grad else None, _ptr(filter_3d),
-                  int(antialiased), _ptr(params["sh_0"]), _ptr(params["sh_rest"]), int(exact_grad), int(depth), st)
+                  int(antialiased), _ptr(params["sh_0"]), _ptr(params["sh_rest"]), int(exact_grad), int(depth),
+                  *((_ptr(self.grad_normal),) if normal else ()), st)
 
     def _run(self, kind, sig, fn):
         """Eager the first time a pointer signature is seen, captured into a CUDA graph the second time, replayed afterwards."""
@@ -464,10 +505,11 @@ class ViewWorkspace:
         g.replay()
 
     def forward(self, params, cluster_origin, cluster_extend, cam, sh_degree, clamp_zero=True, antialiased=False, filter_3d=None,
-                render_depth=False):
+                render_depth=False, render_normal=False):
         """cam: dict(view, proj, frustumplane) of device tensors.  Returns the padded image (a view of the workspace).
         render_depth: also render the per-pixel depth D into ``self.depth`` (f32[1,1,Hp,Wp], DESIGN.md section 1); the transmittance
         is ``self.T``.
+        render_normal: also render the per-pixel normal N into ``self.normal`` (f32[1,3,Hp,Wp], DESIGN.md section 1, "Normals").
         antialiased: antialiased mode (DESIGN.md section 1); the backward of this view must be given the same value.
         filter_3d: 3D smoothing filter f32[1,C,S] or None; the backward of this view must be given the same tensor.  Its data
         pointer is part of the graph signature: a replayed graph reads whatever the tensor holds, so recomputing it in place
@@ -475,6 +517,9 @@ class ViewWorkspace:
         filter_3d = check_filter_3d(filter_3d, params["xyz"])
         if render_depth:
             self._plane("depth")
+        if render_normal:
+            self._plane("normal", (1, 3, self.Hp, self.Wp))
+            self._plane("normal_rec", (self.Nmax, 4))
         self.cam_view.copy_(cam["view"], non_blocking=True)
         self.cam_proj.copy_(cam["proj"], non_blocking=True)
         self.cam_planes.copy_(cam["frustumplane"], non_blocking=True)
@@ -483,20 +528,25 @@ class ViewWorkspace:
                0 if filter_3d is None else filter_3d.data_ptr(), bool(antialiased))
         if render_depth:
             sig += ("depth",)
+        if render_normal:
+            sig += ("normal",)
         self._run("fwd", sig, lambda: self._forward_kernels(params, cluster_origin, cluster_extend, sh_degree, clamp_zero, antialiased,
-                                                            filter_3d, bool(render_depth)))
+                                                            filter_3d, bool(render_depth), bool(render_normal)))
         self.rendered_depth = bool(render_depth)
+        self.rendered_normal = bool(render_normal)
         self.views_done += 1
         return self.img
 
     def backward(self, params, d_img, sh_degree, accumulate_into, use_clamp=True, camera_grad=None, antialiased=False, filter_3d=None,
-                 exact_grad=False, d_depth=None, d_trans=None):
+                 exact_grad=False, d_depth=None, d_trans=None, d_normal=None):
         """d_img f32[1,3,H,W] or [1,3,Hp,Wp]: gradient of the loss w.r.t. the (clamped) image.  camera_grad (optional f32[2,4,4]
         CUDA tensor) receives (d view_matrix, d proj_matrix) of this view, copied on the stream after the backward.
         antialiased, filter_3d: the values the forward of this view was given.  exact_grad: exact gradient mode (DESIGN.md
         section 1); a backward-only choice, so it is part of the backward graph's signature and of nothing else.
         d_depth, d_trans: f32[1,1,H,W] or [1,1,Hp,Wp] gradients of the depth (the forward must have rendered it) and of the
-        transmittance, or None; whether each is given is part of the backward graph's signature."""
+        transmittance, or None; whether each is given is part of the backward graph's signature.
+        d_normal: f32[1,3,H,W] or [1,3,Hp,Wp] gradient of the normal (the forward must have rendered it), or None; whether it is
+        given is part of the backward graph's signature."""
         filter_3d = check_filter_3d(filter_3d, params["xyz"])
         if camera_grad is not None and not (camera_grad.is_cuda and camera_grad.dtype == _F32 and tuple(camera_grad.shape) == (2, 4, 4)):
             raise RuntimeError("camera_grad must be a float32 CUDA tensor of shape [2,4,4]")
@@ -509,10 +559,14 @@ class ViewWorkspace:
             self.d_img[..., :H, :W].copy_(d_img, non_blocking=True)
         if d_depth is not None and not self.rendered_depth:
             raise RuntimeError("d_depth is given, but the last forward on this workspace did not render depth (render_depth=False)")
-        for name, g in (("d_depth", d_depth), ("d_trans", d_trans)):
+        if d_normal is not None and not self.rendered_normal:
+            raise RuntimeError("d_normal is given, but the last forward on this workspace did not render normals (render_normal=False)")
+        if d_normal is not None:
+            self._plane("grad_normal", (self.Nmax, 4))
+        for name, g in (("d_depth", d_depth), ("d_trans", d_trans), ("d_normal", d_normal)):
             if g is None:
                 continue
-            plane = self._plane(name)
+            plane = self._plane(name, (1, 3, self.Hp, self.Wp) if name == "d_normal" else None)
             if g.shape[-2:] == (self.Hp, self.Wp):
                 plane.copy_(g, non_blocking=True)
             else:
@@ -526,9 +580,12 @@ class ViewWorkspace:
                camera_grad is not None)
         if d_depth is not None or d_trans is not None:
             sig += (("depth", d_depth is not None, d_trans is not None),)
+        if d_normal is not None:
+            sig += ("normal",)
         cam = camera_grad is not None
         self._run("bwd", sig, lambda: self._backward_kernels(params, sh_degree, accumulate_into, use_clamp, cam, antialiased, filter_3d,
-                                                             bool(exact_grad), d_depth is not None, d_trans is not None))
+                                                             bool(exact_grad), d_depth is not None, d_trans is not None,
+                                                             d_normal is not None))
         if cam:
             camera_grad.copy_(self.d_cam, non_blocking=True)
 

@@ -70,7 +70,7 @@ def render(view_matrix, proj_matrix, xyz, scale, rot, color, opacity,
            valid_length, feedback_binning_allocate_size, idx_tensor,
            actived_sh_degree: int, output_shape, pp):
     """Projection -> binning -> rasterisation; returns (img, transmittance, depth, normal, primitive_visible)
-    as render/__init__.py:50-94.  The antialiased, exact gradient and depth modes exist on the fused path only (render_view,
+    as render/__init__.py:50-94.  The antialiased, exact gradient, depth and normal modes exist on the fused path only (render_view,
     render_views)."""
     if getattr(pp, "antialiased", False):
         raise RuntimeError("pp.antialiased is set, but the op-by-op render() has no antialiased mode and would draw every splat "
@@ -81,6 +81,9 @@ def render(view_matrix, proj_matrix, xyz, scale, rot, color, opacity,
     if getattr(pp, "render_depth", False):
         raise RuntimeError("pp.render_depth is set, but the op-by-op render() has no depth mode (its depth slot keeps the reference's "
                            "enable_depth contract); render through render_view or render_views instead")
+    if getattr(pp, "render_normal", False):
+        raise RuntimeError("pp.render_normal is set, but the op-by-op render() has no normal mode (its normal slot stays None); "
+                           "render through render_view or render_views instead")
     nvtx.range_push("Proj")
     view_pos, ndc_pos = wrapper.MVPTransform.apply(xyz, view_matrix, proj_matrix, valid_length)
     transform_matrix = wrapper.CreateTransformMatrix.call_fused(scale, rot, valid_length)
@@ -142,14 +145,15 @@ class _RenderViewFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, xyz, scale, rot, sh_0, sh_rest, opacity, cluster_origin, cluster_extend, frustumplane,
                 view_matrix, proj_matrix, sh_degree, H, W, th, tw, sparse_grad, enable_transmitance, accumulate_into, antialiased,
-                filter_3d, exact_grad, render_depth):
+                filter_3d, exact_grad, render_depth, render_normal):
         params = dict(xyz=xyz, scale=scale, rot=rot, sh_0=sh_0, sh_rest=sh_rest, opacity=opacity)
         stat = bool(StatisticsHelperInst.bStart)
         ctx.set_materialize_grads(False)       # an unused transmittance output must not cost a zero-filled gradient image
         # the kernel writes clamp(c,0,1) directly (render/__init__.py:87 does it as a separate pass) ...
         img, state, stats = pipeline.render_view_forward(params, cluster_origin, cluster_extend, frustumplane, view_matrix,
                                                          proj_matrix, sh_degree, (H, W), (th, tw), enable_statistic=stat, clamp_zero=True,
-                                                         antialiased=antialiased, filter_3d=filter_3d, render_depth=render_depth)
+                                                         antialiased=antialiased, filter_3d=filter_3d, render_depth=render_depth,
+                                                         render_normal=render_normal)
         ctx.state = state
         ctx.stats = stats
         ctx.stat = stat
@@ -159,10 +163,10 @@ class _RenderViewFn(torch.autograd.Function):
         ctx.exact_grad = bool(exact_grad)           # backward only: the forward does not depend on it
         ctx.save_for_backward(xyz, scale, rot, sh_0, sh_rest, opacity, img)
         ctx.mark_non_differentiable(state.last)
-        return img, state.T, state.last, state.depth          # depth: None unless render_depth
+        return img, state.T, state.last, state.depth, state.normal   # depth, normal: None unless render_depth, render_normal
 
     @staticmethod
-    def backward(ctx, g_img, g_T, _g_last, g_depth):
+    def backward(ctx, g_img, g_T, _g_last, g_depth, g_normal):
         xyz, scale, rot, sh_0, sh_rest, opacity, img_out = ctx.saved_tensors
         params = dict(xyz=xyz, scale=scale, rot=rot, sh_0=sh_0, sh_rest=sh_rest, opacity=opacity)
         state = ctx.state
@@ -176,7 +180,7 @@ class _RenderViewFn(torch.autograd.Function):
         grads, pg = pipeline.render_view_backward(params, state, g_img, g_T if (ctx.trans and g_T is not None) else None,
                                                   enable_statistic=ctx.stat,
                                                   accumulate_into=ctx.accumulate_into, clamped_img=img_out, camera_grad=cam,
-                                                  exact_grad=ctx.exact_grad, d_depth=g_depth)
+                                                  exact_grad=ctx.exact_grad, d_depth=g_depth, d_normal=g_normal)
         if ctx.stat:
             _feed_statistics(state, ctx.stats, pg, state.tile)
         g_view = g_proj = None
@@ -185,7 +189,7 @@ class _RenderViewFn(torch.autograd.Function):
             g_proj = cam[1].reshape(state.proj.shape) if ctx.needs_input_grad[10] else None
         if grads is None:          # gradients went straight into the caller's dense buffers
             ctx.state = None
-            return (None,) * 9 + (g_view, g_proj) + (None,) * 12
+            return (None,) * 9 + (g_view, g_proj) + (None,) * 13
         C, S = xyz.shape[-2:]
         ids = state.chunk_ids[: state.n_chunks_visible]
         out = []
@@ -193,7 +197,7 @@ class _RenderViewFn(torch.autograd.Function):
             ct = CompactedTensor((*g.shape[:-2], C, S), ids, g)
             out.append(ct if ctx.sparse else ct.to_dense())
         ctx.state = None
-        return (*out, None, None, None, g_view, g_proj, None, None, None, None, None, None, None, None, None, None, None, None)
+        return (*out, None, None, None, g_view, g_proj, None, None, None, None, None, None, None, None, None, None, None, None, None)
 
 
 def render_view(cluster_origin, cluster_extend, frustumplane, view_matrix, proj_matrix,
@@ -211,19 +215,24 @@ def render_view(cluster_origin, cluster_extend, frustumplane, view_matrix, proj_
     ``pp.render_depth`` (absent = False) also renders the per-pixel depth D = sum_i w_i z_i (DESIGN.md section 1, "Depth") and
     returns it, differentiable, in the depth slot as [1,1,H,W]; the expected depth is D / (1 - transmittance).  ``pp.enable_depth``
     keeps the reference's meaning.
+    ``pp.render_normal`` (absent = False) also renders the per-pixel normal N = sum_i w_i n_i, n_i the camera-facing view-space
+    normal of Gaussian i's shortest axis (DESIGN.md section 1, "Normals"), and returns it, differentiable, in the normal slot as
+    [1,3,H,W]; the expected normal is N / (1 - transmittance), the unit normal N / |N|.
     ``filter_3d`` (f32[1,C,S] or None): Mip-Splatting's 3D smoothing filter (scene.filter_3d_device, DESIGN.md section 1); it is
     an input without a gradient."""
     if not pp.cluster_size:
         raise RuntimeError("render_view needs the clustered layout (cluster_size > 0); use render_preprocess + render otherwise")
     H, W = int(output_shape[0]), int(output_shape[1])
     th, tw = int(pp.tile_size[0]), int(pp.tile_size[1])
-    img, T, last, depth = _RenderViewFn.apply(xyz, scale, rot, sh_0, sh_rest, opacity, cluster_origin, cluster_extend, frustumplane,
-                                              view_matrix, proj_matrix, int(actived_sh_degree), H, W, th, tw, pp.sparse_grad,
-                                              pp.enable_transmitance, accumulate_into, bool(getattr(pp, "antialiased", False)),
-                                              filter_3d, bool(getattr(pp, "exact_grad", False)), bool(getattr(pp, "render_depth", False)))
+    img, T, last, depth, normal = _RenderViewFn.apply(xyz, scale, rot, sh_0, sh_rest, opacity, cluster_origin, cluster_extend,
+                                                      frustumplane, view_matrix, proj_matrix, int(actived_sh_degree), H, W, th, tw,
+                                                      pp.sparse_grad, pp.enable_transmitance, accumulate_into,
+                                                      bool(getattr(pp, "antialiased", False)), filter_3d,
+                                                      bool(getattr(pp, "exact_grad", False)), bool(getattr(pp, "render_depth", False)),
+                                                      bool(getattr(pp, "render_normal", False)))
     img = img[..., :H, :W]          # already clamped to [0,1] by the kernel
     trans = T[..., :H, :W] if pp.enable_transmitance else None
-    return img, trans, None if depth is None else depth[..., :H, :W], None, last
+    return (img, trans, None if depth is None else depth[..., :H, :W], None if normal is None else normal[..., :H, :W], last)
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -269,7 +278,12 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
     ``pp.render_depth`` (absent = False): every view also renders its depth (see render_view), and the callbacks take it with the
     transmittance: ``loss_fn(i, img, depth, trans)`` -> scalar (autograd over the three [1,C,H,W] inputs) or ``(loss, d_img,
     d_depth, d_trans)``, and ``loss_and_grad_fn(i, img, depth, trans) -> (loss, d_img, d_depth, d_trans)``, where d_depth and
-    d_trans may be None.  An expected-depth loss uses depth / (1 - trans).  Without the flag both callbacks are called as above."""
+    d_trans may be None.  An expected-depth loss uses depth / (1 - trans).  Without the flag both callbacks are called as above.
+
+    ``pp.render_normal`` (absent = False): every view also renders its normal (see render_view), and the callbacks take it
+    appended to the depth form: ``loss_fn(i, img, depth, trans, normal)`` -> scalar or ``(loss, d_img, d_depth, d_trans,
+    d_normal)``, and ``loss_and_grad_fn(i, img, depth, trans, normal) -> (loss, d_img, d_depth, d_trans, d_normal)``; depth (and
+    d_depth) is None unless ``pp.render_depth`` is set.  Without the flag the callbacks are called as above."""
     dev = xyz.device
     filter_3d = pipeline.check_filter_3d(filter_3d, xyz)
     if camera_grads is not None and not (camera_grads.is_cuda and camera_grads.dtype == torch.float32 and camera_grads.is_contiguous()
@@ -282,6 +296,7 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
     aa = bool(getattr(pp, "antialiased", False))
     exact = bool(getattr(pp, "exact_grad", False))
     dep = bool(getattr(pp, "render_depth", False))
+    nrm = bool(getattr(pp, "render_normal", False))
     direct = loss_and_grad_fn is not None or _DIRECT_VIEWS
     if direct:
         params = dict(xyz=xyz.detach(), scale=scale.detach(), rot=rot.detach(), sh_0=sh_0.detach(), sh_rest=sh_rest.detach(),
@@ -292,10 +307,11 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
         cam = camera_fn(i)
         img_p, state, stats = pipeline.render_view_forward(params, cluster_origin, cluster_extend, cam["frustumplane"], cam["view"],
                                                            cam["proj"], int(actived_sh_degree), (H, W), (th, tw), enable_statistic=stat,
-                                                           clamp_zero=True, antialiased=aa, filter_3d=filter_3d, render_depth=dep)
-        d_depth = d_trans = None
-        if dep:
-            loss, d_img, d_depth, d_trans = _depth_loss(i, img_p, state.depth, state.T, H, W)
+                                                           clamp_zero=True, antialiased=aa, filter_3d=filter_3d, render_depth=dep,
+                                                           render_normal=nrm)
+        d_depth = d_trans = d_normal = None
+        if dep or nrm:
+            loss, d_img, d_depth, d_trans, d_normal = _ext_loss(i, img_p, state.depth, state.T, state.normal)
         elif loss_and_grad_fn is not None:
             loss, d_img = loss_and_grad_fn(i, img_p[..., :H, :W])
         else:                          # autograd only through the user's loss, never through the render kernels
@@ -312,7 +328,8 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
         if wait_ev is not None:
             torch.cuda.current_stream(dev).wait_event(wait_ev)
         _, pg_ = pipeline.render_view_backward(params, state, d_img, d_trans, enable_statistic=stat, accumulate_into=accumulate_into,
-                                               clamped_img=img_p, camera_grad=slot(i), exact_grad=exact, d_depth=d_depth)
+                                               clamped_img=img_p, camera_grad=slot(i), exact_grad=exact, d_depth=d_depth,
+                                               d_normal=d_normal)
         if stat:
             _feed_statistics(state, stats, pg_, (th, tw))
         losses.append(loss.detach())
@@ -323,18 +340,21 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
         if camera_grads is not None:              # leaves of this call: their .grad is view i's camera gradient
             view, proj = view.detach().requires_grad_(True), proj.detach().requires_grad_(True)
         pp_i = pp
-        if dep and not pp.enable_transmitance:    # the depth callbacks take the transmittance
+        if (dep or nrm) and not pp.enable_transmitance:    # the depth / normal callbacks take the transmittance
             pp_i = copy.copy(pp)
             pp_i.enable_transmitance = True
         out = render_view(cluster_origin, cluster_extend, cam["frustumplane"], view, proj, xyz, scale, rot, sh_0, sh_rest,
                           opacity, actived_sh_degree, output_shape, pp_i, accumulate_into=accumulate_into, filter_3d=filter_3d)
         img = out[0]
-        loss = loss_fn(i, img, out[2], out[1]) if dep else loss_fn(i, img)
+        if nrm:
+            loss = loss_fn(i, img, out[2], out[1], out[3])
+        else:
+            loss = loss_fn(i, img, out[2], out[1]) if dep else loss_fn(i, img)
         if wait_ev is not None:          # the previous view's accumulate (other stream) must have landed
             torch.cuda.current_stream(dev).wait_event(wait_ev)
-        if isinstance(loss, tuple) and dep:
+        if isinstance(loss, tuple) and (dep or nrm):
             loss, *gs = loss
-            pairs = [(t, g) for t, g in zip((img, out[2], out[1]), gs) if g is not None]
+            pairs = [(t, g) for t, g in zip((img, out[2], out[1], out[3]), gs) if t is not None and g is not None]
             torch.autograd.backward([t for t, _ in pairs], [g for _, g in pairs])
         elif isinstance(loss, tuple):
             loss, d_img = loss
@@ -358,10 +378,10 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
     def one_ws(i, wait_ev, ws):
         cam = camera_fn(i)
         img_p = ws.forward(params, cluster_origin, cluster_extend, cam, int(actived_sh_degree), clamp_zero=True, antialiased=aa,
-                           filter_3d=filter_3d, render_depth=dep)
-        d_depth = d_trans = None
-        if dep:
-            loss, d_img, d_depth, d_trans = _depth_loss(i, img_p, ws.depth, ws.T, H, W)
+                           filter_3d=filter_3d, render_depth=dep, render_normal=nrm)
+        d_depth = d_trans = d_normal = None
+        if dep or nrm:
+            loss, d_img, d_depth, d_trans, d_normal = _ext_loss(i, img_p, ws.depth if dep else None, ws.T, ws.normal if nrm else None)
         elif loss_and_grad_fn is not None:
             loss, d_img = loss_and_grad_fn(i, img_p[..., :H, :W])
         else:
@@ -374,20 +394,28 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
         if wait_ev is not None:
             torch.cuda.current_stream(dev).wait_event(wait_ev)
         ws.backward(params, d_img, int(actived_sh_degree), accumulate_into, use_clamp=True, camera_grad=slot(i), antialiased=aa,
-                    filter_3d=filter_3d, exact_grad=exact, d_depth=d_depth, d_trans=d_trans)
+                    filter_3d=filter_3d, exact_grad=exact, d_depth=d_depth, d_trans=d_trans, d_normal=d_normal)
         losses.append(loss.detach())
 
-    def _depth_loss(i, img_p, depth_p, T_p, H, W):
-        """The depth-mode callbacks on the padded outputs of one view -> (loss, d_img, d_depth or None, d_trans or None)."""
-        img, depth, trans = img_p[..., :H, :W], depth_p[..., :H, :W], T_p[..., :H, :W]
+    def _ext_loss(i, img_p, depth_p, T_p, normal_p):
+        """The depth / normal-mode callbacks on the padded outputs of one view -> (loss, d_img, d_depth, d_trans, d_normal); each
+        gradient but d_img may be None.  depth_p is None unless render_depth; the normal is passed (appended) only in normal mode."""
+        ins = [img_p[..., :H, :W], None if depth_p is None else depth_p[..., :H, :W], T_p[..., :H, :W]]
+        if nrm:
+            ins.append(normal_p[..., :H, :W])
         if loss_and_grad_fn is not None:
-            return tuple(loss_and_grad_fn(i, img, depth, trans))
-        leaves = [t.detach().requires_grad_(True) for t in (img, depth, trans)]
-        loss = loss_fn(i, *leaves)
-        if isinstance(loss, tuple):
-            return tuple(loss)
-        d_img, d_depth, d_trans = torch.autograd.grad(loss, leaves, allow_unused=True)
-        return loss, (torch.zeros_like(img) if d_img is None else d_img), d_depth, d_trans
+            out = tuple(loss_and_grad_fn(i, *ins))
+        else:
+            leaves = [None if t is None else t.detach().requires_grad_(True) for t in ins]
+            loss = loss_fn(i, *leaves)
+            if isinstance(loss, tuple):
+                out = tuple(loss)
+            else:
+                gs = iter(torch.autograd.grad(loss, [t for t in leaves if t is not None], allow_unused=True))
+                out = (loss, *(None if t is None else next(gs) for t in leaves))
+        loss, d_img, d_depth, d_trans = out[:4]
+        d_normal = out[4] if nrm else None
+        return loss, (torch.zeros_like(ins[0]) if d_img is None else d_img), d_depth, d_trans, d_normal
 
     def one_probe(i, wait_ev):
         n0 = len(pipeline.LAST_VIEW_SIZES)
