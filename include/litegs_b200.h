@@ -205,22 +205,17 @@ int lgs_pack_params(const float* ndc, const float* cov2d_inv, const float* color
  * depth f32[V,1,Hp,Wp] or NULL, ours (the reference leaves its depth image zero): per pixel D = sum_i w_i z_i with the weights of
  * the colour and z_i the record's depth slot (the view-space z on the fused path), not clamped (DESIGN.md section 1, "Depth").
  * Only the default kernel renders depth: with bulk staging or the pixel-pair forward selected, a non-NULL depth is refused.
- * NULL = no depth, the same kernels as before. */
+ * NULL = no depth, the same kernels as before.
+ * normal_rec f32[V,N,4] (lgs_project_forward's side rows, aligned with packed_params) and normal f32[V,3,Hp,Wp], both given or
+ * both NULL, ours (DESIGN.md section 1, "Normals"): per pixel N = sum_i w_i n_i with the weights of the colour, neither clamped
+ * nor normalised.  Like depth, only the default kernel renders it: with bulk staging or the pixel-pair forward selected, a
+ * non-NULL normal is refused.  NULL = no normal, the same kernels as before. */
 int lgs_rasterize_forward_packed(const int* sorted_points, const int* start_index, const float* packed_params,
                                  const int* specific_tiles, int n_specific, int V, int N, int cap, int img_h, int img_w,
                                  int tile_h, int tile_w, int enable_statistic, int clamp_zero, float* img,
                                  float* transmittance, short* last_contributor, int* fragment_count,
-                                 float* fragment_weight, int* tile_work, float* depth, void* stream);
-/* The same with the normal channels, ours (DESIGN.md section 1, "Normals"): normal_rec f32[V,N,4] (lgs_project_forward_normal's
- * side rows, aligned with packed_params) and normal f32[V,3,Hp,Wp], both given or both NULL.  Per pixel N = sum_i w_i n_i with the
- * weights of the colour, neither clamped nor normalised.  Like depth, only the default kernel renders it: with bulk staging or
- * the pixel-pair forward selected, a non-NULL normal is refused.  NULL = lgs_rasterize_forward_packed. */
-int lgs_rasterize_forward_packed_normal(const int* sorted_points, const int* start_index, const float* packed_params,
-                                        const int* specific_tiles, int n_specific, int V, int N, int cap, int img_h, int img_w,
-                                        int tile_h, int tile_w, int enable_statistic, int clamp_zero, float* img,
-                                        float* transmittance, short* last_contributor, int* fragment_count,
-                                        float* fragment_weight, int* tile_work, float* depth, const float* normal_rec, float* normal,
-                                        void* stream);
+                                 float* fragment_weight, int* tile_work, float* depth, const float* normal_rec, float* normal,
+                                 void* stream);
 
 /* order i32[V,tiles] = 1-based tile ids by descending work (heaviest lists first), to be passed as specific_tiles:
  * the device-side form of the reference's tile scheduling by last epoch's blend count (render/__init__.py:75-79,
@@ -235,25 +230,18 @@ int lgs_tile_order(const int* work, int V, int ntile, int* order, void* stream);
  * d_depth f32[V,1,Hp,Wp] or NULL, ours: dL/dD of the forward's depth image.  It joins the alpha gradient as one more colour
  * channel with colour z, and packed_grad slot 10 receives sum_pixels w g_z = dL/dz (consumed by lgs_project_backward with depth
  * = 1; the unpack ignores it).  Only the pixel-pair kernel (the default, and the deterministic mode) takes it: with the scalar
- * kernel or bulk staging selected, a non-NULL d_depth is refused.  NULL = no depth gradient, the same kernels as before. */
+ * kernel or bulk staging selected, a non-NULL d_depth is refused.  NULL = no depth gradient, the same kernels as before.
+ * normal_rec f32[V,N,4] (the forward's side rows), d_normal f32[V,3,Hp,Wp] = dL/dN and grad_normal f32[V,N,4] (zeroed here), all
+ * given or all NULL, ours: dL/dN joins the alpha gradient as three more colour channels with colour n (after the depth term), and
+ * grad_normal receives sum_pixels w g_N = dL/dn (consumed by lgs_project_backward).  Pixel-pair kernel and deterministic mode
+ * only, as d_depth.  NULL = no normal gradient, the same kernels as before. */
 int lgs_rasterize_backward(const int* sorted_points, const int* start_index, const float* packed_params,
                            const int* specific_tiles, int n_specific, const float* final_transmittance,
                            const short* last_contributor, const float* d_img, const float* d_trans_img,
                            const float* clamped_img, const float* grad_inv_scaler, int V, int N, int cap, int img_h, int img_w, int tile_h,
                            int tile_w, int enable_statistic, float* packed_grad, float* d_ndc, float* d_cov2d_inv,
                            float* d_color, float* d_opacity, float* err_sum, float* err_square_sum, const float* d_depth,
-                           void* stream);
-/* The same with the normal gradient, ours: normal_rec f32[V,N,4] (the forward's side rows), d_normal f32[V,3,Hp,Wp] = dL/dN and
- * grad_normal f32[V,N,4] (zeroed here), all given or all NULL.  dL/dN joins the alpha gradient as three more colour channels
- * with colour n (after the depth term), and grad_normal receives sum_pixels w g_N = dL/dn (consumed by
- * lgs_project_backward_normal).  Pixel-pair kernel and deterministic mode only, as d_depth.  NULL = lgs_rasterize_backward. */
-int lgs_rasterize_backward_normal(const int* sorted_points, const int* start_index, const float* packed_params,
-                                  const int* specific_tiles, int n_specific, const float* final_transmittance,
-                                  const short* last_contributor, const float* d_img, const float* d_trans_img,
-                                  const float* clamped_img, const float* grad_inv_scaler, int V, int N, int cap, int img_h, int img_w,
-                                  int tile_h, int tile_w, int enable_statistic, float* packed_grad, float* d_ndc, float* d_cov2d_inv,
-                                  float* d_color, float* d_opacity, float* err_sum, float* err_square_sum, const float* d_depth,
-                                  const float* normal_rec, const float* d_normal, float* grad_normal, void* stream);
+                           const float* normal_rec, const float* d_normal, float* grad_normal, void* stream);
 
 /* staging selector for the raster kernels: 0 = cp.async / LDGSTS (default), 1 = cp.async.bulk + mbarrier */
 int lgs_set_staging(int bulk);
@@ -291,22 +279,16 @@ int lgs_set_err_square_mode(int mode);
  * filter_3d f32[C*S] (clustered like opacity) or NULL: Mip-Splatting's 3D smoothing filter, ours (the reference has none).  Each
  * Gaussian's activated scale becomes s' = sqrt(s^2 + f^2) in the whole chain (S.R, M, the 2D covariance, the tile walk) and its
  * opacity sigmoid(opacity) * rho3 with rho3 = sqrt(prod_k s_k^2 / (s_k^2 + f^2)), before the antialiased factor
- * (DESIGN.md section 1, "3D smoothing filter").  NULL = no filter, the same kernels as before. */
+ * (DESIGN.md section 1, "3D smoothing filter").  NULL = no filter, the same kernels as before.
+ * normal_rec f32[A*S,4] or NULL, ours (DESIGN.md section 1, "Normals"): receives (n0, n1, n2, 0) per slot, the view-space normal
+ * of the Gaussian's shortest axis (argmin of the raw log-scales), turned to face the camera; slots of chunks at or past the
+ * visible count get zeros.  NULL = no normals, the same kernels as before. */
 int lgs_project_forward(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
                         const float* view_matrix, const float* proj_matrix, const float* position, const float* scale,
                         const float* rotation, const float* sh_base, const float* sh_rest, const float* opacity, int C,
                         int S, int A, int img_h, int img_w, int tile_h, int tile_w, float* packed_params,
                         unsigned* depth_key, unsigned* iota, int* tile_count, int* totals, const float* filter_3d, int antialiased,
-                        void* stream);
-/* The same with normals, ours (DESIGN.md section 1, "Normals"): normal_rec f32[A*S,4] receives (n0, n1, n2, 0) per slot, the
- * view-space normal of the Gaussian's shortest axis (argmin of the raw log-scales), turned to face the camera; slots of chunks
- * at or past the visible count get zeros.  NULL = lgs_project_forward. */
-int lgs_project_forward_normal(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
-                               const float* view_matrix, const float* proj_matrix, const float* position, const float* scale,
-                               const float* rotation, const float* sh_base, const float* sh_rest, const float* opacity, int C,
-                               int S, int A, int img_h, int img_w, int tile_h, int tile_w, float* packed_params,
-                               unsigned* depth_key, unsigned* iota, int* tile_count, int* totals, const float* filter_3d,
-                               int antialiased, float* normal_rec, void* stream);
+                        float* normal_rec, void* stream);
 
 /* duplicate_with_keys (GR/binning.cu:33-110) reading the packed record: offset = inclusive scan of the depth-ordered
  * counts, order = depth-sorted slot ids; keys/vals i32[cap] must be zero-initialised by the caller. */
@@ -341,7 +323,11 @@ int lgs_emit_pairs_u16(const float* packed_params, const int* offset, const unsi
  * (384 for the heaviest; a larger S is refused with an error naming the limit).  0 = the kernels without the terms.
  * depth != 0: depth mode, ours.  packed_grad slot 10 (dL/dz from lgs_rasterize_backward's d_depth) is added to the view-space
  * z gradient: it reaches g_position through the view matrix and d_cam as d view[k][2] += p~_k dz; d proj gets nothing from it.
- * It is exact in both gradient conventions (z depends on neither J nor the SH direction).  0 = slot 10 is not read. */
+ * It is exact in both gradient conventions (z depends on neither J nor the SH direction).  0 = slot 10 is not read.
+ * grad_normal f32[A*S,4] (lgs_rasterize_backward's) or NULL, ours: with dn_c = sigma dn and dn_w = V3x3 dn_c, dn_w is added to
+ * row a (the shortest axis) of the rotation-matrix gradient, so it reaches g_rotation; d_cam gains d view[k][j] += n_w[k] dn_c[j]
+ * for k, j < 3.  Nothing reaches g_position, g_scale or d proj; a and the facing sign sigma are held constant.  The same in both
+ * gradient conventions.  NULL = no normal term, the same kernels as before. */
 int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
                          const float* view_matrix, const float* proj_matrix, const float* position, const float* scale,
                          const float* rotation, const float* opacity, int C, int S, int A, int rest_dim, int img_h,
@@ -349,19 +335,7 @@ int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_id, const i
                          int zero_outputs, float* g_position, float* g_scale, float* g_rotation, float* g_sh_base,
                          float* g_sh_rest, float* g_opacity, float* touched, float* cam_partials, float* d_cam,
                          const float* filter_3d, int antialiased, const float* sh_base, const float* sh_rest, int exact_grad,
-                         int depth, void* stream);
-/* The same with the normal gradient, ours: grad_normal f32[A*S,4] (lgs_rasterize_backward_normal's) or NULL.  With
- * dn_c = sigma dn and dn_w = V3x3 dn_c, dn_w is added to row a (the shortest axis) of the rotation-matrix gradient, so it reaches
- * g_rotation; d_cam gains d view[k][j] += n_w[k] dn_c[j] for k, j < 3.  Nothing reaches g_position, g_scale or d proj; a and the
- * facing sign sigma are held constant.  The same in both gradient conventions.  NULL = lgs_project_backward. */
-int lgs_project_backward_normal(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
-                                const float* view_matrix, const float* proj_matrix, const float* position, const float* scale,
-                                const float* rotation, const float* opacity, int C, int S, int A, int rest_dim, int img_h,
-                                int img_w, int true_sigmoid_grad, const float* packed_grad, const float* grad_inv_scaler,
-                                int zero_outputs, float* g_position, float* g_scale, float* g_rotation, float* g_sh_base,
-                                float* g_sh_rest, float* g_opacity, float* touched, float* cam_partials, float* d_cam,
-                                const float* filter_3d, int antialiased, const float* sh_base, const float* sh_rest, int exact_grad,
-                                int depth, const float* grad_normal, void* stream);
+                         int depth, const float* grad_normal, void* stream);
 
 /* create_viewproj_forward, GR/compact.cu:17-141: view_params f32[V,7] (qw qx qy qz tx ty tz), recp_tan_half_fov_x f32[1] ->
  * view, proj, viewproj f32[V,4,4] (row-vector convention) and frustumplane f32[V,6,4].  One thread per view. */

@@ -52,14 +52,11 @@ SIGNATURES = {
     "lgs_tile_range_u16_dev": [_P, _I, _P, _I, _I, _P, _P],
     "lgs_tile_range_dev": [_P, _I, _P, _I, _I, _P, _P],
     "lgs_pack_params": [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P],
-    "lgs_rasterize_forward_packed": [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P],
-    "lgs_rasterize_forward_packed_normal": [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P,
-                                            _P, _P],
+    "lgs_rasterize_forward_packed": [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P,
+                                     _P, _P],
     "lgs_tile_order": [_P, _I, _I, _P, _P],
     "lgs_rasterize_backward": [_P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I,
-                               _P, _P, _P, _P, _P, _P, _P, _P, _P],
-    "lgs_rasterize_backward_normal": [_P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I,
-                                      _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P],
+                               _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P],
     "lgs_set_staging": [_I],
     "lgs_set_sort_impl": [_I],
     "lgs_set_radix_form": [_I],
@@ -69,14 +66,11 @@ SIGNATURES = {
     "lgs_set_forward_pairs": [_I],
     "lgs_set_err_square_mode": [_I],
     "lgs_set_deterministic": [_I],
-    "lgs_project_forward": [_I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _I, _P],
-    "lgs_project_forward_normal": [_I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _I, _P,
-                                   _P],
+    "lgs_project_forward": [_I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _I, _P,
+                            _P],
     "lgs_emit_pairs": [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P],
     "lgs_project_backward": [_I, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _I,
-                             _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _P, _I, _I, _P],
-    "lgs_project_backward_normal": [_I, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _I,
-                                    _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _P, _I, _I, _P, _P],
+                             _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _P, _I, _I, _P, _P],
     "lgs_create_viewproj_forward": [_P, _P, _I, _I, _I, _F, _F, _P, _P, _P, _P, _P],
     "lgs_create_viewproj_backward": [_P, _P, _P, _P, _P, _I, _I, _I, _F, _F, _P, _P, _P],
     "lgs_adam_update_chunk": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _D, _D, _D, _D, _P],

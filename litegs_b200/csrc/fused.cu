@@ -330,12 +330,12 @@ static int project_forward_normal_max_threads()
 }
 
 // normal_rec f32[A*S,4] or NULL: normal mode, the camera-facing view-space normal of each record (DESIGN.md section 1, "Normals").
-extern "C" int lgs_project_forward_normal(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
-                                          const float* view_matrix, const float* proj_matrix, const float* position,
-                                          const float* scale, const float* rotation, const float* sh_base, const float* sh_rest,
-                                          const float* opacity, int C, int S, int A, int img_h, int img_w, int tile_h, int tile_w,
-                                          float* packed_params, unsigned* depth_key, unsigned* iota, int* tile_count, int* totals,
-                                          const float* filter_3d, int antialiased, float* normal_rec, void* stream)
+extern "C" int lgs_project_forward(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
+                                   const float* view_matrix, const float* proj_matrix, const float* position,
+                                   const float* scale, const float* rotation, const float* sh_base, const float* sh_rest,
+                                   const float* opacity, int C, int S, int A, int img_h, int img_w, int tile_h, int tile_w,
+                                   float* packed_params, unsigned* depth_key, unsigned* iota, int* tile_count, int* totals,
+                                   const float* filter_3d, int antialiased, float* normal_rec, void* stream)
 {
     LGS_REQUIRE(sh_degree >= 0 && sh_degree <= 3, "project_forward: sh_degree %d not in 0..3", sh_degree);
     LGS_REQUIRE(lgs_tile_ok(tile_h, tile_w), "project_forward: tile %dx%d not one of 8x16, 12x16, 16x16, 8x8", tile_h, tile_w);
@@ -367,19 +367,6 @@ extern "C" int lgs_project_forward_normal(int sh_degree, const int64_t* visible_
 #undef PF
     LGS_CHECK_LAUNCH("project_forward_kernel");
     return LGS_OK;
-}
-
-// The form without normals: lgs_project_forward_normal with normal_rec = NULL.
-extern "C" int lgs_project_forward(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
-                                   const float* view_matrix, const float* proj_matrix, const float* position,
-                                   const float* scale, const float* rotation, const float* sh_base, const float* sh_rest,
-                                   const float* opacity, int C, int S, int A, int img_h, int img_w, int tile_h, int tile_w,
-                                   float* packed_params, unsigned* depth_key, unsigned* iota, int* tile_count, int* totals,
-                                   const float* filter_3d, int antialiased, void* stream)
-{
-    return lgs_project_forward_normal(sh_degree, visible_chunk_id, visible_chunks_num, view_matrix, proj_matrix, position, scale,
-                                      rotation, sh_base, sh_rest, opacity, C, S, A, img_h, img_w, tile_h, tile_w, packed_params,
-                                      depth_key, iota, tile_count, totals, filter_3d, antialiased, nullptr, stream);
 }
 
 // (tile+1, splat) emission in depth order from the packed record.    replaces GR/binning.cu:33-110
@@ -915,15 +902,15 @@ static int project_backward_max_threads()
 // this view's gradients are accumulated into them (the multi-view / data-parallel path: no compacted round trip).
 // depth: 1 = the record gradient carries a depth slot (lgs_rasterize_backward was given d_depth), 0 = it does not.
 // grad_normal: f32[A*S,4] normal gradient of lgs_rasterize_backward (normal mode), or NULL = no normal term.
-extern "C" int lgs_project_backward_normal(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
-                                           const float* view_matrix, const float* proj_matrix, const float* position,
-                                           const float* scale, const float* rotation, const float* opacity, int C, int S, int A,
-                                           int rest_dim, int img_h, int img_w, int true_sigmoid_grad, const float* packed_grad,
-                                           const float* grad_inv_scaler, int zero_outputs, float* g_position, float* g_scale,
-                                           float* g_rotation, float* g_sh_base, float* g_sh_rest, float* g_opacity, float* touched,
-                                           float* cam_partials, float* d_cam, const float* filter_3d, int antialiased,
-                                           const float* sh_base, const float* sh_rest, int exact_grad, int depth,
-                                           const float* grad_normal, void* stream)
+extern "C" int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
+                                    const float* view_matrix, const float* proj_matrix, const float* position,
+                                    const float* scale, const float* rotation, const float* opacity, int C, int S, int A,
+                                    int rest_dim, int img_h, int img_w, int true_sigmoid_grad, const float* packed_grad,
+                                    const float* grad_inv_scaler, int zero_outputs, float* g_position, float* g_scale,
+                                    float* g_rotation, float* g_sh_base, float* g_sh_rest, float* g_opacity, float* touched,
+                                    float* cam_partials, float* d_cam, const float* filter_3d, int antialiased,
+                                    const float* sh_base, const float* sh_rest, int exact_grad, int depth,
+                                    const float* grad_normal, void* stream)
 {
     LGS_REQUIRE(sh_degree >= 0 && sh_degree <= 3, "project_backward: sh_degree %d not in 0..3", sh_degree);
     LGS_REQUIRE(rest_dim >= (sh_degree + 1) * (sh_degree + 1) - 1, "project_backward: sh_rest has %d rows, degree %d needs %d", rest_dim,
@@ -986,23 +973,6 @@ extern "C" int lgs_project_backward_normal(int sh_degree, const int64_t* visible
         LGS_CHECK_LAUNCH("camera_grad_sum_kernel");
     }
     return LGS_OK;
-}
-
-// The form without normals: lgs_project_backward_normal with grad_normal = NULL.
-extern "C" int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
-                                    const float* view_matrix, const float* proj_matrix, const float* position,
-                                    const float* scale, const float* rotation, const float* opacity, int C, int S, int A,
-                                    int rest_dim, int img_h, int img_w, int true_sigmoid_grad, const float* packed_grad,
-                                    const float* grad_inv_scaler, int zero_outputs, float* g_position, float* g_scale,
-                                    float* g_rotation, float* g_sh_base, float* g_sh_rest, float* g_opacity, float* touched,
-                                    float* cam_partials, float* d_cam, const float* filter_3d, int antialiased,
-                                    const float* sh_base, const float* sh_rest, int exact_grad, int depth, void* stream)
-{
-    return lgs_project_backward_normal(sh_degree, visible_chunk_id, visible_chunks_num, view_matrix, proj_matrix, position, scale,
-                                       rotation, opacity, C, S, A, rest_dim, img_h, img_w, true_sigmoid_grad, packed_grad,
-                                       grad_inv_scaler, zero_outputs, g_position, g_scale, g_rotation, g_sh_base, g_sh_rest, g_opacity,
-                                       touched, cam_partials, d_cam, filter_3d, antialiased, sh_base, sh_rest, exact_grad, depth,
-                                       nullptr, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -1146,12 +1146,12 @@ extern "C" int lgs_pack_params(const float* ndc, const float* cov2d_inv, const f
 // of the records' view-space z (default kernel only: refused while bulk staging or the pair forward is forced).
 // normal_rec f32[V,N,4] and normal f32[V,3,Hp,Wp], both or neither: the per-pixel normal N = sum w n of the side rows n
 // (lgs_project_forward's normal_rec; default kernel only, as depth).
-extern "C" int lgs_rasterize_forward_packed_normal(const int* sorted_points, const int* start_index, const float* packed_params,
-                                                   const int* specific_tiles, int n_specific, int V, int N, int cap, int img_h,
-                                                   int img_w, int tile_h, int tile_w, int enable_statistic, int clamp_zero, float* img,
-                                                   float* transmittance, short* last_contributor, int* fragment_count,
-                                                   float* fragment_weight, int* tile_work, float* depth, const float* normal_rec,
-                                                   float* normal, void* stream)
+extern "C" int lgs_rasterize_forward_packed(const int* sorted_points, const int* start_index, const float* packed_params,
+                                            const int* specific_tiles, int n_specific, int V, int N, int cap, int img_h,
+                                            int img_w, int tile_h, int tile_w, int enable_statistic, int clamp_zero, float* img,
+                                            float* transmittance, short* last_contributor, int* fragment_count,
+                                            float* fragment_weight, int* tile_work, float* depth, const float* normal_rec,
+                                            float* normal, void* stream)
 {
     LGS_REQUIRE(lgs_tile_ok(tile_h, tile_w), "rasterize_forward: tile %dx%d not one of 8x16, 12x16, 16x16, 8x8", tile_h, tile_w);
     LGS_REQUIRE(V >= 1 && img_h > 0 && img_w > 0, "rasterize_forward: bad sizes V=%d H=%d W=%d", V, img_h, img_w);
@@ -1202,29 +1202,17 @@ extern "C" int lgs_rasterize_forward_packed_normal(const int* sorted_points, con
     return LGS_OK;
 }
 
-// The form without normals: lgs_rasterize_forward_packed_normal with normal_rec = normal = NULL.
-extern "C" int lgs_rasterize_forward_packed(const int* sorted_points, const int* start_index, const float* packed_params,
-                                            const int* specific_tiles, int n_specific, int V, int N, int cap, int img_h, int img_w,
-                                            int tile_h, int tile_w, int enable_statistic, int clamp_zero, float* img,
-                                            float* transmittance, short* last_contributor, int* fragment_count,
-                                            float* fragment_weight, int* tile_work, float* depth, void* stream)
-{
-    return lgs_rasterize_forward_packed_normal(sorted_points, start_index, packed_params, specific_tiles, n_specific, V, N, cap, img_h,
-                                               img_w, tile_h, tile_w, enable_statistic, clamp_zero, img, transmittance, last_contributor,
-                                               fragment_count, fragment_weight, tile_work, depth, nullptr, nullptr, stream);
-}
-
 // packed_grad: f32[V,N,12] scratch, zeroed here.  d_trans may be null.  Outputs as GR/raster.cu:1021-1036.
 // normal_rec f32[V,N,4], d_normal f32[V,3,Hp,Wp] and grad_normal f32[V,N,4] (zeroed here), all or none: dL/dN joins the alpha
 // gradient as three more colour channels with colour n, and grad_normal receives sum_pixels w g_N = dL/dn.
-extern "C" int lgs_rasterize_backward_normal(const int* sorted_points, const int* start_index, const float* packed_params,
-                                             const int* specific_tiles, int n_specific, const float* final_transmittance,
-                                             const short* last_contributor, const float* d_img, const float* d_trans_img,
-                                             const float* clamped_img, const float* grad_inv_scaler, int V, int N, int cap, int img_h,
-                                             int img_w, int tile_h, int tile_w, int enable_statistic, float* packed_grad, float* d_ndc,
-                                             float* d_cov2d_inv, float* d_color, float* d_opacity, float* err_sum,
-                                             float* err_square_sum, const float* d_depth, const float* normal_rec,
-                                             const float* d_normal, float* grad_normal, void* stream)
+extern "C" int lgs_rasterize_backward(const int* sorted_points, const int* start_index, const float* packed_params,
+                                      const int* specific_tiles, int n_specific, const float* final_transmittance,
+                                      const short* last_contributor, const float* d_img, const float* d_trans_img,
+                                      const float* clamped_img, const float* grad_inv_scaler, int V, int N, int cap, int img_h,
+                                      int img_w, int tile_h, int tile_w, int enable_statistic, float* packed_grad, float* d_ndc,
+                                      float* d_cov2d_inv, float* d_color, float* d_opacity, float* err_sum,
+                                      float* err_square_sum, const float* d_depth, const float* normal_rec,
+                                      const float* d_normal, float* grad_normal, void* stream)
 {
     LGS_REQUIRE(lgs_tile_ok(tile_h, tile_w), "rasterize_backward: tile %dx%d not one of 8x16, 12x16, 16x16, 8x8", tile_h, tile_w);
     LGS_REQUIRE(V >= 1 && img_h > 0 && img_w > 0, "rasterize_backward: bad sizes V=%d H=%d W=%d", V, img_h, img_w);
@@ -1315,20 +1303,4 @@ extern "C" int lgs_rasterize_backward_normal(const int* sorted_points, const int
         LGS_CHECK_LAUNCH("unpack_kernel");
     }
     return LGS_OK;
-}
-
-// The form without normals: lgs_rasterize_backward_normal with normal_rec = d_normal = grad_normal = NULL.
-extern "C" int lgs_rasterize_backward(const int* sorted_points, const int* start_index, const float* packed_params,
-                                      const int* specific_tiles, int n_specific, const float* final_transmittance,
-                                      const short* last_contributor, const float* d_img, const float* d_trans_img,
-                                      const float* clamped_img, const float* grad_inv_scaler, int V, int N, int cap, int img_h,
-                                      int img_w, int tile_h,
-                                      int tile_w, int enable_statistic, float* packed_grad, float* d_ndc, float* d_cov2d_inv,
-                                      float* d_color, float* d_opacity, float* err_sum, float* err_square_sum, const float* d_depth,
-                                      void* stream)
-{
-    return lgs_rasterize_backward_normal(sorted_points, start_index, packed_params, specific_tiles, n_specific, final_transmittance,
-                                         last_contributor, d_img, d_trans_img, clamped_img, grad_inv_scaler, V, N, cap, img_h, img_w,
-                                         tile_h, tile_w, enable_statistic, packed_grad, d_ndc, d_cov2d_inv, d_color, d_opacity, err_sum,
-                                         err_square_sum, d_depth, nullptr, nullptr, nullptr, stream);
 }

@@ -396,7 +396,8 @@ def _raster_forward_impl(sorted_points, start_index, packed, specific_tiles, img
     fc = torch.zeros((V, 1, N), dtype=_I32, device=dev)
     fw = torch.zeros((V, 1, N), dtype=_F32, device=dev)
     _lib.call("lgs_rasterize_forward_packed", _ptr(sp), _ptr(si), _ptr(packed), _ptr(tiles), n_sel, V, N, cap, int(img_h), int(img_w),
-              int(th), int(tw), int(bool(enable_statistic)), 0, _ptr(img), _ptr(T), _ptr(last), _ptr(fc), _ptr(fw), None, None, _stream(dev))
+              int(th), int(tw), int(bool(enable_statistic)), 0, _ptr(img), _ptr(T), _ptr(last), _ptr(fc), _ptr(fw), None, None, None, None,
+              _stream(dev))
     return img, T, depth, last, fc, fw
 
 
@@ -455,7 +456,7 @@ def rasterize_backward(sorted_points, start_index, packed_params, specific_tiles
         _lib.call("lgs_rasterize_backward", _ptr(sp), _ptr(si), _ptr(packed), _ptr(tiles), 0 if tiles is None else tiles.shape[1],
                   _ptr(T), _ptr(last), _ptr(g), _ptr(gt), None, _ptr(sc), V, N, cap, int(img_h), int(img_w), int(tilesize_h),
                   int(tilesize_w), int(bool(enable_statistic)), _ptr(pg), _ptr(d_ndc), _ptr(d_cov), _ptr(d_col), _ptr(d_op),
-                  _ptr(e1), _ptr(e2), None, _stream(dev))
+                  _ptr(e1), _ptr(e2), None, None, None, None, _stream(dev))
     return [d_ndc, d_cov, d_col, d_op, e1, e2]
 
 

@@ -23,6 +23,7 @@ from . import _lib
 from .fused import CONFIG, _on, _ptr, _stream
 
 _F32, _I32, _I64, _U8 = torch.float32, torch.int32, torch.int64, torch.uint8
+_KEYS = ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")
 
 _ws_bytes_cache: dict = {}
 LAST_VIEW_SIZES: list = []      # (pairs, depth-key bits) of the views that went through the synchronising forward (capacity probe)
@@ -101,6 +102,45 @@ def check_filter_3d(filter_3d: Optional[torch.Tensor], xyz: torch.Tensor) -> Opt
     return filter_3d.detach()
 
 
+# The four fused stages, each issued from here alone for both view paths (the synchronising functions below and ViewWorkspace).
+# An absent buffer is None, and NULL selects the kernels without that mode.  hw = (H, W), tile = (th, tw).
+
+def _project_forward(st, params, sh_degree, chunk_ids, counters, view, proj, hw, tile, packed, dkey, iota, tcount, filter_3d,
+                     antialiased, normal_rec):
+    C, S = params["xyz"].shape[-2:]
+    cnt = counters.data_ptr()
+    _lib.call("lgs_project_forward", int(sh_degree), _ptr(chunk_ids), ctypes.c_void_p(cnt), _ptr(view), _ptr(proj),
+              *[_ptr(params[k]) for k in _KEYS], C, S, C, *hw, *tile, _ptr(packed), _ptr(dkey), _ptr(iota), _ptr(tcount),
+              ctypes.c_void_p(cnt + 4), _ptr(filter_3d), int(bool(antialiased)), _ptr(normal_rec), st)
+
+
+def _raster_forward(st, hw, tile, sorted_pid, ranges, packed, tiles, stats, clamp_zero, img, T, last, work, depth, normal_rec, normal):
+    fc, fw = stats if stats is not None else (None, None)
+    _lib.call("lgs_rasterize_forward_packed", _ptr(sorted_pid), _ptr(ranges), _ptr(packed), _ptr(tiles),
+              0 if tiles is None else tiles.shape[1], 1, packed.shape[1], sorted_pid.shape[1], *hw, *tile, int(stats is not None),
+              int(bool(clamp_zero)), _ptr(img), _ptr(T), _ptr(last), _ptr(fc), _ptr(fw), _ptr(work), _ptr(depth), _ptr(normal_rec),
+              _ptr(normal), st)
+
+
+def _raster_backward(st, hw, tile, sorted_pid, ranges, packed, tiles, T, last, d_img, d_trans, clamped_img, enable_statistic, pg,
+                     d_depth, normal_rec, d_normal, grad_normal):
+    _lib.call("lgs_rasterize_backward", _ptr(sorted_pid), _ptr(ranges), _ptr(packed), _ptr(tiles), 0 if tiles is None else tiles.shape[1],
+              _ptr(T), _ptr(last), _ptr(d_img), _ptr(d_trans), _ptr(clamped_img), None, 1, packed.shape[1], sorted_pid.shape[1], *hw,
+              *tile, int(bool(enable_statistic)), _ptr(pg), None, None, None, None, None, None, _ptr(d_depth), _ptr(normal_rec),
+              _ptr(d_normal), _ptr(grad_normal), st)
+
+
+def _project_backward(st, params, sh_degree, chunk_ids, counters, view, proj, hw, A, pg, zero_outputs, outs, touched, cam_partials,
+                      d_cam, filter_3d, antialiased, exact_grad, depth, grad_normal):
+    """outs: the six gradient outputs in _KEYS order; depth: whether pg carries the depth slot."""
+    C, S = params["xyz"].shape[-2:]
+    _lib.call("lgs_project_backward", int(sh_degree), _ptr(chunk_ids), ctypes.c_void_p(counters.data_ptr()), _ptr(view), _ptr(proj),
+              _ptr(params["xyz"]), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["opacity"]), C, S, A,
+              params["sh_rest"].shape[0], *hw, int(CONFIG["true_sigmoid_grad"]), _ptr(pg), None, zero_outputs, *[_ptr(t) for t in outs],
+              _ptr(touched), _ptr(cam_partials), _ptr(d_cam), _ptr(filter_3d), int(bool(antialiased)), _ptr(params["sh_0"]),
+              _ptr(params["sh_rest"]), int(bool(exact_grad)), int(bool(depth)), _ptr(grad_normal), st)
+
+
 def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_extend: torch.Tensor, frustumplane: torch.Tensor,
                         view_matrix: torch.Tensor, proj_matrix: torch.Tensor, sh_degree: int, hw: tuple, tile: tuple,
                         enable_statistic: bool = False, specific_tiles: Optional[torch.Tensor] = None, clamp_zero: bool = False,
@@ -131,7 +171,7 @@ def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_exte
     th, tw = int(tile[0]), int(tile[1])
     if view_matrix.shape[0] != 1:
         raise RuntimeError("the fused pipeline renders one view per call (loop over views on the host)")
-    for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity"):
+    for k in _KEYS:
         t = params[k]
         if not (t.is_cuda and t.dtype == _F32 and t.is_contiguous()):
             raise RuntimeError(f"params['{k}'] must be a contiguous float32 CUDA tensor")
@@ -152,12 +192,8 @@ def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_exte
         iota = torch.empty(Nmax, dtype=_I32, device=dev)
         tcount = torch.empty(Nmax, dtype=_I32, device=dev)
         normal_rec = torch.empty((Nmax, 4), dtype=_F32, device=dev) if render_normal else None
-        _lib.call("lgs_project_forward_normal" if render_normal else "lgs_project_forward", int(sh_degree), _ptr(ids),
-                  ctypes.c_void_p(counters.data_ptr()), _ptr(view_matrix),
-                  _ptr(proj_matrix), _ptr(xyz), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["sh_0"]),
-                  _ptr(params["sh_rest"]), _ptr(params["opacity"]), C, S, M, H, W, th, tw, _ptr(packed), _ptr(dkey), _ptr(iota),
-                  _ptr(tcount), ctypes.c_void_p(counters.data_ptr() + 4), _ptr(filter_3d), int(bool(antialiased)),
-                  *((_ptr(normal_rec),) if render_normal else ()), st)
+        _project_forward(st, params, sh_degree, ids, counters, view_matrix, proj_matrix, (H, W), (th, tw), packed, dkey, iota, tcount,
+                         filter_3d, antialiased, normal_rec)
         pinned = _Pinned.get(dev)
         pinned.copy_(counters, non_blocking=True)
         torch.cuda.current_stream(dev).synchronize()
@@ -209,27 +245,20 @@ def render_view_forward(params: dict, cluster_origin: torch.Tensor, cluster_exte
         last = torch.empty((1, 1, Hp, Wp), dtype=torch.int16, device=dev)
         depth = torch.empty((1, 1, Hp, Wp), dtype=_F32, device=dev) if render_depth else None
         normal = torch.empty((1, 3, Hp, Wp), dtype=_F32, device=dev) if render_normal else None
-        n_sel = 0
         if specific_tiles is not None:
-            n_sel = specific_tiles.shape[1]
             img.zero_(); T.fill_(1.0); last.zero_()
             if depth is not None:
                 depth.zero_()
             if normal is not None:
                 normal.zero_()
         stats = None
-        fc = fw = None
-        if enable_statistic:
-            fc = torch.zeros((1, 1, Nmax), dtype=_I32, device=dev)
-            fw = torch.zeros((1, 1, Nmax), dtype=_F32, device=dev)
-            stats = (fc, fw)
+        if enable_statistic:           # (fragment_count, fragment_weight)
+            stats = (torch.zeros((1, 1, Nmax), dtype=_I32, device=dev), torch.zeros((1, 1, Nmax), dtype=_F32, device=dev))
         # per-tile trip count of the backward (deepest list position any pixel consumed) -> heaviest-first tile order
         order = None
         work = torch.empty((1, ntile), dtype=_I32, device=dev) if (CONFIG["tile_order"] and specific_tiles is None and D > 0) else None
-        _lib.call("lgs_rasterize_forward_packed_normal" if render_normal else "lgs_rasterize_forward_packed", _ptr(sorted_pid),
-                  _ptr(ranges), _ptr(packed), _ptr(specific_tiles), n_sel, 1,
-                  Nmax, sorted_pid.shape[1], H, W, th, tw, int(bool(enable_statistic)), int(bool(clamp_zero)), _ptr(img), _ptr(T),
-                  _ptr(last), _ptr(fc), _ptr(fw), _ptr(work), _ptr(depth), *((_ptr(normal_rec), _ptr(normal)) if render_normal else ()), st)
+        _raster_forward(st, (H, W), (th, tw), sorted_pid, ranges, packed, specific_tiles, stats, clamp_zero, img, T, last, work, depth,
+                        normal_rec, normal)
         if work is not None:
             order = torch.empty((1, ntile), dtype=_I32, device=dev)
             _lib.call("lgs_tile_order", _ptr(work), 1, ntile, _ptr(order), st)
@@ -265,11 +294,8 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
     d_normal: dL/dN f32[1,3,H,W] or [1,3,Hp,Wp] of the normal the forward rendered (render_normal=True), or None.  It reaches
     every parameter through the blend weights, and the rotations and the camera through the normals (the shortest axis and the
     facing sign held constant)."""
-    xyz = params["xyz"]
-    dev = xyz.device
-    C, S = xyz.shape[-2:]
-    H, W = state.hw
-    th, tw = state.tile
+    dev = params["xyz"].device
+    S = params["xyz"].shape[-1]
     A = state.n_chunks_visible
     R = params["sh_rest"].shape[0]
     Nmax = state.packed.shape[1]
@@ -291,56 +317,38 @@ def render_view_backward(params: dict, state: ViewState, d_img: torch.Tensor, d_
         raise RuntimeError("camera_grad must be a contiguous float32 CUDA tensor of shape [2,4,4]")
     with _on(dev):
         st = _stream(dev)
-        cam_partials = None if camera_grad is None else torch.empty((max(A, 1), 32), dtype=_F32, device=dev)
-        cam_args = (_ptr(cam_partials), _ptr(camera_grad))
-        exact_args = (_ptr(params["sh_0"]), _ptr(params["sh_rest"]), int(bool(exact_grad)))
         pg = torch.empty((1, Nmax, 12), dtype=_F32, device=dev)
         if specific_tiles is None:
             specific_tiles = state.tile_order          # every tile, longest lists first (None = index order)
-        n_sel = 0 if specific_tiles is None else specific_tiles.shape[1]
         nrm = d_normal is not None
         gn = torch.empty((Nmax, 4), dtype=_F32, device=dev) if nrm else None     # dL/dn per record (zeroed by the raster backward)
-        _lib.call("lgs_rasterize_backward_normal" if nrm else "lgs_rasterize_backward", _ptr(state.sorted_pid), _ptr(state.ranges),
-                  _ptr(state.packed), _ptr(specific_tiles), n_sel,
-                  _ptr(state.T), _ptr(state.last), _ptr(d_img), _ptr(d_trans), _ptr(clamped_img), None, 1, Nmax, state.sorted_pid.shape[1],
-                  H, W, th, tw,
-                  int(bool(enable_statistic)), _ptr(pg), None, None, None, None, None, None, _ptr(d_depth),
-                  *((_ptr(state.normal_rec), _ptr(d_normal), _ptr(gn)) if nrm else ()), st)
-        depth_arg = int(d_depth is not None)            # the record gradient carries the depth slot
-        pb = "lgs_project_backward_normal" if nrm else "lgs_project_backward"
-        pb_tail = (_ptr(gn),) if nrm else ()
+        _raster_backward(st, state.hw, state.tile, state.sorted_pid, state.ranges, state.packed, specific_tiles, state.T, state.last,
+                         d_img, d_trans, clamped_img, enable_statistic, pg, d_depth, state.normal_rec if nrm else None, d_normal, gn)
         if accumulate_into is not None:
-            for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity"):
+            for k in _KEYS:
                 t = accumulate_into[k]
                 if not (t.is_cuda and t.dtype == _F32 and t.is_contiguous() and tuple(t.shape) == tuple(params[k].shape)):
                     raise RuntimeError(f"accumulate_into['{k}'] must be a contiguous float32 CUDA tensor shaped like the parameter")
-            if A > 0:
-                d = accumulate_into
-                _lib.call(pb, state.sh_degree, _ptr(state.chunk_ids), ctypes.c_void_p(state.counters.data_ptr()),
-                          _ptr(state.view), _ptr(state.proj), _ptr(xyz), _ptr(params["scale"]), _ptr(params["rot"]),
-                          _ptr(params["opacity"]), C, S, A, R, H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(pg), None, 2,
-                          _ptr(d["xyz"]), _ptr(d["scale"]), _ptr(d["rot"]), _ptr(d["sh_0"]), _ptr(d["sh_rest"]), _ptr(d["opacity"]),
-                          _ptr(d.get("_touched")), *cam_args, _ptr(state.filter_3d), int(state.antialiased), *exact_args, depth_arg,
-                          *pb_tail, st)   # "_touched": chunk marks for the fused optimizer step
-            elif camera_grad is not None:
-                camera_grad.zero_()
-            return None, pg
-        g_pos = torch.empty((3, A, S), dtype=_F32, device=dev)
-        g_sc = torch.empty((3, A, S), dtype=_F32, device=dev)
-        g_rot = torch.empty((4, A, S), dtype=_F32, device=dev)
-        g_s0 = torch.empty((1, 3, A, S), dtype=_F32, device=dev)
-        K = (state.sh_degree + 1) ** 2
-        g_sr = torch.zeros((R, 3, A, S), dtype=_F32, device=dev) if R > K - 1 else torch.empty((R, 3, A, S), dtype=_F32, device=dev)
-        g_op = torch.empty((1, A, S), dtype=_F32, device=dev)
+            # "_touched": chunk marks for the fused optimizer step
+            grads, outs, touched = None, [accumulate_into[k] for k in _KEYS], accumulate_into.get("_touched")
+        else:
+            g_pos = torch.empty((3, A, S), dtype=_F32, device=dev)
+            g_sc = torch.empty((3, A, S), dtype=_F32, device=dev)
+            g_rot = torch.empty((4, A, S), dtype=_F32, device=dev)
+            g_s0 = torch.empty((1, 3, A, S), dtype=_F32, device=dev)
+            K = (state.sh_degree + 1) ** 2
+            g_sr = torch.zeros((R, 3, A, S), dtype=_F32, device=dev) if R > K - 1 else torch.empty((R, 3, A, S), dtype=_F32, device=dev)
+            g_op = torch.empty((1, A, S), dtype=_F32, device=dev)
+            grads = outs = [g_pos, g_sc, g_rot, g_s0, g_sr, g_op]
+            touched = None
         if A > 0:
-            _lib.call(pb, state.sh_degree, _ptr(state.chunk_ids), ctypes.c_void_p(state.counters.data_ptr()),
-                      _ptr(state.view), _ptr(state.proj), _ptr(xyz), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["opacity"]),
-                      C, S, A, R, H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(pg), None, 0, _ptr(g_pos), _ptr(g_sc), _ptr(g_rot),
-                      _ptr(g_s0), _ptr(g_sr), _ptr(g_op), None, *cam_args, _ptr(state.filter_3d), int(state.antialiased), *exact_args, depth_arg,
-                      *pb_tail, st)
+            cam_partials = None if camera_grad is None else torch.empty((A, 32), dtype=_F32, device=dev)
+            _project_backward(st, params, state.sh_degree, state.chunk_ids, state.counters, state.view, state.proj, state.hw, A, pg,
+                              0 if grads is not None else 2, outs, touched, cam_partials, camera_grad, state.filter_3d, state.antialiased,
+                              exact_grad, d_depth is not None, gn)
         elif camera_grad is not None:
             camera_grad.zero_()
-    return [g_pos, g_sc, g_rot, g_s0, g_sr, g_op], pg
+    return grads, pg
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -421,68 +429,6 @@ class ViewWorkspace:
             setattr(self, name, torch.zeros(shape or (1, 1, self.Hp, self.Wp), dtype=_F32, device=self.dev))
         return getattr(self, name)
 
-    def _forward_kernels(self, params, cluster_origin, cluster_extend, sh_degree, clamp_zero, antialiased, filter_3d, render_depth,
-                         render_normal=False):
-        dev, st = self.dev, _stream(self.dev)
-        H, W = self.hw
-        th, tw = self.tile
-        C, S, N, D = self.C, self.S, self.Nmax, self.cap
-        cnt = self.counters.data_ptr()
-        vp = self.vparams.data_ptr()
-        _lib.call("lgs_frustum_culling_aabb", _ptr(cluster_origin), _ptr(cluster_extend), _ptr(self.cam_planes), C, 1, _ptr(self.vis),
-                  ctypes.c_void_p(cnt), _ptr(self.chunk_ids), st)
-        _lib.call("lgs_project_forward_normal" if render_normal else "lgs_project_forward", int(sh_degree), _ptr(self.chunk_ids),
-                  ctypes.c_void_p(cnt), _ptr(self.cam_view), _ptr(self.cam_proj),
-                  _ptr(params["xyz"]), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["sh_0"]), _ptr(params["sh_rest"]),
-                  _ptr(params["opacity"]), C, S, C, H, W, th, tw, _ptr(self.packed), _ptr(self.dkey), _ptr(self.iota), _ptr(self.tcount),
-                  ctypes.c_void_p(cnt + 4), _ptr(filter_3d), int(antialiased), *((_ptr(self.normal_rec),) if render_normal else ()), st)
-        _lib.call("lgs_view_params", ctypes.c_void_p(cnt), S, D, self.planned_bits, ctypes.c_void_p(vp), _ptr(self.sticky), st)
-        n_dev, d_dev, bias_dev = ctypes.c_void_p(vp), ctypes.c_void_p(vp + 4), ctypes.c_void_p(vp + 8)
-        wsz = ctypes.c_size_t(self.ws_bytes)
-        _lib.call("lgs_sort_pairs_u32_dev", _ptr(self.dkey), _ptr(self.dkey_s), _ptr(self.iota), _ptr(self.order), N, n_dev, bias_dev,
-                  self.planned_bits, _ptr(self.ws), wsz, st)
-        offsets = self.dkey_s           # the sorted keys are dead: their storage receives the scan
-        _lib.call("lgs_scan_gathered_dev", _ptr(self.tcount), _ptr(self.order), N, n_dev, _ptr(offsets), _ptr(self.ws), wsz, st)
-        _lib.call("lgs_emit_pairs_dev", _ptr(self.packed), _ptr(offsets), _ptr(self.order), N, n_dev, D, H, W, th, tw, 16 if self.u16 else 32,
-                  _ptr(self.keys), _ptr(self.vals), d_dev, st)
-        bits = self.ntile.bit_length()
-        _lib.call("lgs_sort_pairs_u16_dev" if self.u16 else "lgs_sort_pairs_u32k_dev", _ptr(self.keys), _ptr(self.keys_s), _ptr(self.vals),
-                  _ptr(self.sorted_pid), D, d_dev, 0, bits, _ptr(self.ws), wsz, st)
-        _lib.call("lgs_tile_range_u16_dev" if self.u16 else "lgs_tile_range_dev", _ptr(self.keys_s), D, d_dev, self.ntile,
-                  int(CONFIG["fix_last_tile"]), _ptr(self.ranges), st)
-        order = CONFIG["tile_order"]
-        _lib.call("lgs_rasterize_forward_packed_normal" if render_normal else "lgs_rasterize_forward_packed", _ptr(self.sorted_pid),
-                  _ptr(self.ranges), _ptr(self.packed), None, 0, 1, N, D, H, W, th, tw,
-                  0, int(bool(clamp_zero)), _ptr(self.img), _ptr(self.T), _ptr(self.last), None, None, _ptr(self.work) if order else None,
-                  _ptr(self.depth) if render_depth else None, *((_ptr(self.normal_rec), _ptr(self.normal)) if render_normal else ()), st)
-        if order:
-            _lib.call("lgs_tile_order", _ptr(self.work), 1, self.ntile, _ptr(self.tile_order), st)
-
-    def _backward_kernels(self, params, sh_degree, accumulate_into, use_clamp, camera_grad, antialiased, filter_3d, exact_grad, depth,
-                          trans, normal=False):
-        st = _stream(self.dev)
-        H, W = self.hw
-        th, tw = self.tile
-        C, S, N, D = self.C, self.S, self.Nmax, self.cap
-        tiles = self.tile_order if CONFIG["tile_order"] else None
-        _lib.call("lgs_rasterize_backward_normal" if normal else "lgs_rasterize_backward", _ptr(self.sorted_pid), _ptr(self.ranges),
-                  _ptr(self.packed), _ptr(tiles),
-                  self.ntile if tiles is not None else 0, _ptr(self.T), _ptr(self.last), _ptr(self.d_img), _ptr(self.d_trans) if trans else None,
-                  _ptr(self.img) if use_clamp else None, None, 1, N, D, H, W, th, tw, 0, _ptr(self.pg), None, None, None, None, None, None,
-                  _ptr(self.d_depth) if depth else None,
-                  *((_ptr(self.normal_rec), _ptr(self.d_normal), _ptr(self.grad_normal)) if normal else ()), st)
-        d = accumulate_into
-        R = params["sh_rest"].shape[0]
-        # A = all chunks: project_backward returns at once for chunks past the (device) visible count
-        _lib.call("lgs_project_backward_normal" if normal else "lgs_project_backward", int(sh_degree), _ptr(self.chunk_ids),
-                  ctypes.c_void_p(self.counters.data_ptr()), _ptr(self.cam_view),
-                  _ptr(self.cam_proj), _ptr(params["xyz"]), _ptr(params["scale"]), _ptr(params["rot"]), _ptr(params["opacity"]), C, S, C, R,
-                  H, W, int(CONFIG["true_sigmoid_grad"]), _ptr(self.pg), None, 2, _ptr(d["xyz"]), _ptr(d["scale"]), _ptr(d["rot"]),
-                  _ptr(d["sh_0"]), _ptr(d["sh_rest"]), _ptr(d["opacity"]), _ptr(d.get("_touched")),
-                  _ptr(self.cam_partials) if camera_grad else None, _ptr(self.d_cam) if camera_grad else None, _ptr(filter_3d),
-                  int(antialiased), _ptr(params["sh_0"]), _ptr(params["sh_rest"]), int(exact_grad), int(depth),
-                  *((_ptr(self.grad_normal),) if normal else ()), st)
-
     def _run(self, kind, sig, fn):
         """Eager the first time a pointer signature is seen, captured into a CUDA graph the second time, replayed afterwards."""
         key = (kind, sig)
@@ -515,6 +461,7 @@ class ViewWorkspace:
         pointer is part of the graph signature: a replayed graph reads whatever the tensor holds, so recomputing it in place
         (scene.filter_3d_device(..., out=)) needs no new capture."""
         filter_3d = check_filter_3d(filter_3d, params["xyz"])
+        render_depth, render_normal, order = bool(render_depth), bool(render_normal), bool(CONFIG["tile_order"])
         if render_depth:
             self._plane("depth")
         if render_normal:
@@ -523,17 +470,47 @@ class ViewWorkspace:
         self.cam_view.copy_(cam["view"], non_blocking=True)
         self.cam_proj.copy_(cam["proj"], non_blocking=True)
         self.cam_planes.copy_(cam["frustumplane"], non_blocking=True)
-        sig = (tuple(params[k].data_ptr() for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")), cluster_origin.data_ptr(),
-               cluster_extend.data_ptr(), int(sh_degree), bool(clamp_zero), bool(CONFIG["tile_order"]),
-               0 if filter_3d is None else filter_3d.data_ptr(), bool(antialiased))
+
+        def kernels():
+            st = _stream(self.dev)
+            H, W = self.hw
+            th, tw = self.tile
+            N, D = self.Nmax, self.cap
+            cnt, vp = self.counters.data_ptr(), self.vparams.data_ptr()
+            _lib.call("lgs_frustum_culling_aabb", _ptr(cluster_origin), _ptr(cluster_extend), _ptr(self.cam_planes), self.C, 1,
+                      _ptr(self.vis), ctypes.c_void_p(cnt), _ptr(self.chunk_ids), st)
+            _project_forward(st, params, sh_degree, self.chunk_ids, self.counters, self.cam_view, self.cam_proj, self.hw, self.tile,
+                             self.packed, self.dkey, self.iota, self.tcount, filter_3d, antialiased,
+                             self.normal_rec if render_normal else None)
+            _lib.call("lgs_view_params", ctypes.c_void_p(cnt), self.S, D, self.planned_bits, ctypes.c_void_p(vp), _ptr(self.sticky), st)
+            n_dev, d_dev, bias_dev = ctypes.c_void_p(vp), ctypes.c_void_p(vp + 4), ctypes.c_void_p(vp + 8)
+            wsz = ctypes.c_size_t(self.ws_bytes)
+            _lib.call("lgs_sort_pairs_u32_dev", _ptr(self.dkey), _ptr(self.dkey_s), _ptr(self.iota), _ptr(self.order), N, n_dev, bias_dev,
+                      self.planned_bits, _ptr(self.ws), wsz, st)
+            offsets = self.dkey_s           # the sorted keys are dead: their storage receives the scan
+            _lib.call("lgs_scan_gathered_dev", _ptr(self.tcount), _ptr(self.order), N, n_dev, _ptr(offsets), _ptr(self.ws), wsz, st)
+            _lib.call("lgs_emit_pairs_dev", _ptr(self.packed), _ptr(offsets), _ptr(self.order), N, n_dev, D, H, W, th, tw,
+                      16 if self.u16 else 32, _ptr(self.keys), _ptr(self.vals), d_dev, st)
+            bits = self.ntile.bit_length()
+            _lib.call("lgs_sort_pairs_u16_dev" if self.u16 else "lgs_sort_pairs_u32k_dev", _ptr(self.keys), _ptr(self.keys_s),
+                      _ptr(self.vals), _ptr(self.sorted_pid), D, d_dev, 0, bits, _ptr(self.ws), wsz, st)
+            _lib.call("lgs_tile_range_u16_dev" if self.u16 else "lgs_tile_range_dev", _ptr(self.keys_s), D, d_dev, self.ntile,
+                      int(CONFIG["fix_last_tile"]), _ptr(self.ranges), st)
+            _raster_forward(st, self.hw, self.tile, self.sorted_pid, self.ranges, self.packed, None, None, clamp_zero, self.img, self.T,
+                            self.last, self.work if order else None, self.depth if render_depth else None,
+                            self.normal_rec if render_normal else None, self.normal if render_normal else None)
+            if order:
+                _lib.call("lgs_tile_order", _ptr(self.work), 1, self.ntile, _ptr(self.tile_order), st)
+
+        sig = (tuple(params[k].data_ptr() for k in _KEYS), cluster_origin.data_ptr(), cluster_extend.data_ptr(), int(sh_degree),
+               bool(clamp_zero), order, 0 if filter_3d is None else filter_3d.data_ptr(), bool(antialiased))
         if render_depth:
             sig += ("depth",)
         if render_normal:
             sig += ("normal",)
-        self._run("fwd", sig, lambda: self._forward_kernels(params, cluster_origin, cluster_extend, sh_degree, clamp_zero, antialiased,
-                                                            filter_3d, bool(render_depth), bool(render_normal)))
-        self.rendered_depth = bool(render_depth)
-        self.rendered_normal = bool(render_normal)
+        self._run("fwd", sig, kernels)
+        self.rendered_depth = render_depth
+        self.rendered_normal = render_normal
         self.views_done += 1
         return self.img
 
@@ -550,42 +527,45 @@ class ViewWorkspace:
         filter_3d = check_filter_3d(filter_3d, params["xyz"])
         if camera_grad is not None and not (camera_grad.is_cuda and camera_grad.dtype == _F32 and tuple(camera_grad.shape) == (2, 4, 4)):
             raise RuntimeError("camera_grad must be a float32 CUDA tensor of shape [2,4,4]")
-        H, W = self.hw
-        if d_img.shape[-2:] == (self.Hp, self.Wp):
-            self.d_img.copy_(d_img, non_blocking=True)
-        else:
-            if self.Hp != H or self.Wp != W:
-                self.d_img.zero_()
-            self.d_img[..., :H, :W].copy_(d_img, non_blocking=True)
         if d_depth is not None and not self.rendered_depth:
             raise RuntimeError("d_depth is given, but the last forward on this workspace did not render depth (render_depth=False)")
         if d_normal is not None and not self.rendered_normal:
             raise RuntimeError("d_normal is given, but the last forward on this workspace did not render normals (render_normal=False)")
-        if d_normal is not None:
+        cam, dep, trans, nrm = camera_grad is not None, d_depth is not None, d_trans is not None, d_normal is not None
+        tiled = bool(CONFIG["tile_order"])
+        if nrm:
             self._plane("grad_normal", (self.Nmax, 4))
-        for name, g in (("d_depth", d_depth), ("d_trans", d_trans), ("d_normal", d_normal)):
+        H, W = self.hw
+        for name, g, c in (("d_img", d_img, 3), ("d_depth", d_depth, 1), ("d_trans", d_trans, 1), ("d_normal", d_normal, 3)):
             if g is None:
                 continue
-            plane = self._plane(name, (1, 3, self.Hp, self.Wp) if name == "d_normal" else None)
+            plane = self._plane(name, (1, c, self.Hp, self.Wp))
             if g.shape[-2:] == (self.Hp, self.Wp):
                 plane.copy_(g, non_blocking=True)
             else:
                 if self.Hp != H or self.Wp != W:
                     plane.zero_()
                 plane[..., :H, :W].copy_(g, non_blocking=True)
-        sig = (tuple(params[k].data_ptr() for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")),
-               tuple(accumulate_into[k].data_ptr() for k in ("xyz", "scale", "rot", "sh_0", "sh_rest", "opacity")),
+
+        def kernels():
+            st = _stream(self.dev)
+            _raster_backward(st, self.hw, self.tile, self.sorted_pid, self.ranges, self.packed, self.tile_order if tiled else None, self.T,
+                             self.last, self.d_img, self.d_trans if trans else None, self.img if use_clamp else None, False, self.pg,
+                             self.d_depth if dep else None, self.normal_rec if nrm else None, self.d_normal if nrm else None,
+                             self.grad_normal if nrm else None)
+            # A = all chunks: project_backward returns at once for chunks past the (device) visible count
+            _project_backward(st, params, sh_degree, self.chunk_ids, self.counters, self.cam_view, self.cam_proj, self.hw, self.C, self.pg,
+                              2, [accumulate_into[k] for k in _KEYS], accumulate_into.get("_touched"), self.cam_partials if cam else None,
+                              self.d_cam if cam else None, filter_3d, antialiased, exact_grad, dep, self.grad_normal if nrm else None)
+
+        sig = (tuple(params[k].data_ptr() for k in _KEYS), tuple(accumulate_into[k].data_ptr() for k in _KEYS),
                0 if accumulate_into.get("_touched") is None else accumulate_into["_touched"].data_ptr(), int(sh_degree), bool(use_clamp),
-               bool(CONFIG["tile_order"]), bool(antialiased), 0 if filter_3d is None else filter_3d.data_ptr(), bool(exact_grad),
-               camera_grad is not None)
-        if d_depth is not None or d_trans is not None:
-            sig += (("depth", d_depth is not None, d_trans is not None),)
-        if d_normal is not None:
+               tiled, bool(antialiased), 0 if filter_3d is None else filter_3d.data_ptr(), bool(exact_grad), cam)
+        if dep or trans:
+            sig += (("depth", dep, trans),)
+        if nrm:
             sig += ("normal",)
-        cam = camera_grad is not None
-        self._run("bwd", sig, lambda: self._backward_kernels(params, sh_degree, accumulate_into, use_clamp, cam, antialiased, filter_3d,
-                                                             bool(exact_grad), d_depth is not None, d_trans is not None,
-                                                             d_normal is not None))
+        self._run("bwd", sig, kernels)
         if cam:
             camera_grad.copy_(self.d_cam, non_blocking=True)
 

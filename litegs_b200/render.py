@@ -10,6 +10,7 @@ from __future__ import annotations
 import copy
 import math
 import os
+from collections import namedtuple
 from typing import Optional
 
 import torch
@@ -23,6 +24,15 @@ from .statistics import StatisticsHelperInst
 def uncluster(*tensors):
     """[..., chunks, chunk_size] -> [..., chunks*chunk_size] views (reference scene/cluster.py:24-28)."""
     return tuple(t.reshape(*t.shape[:-2], t.shape[-2] * t.shape[-1]) for t in tensors)
+
+
+_Modes = namedtuple("_Modes", "antialiased exact_grad render_depth render_normal")
+
+
+def _modes(pp) -> _Modes:
+    """The fused path's opt-in modes (DESIGN.md section 1), read with getattr so that the reference's own PipelineParams, which
+    has none of them, still works (absent = off)."""
+    return _Modes(*(bool(getattr(pp, f, False)) for f in _Modes._fields))
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -72,18 +82,13 @@ def render(view_matrix, proj_matrix, xyz, scale, rot, color, opacity,
     """Projection -> binning -> rasterisation; returns (img, transmittance, depth, normal, primitive_visible)
     as render/__init__.py:50-94.  The antialiased, exact gradient, depth and normal modes exist on the fused path only (render_view,
     render_views)."""
-    if getattr(pp, "antialiased", False):
-        raise RuntimeError("pp.antialiased is set, but the op-by-op render() has no antialiased mode and would draw every splat "
-                           "without its opacity compensation; render through render_view or render_views instead")
-    if getattr(pp, "exact_grad", False):
-        raise RuntimeError("pp.exact_grad is set, but the op-by-op render() has no exact gradient mode and would return position "
-                           "gradients with J and the SH direction held constant; render through render_view or render_views instead")
-    if getattr(pp, "render_depth", False):
-        raise RuntimeError("pp.render_depth is set, but the op-by-op render() has no depth mode (its depth slot keeps the reference's "
-                           "enable_depth contract); render through render_view or render_views instead")
-    if getattr(pp, "render_normal", False):
-        raise RuntimeError("pp.render_normal is set, but the op-by-op render() has no normal mode (its normal slot stays None); "
-                           "render through render_view or render_views instead")
+    why = {"antialiased": "has no antialiased mode and would draw every splat without its opacity compensation",
+           "exact_grad": "has no exact gradient mode and would return position gradients with J and the SH direction held constant",
+           "render_depth": "has no depth mode (its depth slot keeps the reference's enable_depth contract)",
+           "render_normal": "has no normal mode (its normal slot stays None)"}
+    for flag, on in _modes(pp)._asdict().items():
+        if on:
+            raise RuntimeError(f"pp.{flag} is set, but the op-by-op render() {why[flag]}; render through render_view or render_views instead")
     nvtx.range_push("Proj")
     view_pos, ndc_pos = wrapper.MVPTransform.apply(xyz, view_matrix, proj_matrix, valid_length)
     transform_matrix = wrapper.CreateTransformMatrix.call_fused(scale, rot, valid_length)
@@ -144,23 +149,22 @@ def _feed_statistics(state, stats, packed_grad, tile):
 class _RenderViewFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, xyz, scale, rot, sh_0, sh_rest, opacity, cluster_origin, cluster_extend, frustumplane,
-                view_matrix, proj_matrix, sh_degree, H, W, th, tw, sparse_grad, enable_transmitance, accumulate_into, antialiased,
-                filter_3d, exact_grad, render_depth, render_normal):
+                view_matrix, proj_matrix, sh_degree, hw, tile, sparse_grad, enable_transmitance, accumulate_into, filter_3d, modes):
         params = dict(xyz=xyz, scale=scale, rot=rot, sh_0=sh_0, sh_rest=sh_rest, opacity=opacity)
         stat = bool(StatisticsHelperInst.bStart)
         ctx.set_materialize_grads(False)       # an unused transmittance output must not cost a zero-filled gradient image
         # the kernel writes clamp(c,0,1) directly (render/__init__.py:87 does it as a separate pass) ...
         img, state, stats = pipeline.render_view_forward(params, cluster_origin, cluster_extend, frustumplane, view_matrix,
-                                                         proj_matrix, sh_degree, (H, W), (th, tw), enable_statistic=stat, clamp_zero=True,
-                                                         antialiased=antialiased, filter_3d=filter_3d, render_depth=render_depth,
-                                                         render_normal=render_normal)
+                                                         proj_matrix, sh_degree, hw, tile, enable_statistic=stat, clamp_zero=True,
+                                                         antialiased=modes.antialiased, filter_3d=filter_3d,
+                                                         render_depth=modes.render_depth, render_normal=modes.render_normal)
         ctx.state = state
         ctx.stats = stats
         ctx.stat = stat
         ctx.sparse = bool(sparse_grad)
         ctx.trans = bool(enable_transmitance)
         ctx.accumulate_into = accumulate_into
-        ctx.exact_grad = bool(exact_grad)           # backward only: the forward does not depend on it
+        ctx.exact_grad = modes.exact_grad           # backward only: the forward does not depend on it
         ctx.save_for_backward(xyz, scale, rot, sh_0, sh_rest, opacity, img)
         ctx.mark_non_differentiable(state.last)
         return img, state.T, state.last, state.depth, state.normal   # depth, normal: None unless render_depth, render_normal
@@ -183,21 +187,18 @@ class _RenderViewFn(torch.autograd.Function):
                                                   exact_grad=ctx.exact_grad, d_depth=g_depth, d_normal=g_normal)
         if ctx.stat:
             _feed_statistics(state, ctx.stats, pg, state.tile)
-        g_view = g_proj = None
+        out = [None] * len(ctx.needs_input_grad)           # one slot per input of forward
         if cam is not None:
-            g_view = cam[0].reshape(state.view.shape) if ctx.needs_input_grad[9] else None
-            g_proj = cam[1].reshape(state.proj.shape) if ctx.needs_input_grad[10] else None
-        if grads is None:          # gradients went straight into the caller's dense buffers
-            ctx.state = None
-            return (None,) * 9 + (g_view, g_proj) + (None,) * 13
-        C, S = xyz.shape[-2:]
-        ids = state.chunk_ids[: state.n_chunks_visible]
-        out = []
-        for g in grads:
-            ct = CompactedTensor((*g.shape[:-2], C, S), ids, g)
-            out.append(ct if ctx.sparse else ct.to_dense())
+            out[9] = cam[0].reshape(state.view.shape) if ctx.needs_input_grad[9] else None
+            out[10] = cam[1].reshape(state.proj.shape) if ctx.needs_input_grad[10] else None
+        if grads is not None:      # None: the gradients went straight into the caller's dense buffers
+            C, S = xyz.shape[-2:]
+            ids = state.chunk_ids[: state.n_chunks_visible]
+            for k, g in enumerate(grads):
+                ct = CompactedTensor((*g.shape[:-2], C, S), ids, g)
+                out[k] = ct if ctx.sparse else ct.to_dense()
         ctx.state = None
-        return (*out, None, None, None, g_view, g_proj, None, None, None, None, None, None, None, None, None, None, None, None, None)
+        return tuple(out)
 
 
 def render_view(cluster_origin, cluster_extend, frustumplane, view_matrix, proj_matrix,
@@ -225,11 +226,8 @@ def render_view(cluster_origin, cluster_extend, frustumplane, view_matrix, proj_
     H, W = int(output_shape[0]), int(output_shape[1])
     th, tw = int(pp.tile_size[0]), int(pp.tile_size[1])
     img, T, last, depth, normal = _RenderViewFn.apply(xyz, scale, rot, sh_0, sh_rest, opacity, cluster_origin, cluster_extend,
-                                                      frustumplane, view_matrix, proj_matrix, int(actived_sh_degree), H, W, th, tw,
-                                                      pp.sparse_grad, pp.enable_transmitance, accumulate_into,
-                                                      bool(getattr(pp, "antialiased", False)), filter_3d,
-                                                      bool(getattr(pp, "exact_grad", False)), bool(getattr(pp, "render_depth", False)),
-                                                      bool(getattr(pp, "render_normal", False)))
+                                                      frustumplane, view_matrix, proj_matrix, int(actived_sh_degree), (H, W), (th, tw),
+                                                      pp.sparse_grad, pp.enable_transmitance, accumulate_into, filter_3d, _modes(pp))
     img = img[..., :H, :W]          # already clamped to [0,1] by the kernel
     trans = T[..., :H, :W] if pp.enable_transmitance else None
     return (img, trans, None if depth is None else depth[..., :H, :W], None if normal is None else normal[..., :H, :W], last)
@@ -293,15 +291,31 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
     losses = []
     H, W = int(output_shape[0]), int(output_shape[1])
     th, tw = int(pp.tile_size[0]), int(pp.tile_size[1])
-    aa = bool(getattr(pp, "antialiased", False))
-    exact = bool(getattr(pp, "exact_grad", False))
-    dep = bool(getattr(pp, "render_depth", False))
-    nrm = bool(getattr(pp, "render_normal", False))
+    aa, exact, dep, nrm = _modes(pp)
     direct = loss_and_grad_fn is not None or _DIRECT_VIEWS
     if direct:
         params = dict(xyz=xyz.detach(), scale=scale.detach(), rot=rot.detach(), sh_0=sh_0.detach(), sh_rest=sh_rest.detach(),
                       opacity=opacity.detach())
         stat = bool(StatisticsHelperInst.bStart)
+
+    def callback_args(img, depth, trans, normal):
+        """What the callbacks take after i: the image, then (depth, trans) with depth or normals on, then the normal with normals on."""
+        return [img] + ([depth, trans] if dep or nrm else []) + ([normal] if nrm else [])
+
+    def loss_and_grads(i, img_p, depth_p, T_p, normal_p):
+        """Either callback on view i's padded outputs -> (loss, d_img, d_depth, d_trans, d_normal); every gradient but d_img may be
+        None.  Autograd runs through the caller's loss only, never through the render kernels."""
+        ins = [None if t is None else t[..., :H, :W] for t in callback_args(img_p, depth_p, T_p, normal_p)]
+        if loss_and_grad_fn is not None:
+            out = tuple(loss_and_grad_fn(i, *ins))
+        else:
+            leaves = [None if t is None else t.detach().requires_grad_(True) for t in ins]
+            out = loss_fn(i, *leaves)
+            if not isinstance(out, tuple):
+                gs = iter(torch.autograd.grad(out, [t for t in leaves if t is not None], allow_unused=True))
+                out = (out, *(None if t is None else next(gs) for t in leaves))
+        loss, d_img, d_depth, d_trans, d_normal = out + (None,) * (5 - len(out))
+        return loss, (torch.zeros_like(ins[0]) if d_img is None else d_img), d_depth, d_trans, d_normal
 
     def one_direct(i, wait_ev):
         cam = camera_fn(i)
@@ -309,18 +323,7 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
                                                            cam["proj"], int(actived_sh_degree), (H, W), (th, tw), enable_statistic=stat,
                                                            clamp_zero=True, antialiased=aa, filter_3d=filter_3d, render_depth=dep,
                                                            render_normal=nrm)
-        d_depth = d_trans = d_normal = None
-        if dep or nrm:
-            loss, d_img, d_depth, d_trans, d_normal = _ext_loss(i, img_p, state.depth, state.T, state.normal)
-        elif loss_and_grad_fn is not None:
-            loss, d_img = loss_and_grad_fn(i, img_p[..., :H, :W])
-        else:                          # autograd only through the user's loss, never through the render kernels
-            leaf = img_p[..., :H, :W].detach().requires_grad_(True)
-            loss = loss_fn(i, leaf)
-            if isinstance(loss, tuple):
-                loss, d_img = loss
-            else:
-                (d_img,) = torch.autograd.grad(loss, leaf)
+        loss, d_img, d_depth, d_trans, d_normal = loss_and_grads(i, img_p, state.depth, state.T, state.normal)
         if d_img.shape[-2:] != img_p.shape[-2:]:                        # image padded to whole tiles: pad the gradient with zeros
             d_img = torch.nn.functional.pad(d_img, (0, img_p.shape[-1] - W, 0, img_p.shape[-2] - H))
         if d_trans is not None:
@@ -343,22 +346,17 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
         if (dep or nrm) and not pp.enable_transmitance:    # the depth / normal callbacks take the transmittance
             pp_i = copy.copy(pp)
             pp_i.enable_transmitance = True
-        out = render_view(cluster_origin, cluster_extend, cam["frustumplane"], view, proj, xyz, scale, rot, sh_0, sh_rest,
-                          opacity, actived_sh_degree, output_shape, pp_i, accumulate_into=accumulate_into, filter_3d=filter_3d)
-        img = out[0]
-        if nrm:
-            loss = loss_fn(i, img, out[2], out[1], out[3])
-        else:
-            loss = loss_fn(i, img, out[2], out[1]) if dep else loss_fn(i, img)
+        img, trans, depth, normal, _ = render_view(cluster_origin, cluster_extend, cam["frustumplane"], view, proj, xyz, scale, rot,
+                                                   sh_0, sh_rest, opacity, actived_sh_degree, output_shape, pp_i,
+                                                   accumulate_into=accumulate_into, filter_3d=filter_3d)
+        ins = callback_args(img, depth, trans, normal)
+        loss = loss_fn(i, *ins)
         if wait_ev is not None:          # the previous view's accumulate (other stream) must have landed
             torch.cuda.current_stream(dev).wait_event(wait_ev)
-        if isinstance(loss, tuple) and (dep or nrm):
+        if isinstance(loss, tuple):
             loss, *gs = loss
-            pairs = [(t, g) for t, g in zip((img, out[2], out[1], out[3]), gs) if t is not None and g is not None]
+            pairs = [(t, g) for t, g in zip(ins, gs) if t is not None and g is not None]
             torch.autograd.backward([t for t, _ in pairs], [g for _, g in pairs])
-        elif isinstance(loss, tuple):
-            loss, d_img = loss
-            img.backward(d_img)
         else:
             loss.backward()
         if camera_grads is not None:
@@ -375,47 +373,17 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
             slots = None
     probe = {"pairs": 0, "bits": 1} if (slots is not None and slots.ws is None) else None
 
-    def one_ws(i, wait_ev, ws):
+    def one_ws(i, wait_ev):
+        ws = slots.ws[i % max(1, n_streams)]
         cam = camera_fn(i)
         img_p = ws.forward(params, cluster_origin, cluster_extend, cam, int(actived_sh_degree), clamp_zero=True, antialiased=aa,
                            filter_3d=filter_3d, render_depth=dep, render_normal=nrm)
-        d_depth = d_trans = d_normal = None
-        if dep or nrm:
-            loss, d_img, d_depth, d_trans, d_normal = _ext_loss(i, img_p, ws.depth if dep else None, ws.T, ws.normal if nrm else None)
-        elif loss_and_grad_fn is not None:
-            loss, d_img = loss_and_grad_fn(i, img_p[..., :H, :W])
-        else:
-            leaf = img_p[..., :H, :W].detach().requires_grad_(True)
-            loss = loss_fn(i, leaf)
-            if isinstance(loss, tuple):
-                loss, d_img = loss
-            else:
-                (d_img,) = torch.autograd.grad(loss, leaf)
+        loss, d_img, d_depth, d_trans, d_normal = loss_and_grads(i, img_p, ws.depth if dep else None, ws.T, ws.normal)
         if wait_ev is not None:
             torch.cuda.current_stream(dev).wait_event(wait_ev)
         ws.backward(params, d_img, int(actived_sh_degree), accumulate_into, use_clamp=True, camera_grad=slot(i), antialiased=aa,
                     filter_3d=filter_3d, exact_grad=exact, d_depth=d_depth, d_trans=d_trans, d_normal=d_normal)
         losses.append(loss.detach())
-
-    def _ext_loss(i, img_p, depth_p, T_p, normal_p):
-        """The depth / normal-mode callbacks on the padded outputs of one view -> (loss, d_img, d_depth, d_trans, d_normal); each
-        gradient but d_img may be None.  depth_p is None unless render_depth; the normal is passed (appended) only in normal mode."""
-        ins = [img_p[..., :H, :W], None if depth_p is None else depth_p[..., :H, :W], T_p[..., :H, :W]]
-        if nrm:
-            ins.append(normal_p[..., :H, :W])
-        if loss_and_grad_fn is not None:
-            out = tuple(loss_and_grad_fn(i, *ins))
-        else:
-            leaves = [None if t is None else t.detach().requires_grad_(True) for t in ins]
-            loss = loss_fn(i, *leaves)
-            if isinstance(loss, tuple):
-                out = tuple(loss)
-            else:
-                gs = iter(torch.autograd.grad(loss, [t for t in leaves if t is not None], allow_unused=True))
-                out = (loss, *(None if t is None else next(gs) for t in leaves))
-        loss, d_img, d_depth, d_trans = out[:4]
-        d_normal = out[4] if nrm else None
-        return loss, (torch.zeros_like(ins[0]) if d_img is None else d_img), d_depth, d_trans, d_normal
 
     def one_probe(i, wait_ev):
         n0 = len(pipeline.LAST_VIEW_SIZES)
@@ -424,20 +392,18 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
             probe["pairs"] = max(probe["pairs"], pairs); probe["bits"] = max(probe["bits"], bits)
         del pipeline.LAST_VIEW_SIZES[:]
 
-    if slots is not None and slots.ws is not None:
+    use_ws = slots is not None and slots.ws is not None
+    if use_ws:
         slots.check()
-        one = None
+        one = one_ws
     elif probe is not None:
         one = one_probe
     else:
         one = one_direct if direct else one_autograd
     if n_streams <= 1:
         for i in range(n_views):
-            if one is None:
-                one_ws(i, None, slots.ws[0])
-            else:
-                one(i, None)
-        if one is None:
+            one(i, None)
+        if use_ws:
             slots.ws[0].post_flags()
         elif probe is not None:
             slots.size(probe["pairs"], probe["bits"])
@@ -450,13 +416,10 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
     for i in range(n_views):
         s = side[i % n_streams]
         with torch.cuda.stream(s):
-            if one is None:
-                one_ws(i, prev, slots.ws[i % n_streams])
-            else:
-                one(i, prev)
+            one(i, prev)
             prev = torch.cuda.Event()
             prev.record(s)
-    if one is None:
+    if use_ws:
         for k, s in enumerate(side[: min(n_streams, n_views)]):
             with torch.cuda.stream(s):
                 slots.ws[k].post_flags()

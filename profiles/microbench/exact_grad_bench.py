@@ -54,7 +54,7 @@ def main(n_views=8, reps=20):
             _lib.call("lgs_project_backward", 3, _ptr(st.chunk_ids), ctypes.c_void_p(st.counters.data_ptr()), _ptr(st.view), _ptr(st.proj),
                       _ptr(P["xyz"]), _ptr(P["scale"]), _ptr(P["rot"]), _ptr(P["opacity"]), C, S, st.n_chunks_visible, R, H, W,
                       int(CONFIG["true_sigmoid_grad"]), _ptr(pg), None, 2, *(_ptr(acc[k]) for k in KEYS), None, None, None, None, 0,
-                      _ptr(P["sh_0"]), _ptr(P["sh_rest"]), int(exact), 0, st_)
+                      _ptr(P["sh_0"]), _ptr(P["sh_rest"]), int(exact), 0, None, st_)
 
     arms = {("backward", e, c): (lambda e=e, c=c: backward(e, c)) for e in (False, True) for c in (False, True)}
     arms.update({("project", e, False): (lambda e=e: project(e)) for e in (False, True)})

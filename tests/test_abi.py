@@ -34,7 +34,7 @@ def test_library_exports_every_declared_symbol():
     for name, n in decls.items():
         if name in _lib.SIGNATURES:
             assert len(_lib.SIGNATURES[name]) == n, name
-    assert lib.lgs_abi_version() == 2
+    assert lib.lgs_abi_version() == 3
 
 
 def test_library_contains_sm90a_code_and_bulk_copy():

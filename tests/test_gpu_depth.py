@@ -96,7 +96,7 @@ def test_weights_sum_to_one_minus_T(cuda):
     img2, last = torch.empty_like(img), torch.empty_like(st.last)
     _lib.call("lgs_rasterize_forward_packed", pipeline._ptr(st.sorted_pid), pipeline._ptr(st.ranges), pipeline._ptr(packed), None, 0, 1,
               packed.shape[1], st.sorted_pid.shape[1], hw[0], hw[1], tile[0], tile[1], 0, 1, pipeline._ptr(img2), pipeline._ptr(T),
-              pipeline._ptr(last), None, None, None, pipeline._ptr(sw), pipeline._stream(cuda))
+              pipeline._ptr(last), None, None, None, pipeline._ptr(sw), None, None, pipeline._stream(cuda))
     torch.cuda.synchronize()
     assert torch.equal(T, st.T) and torch.equal(img2, img)
     err = (sw - (1 - T)).abs().max().item()
@@ -321,7 +321,7 @@ def _project(cuda, P, st, pg, depth):
     p = pipeline._ptr
     _lib.call("lgs_project_backward", st.sh_degree, p(st.chunk_ids), p(st.counters), p(st.view), p(st.proj), p(P["xyz"]), p(P["scale"]),
               p(P["rot"]), p(P["opacity"]), C, S, A, R, *st.hw, 0, p(pg), None, 1, *(p(t) for t in out), None, p(part), p(cam), None, 0,
-              p(P["sh_0"]), p(P["sh_rest"]), 0, int(depth), pipeline._stream(cuda))
+              p(P["sh_0"]), p(P["sh_rest"]), 0, int(depth), None, pipeline._stream(cuda))
     torch.cuda.synchronize()
     return out, cam
 
