@@ -7,6 +7,7 @@
 - camera_backward is the camera gradient of one view (DESIGN.md section 1): per-Gaussian contributions through the NDC mean and
   through the V3x3 factor of M = T.V3x3.J, with J and the SH direction held constant, summed over the Gaussians.  It reads the
   intermediates oracle.render_forward_backward returns, so it is the same computation the oracle's position gradient uses.
+  tests/fused_oracle.py adds the modes' terms to it.
 """
 import numpy as np
 
@@ -82,6 +83,18 @@ def create_viewproj_backward(view_grad, proj_grad, viewproj_grad, view_params, r
     return gvp_out, np.array([fov], dt)
 
 
+def sigma_chain(inter, view, G, dt):
+    """The Sigma2 path of a d cov2d G [2,2,N] in dtype dt, every Gaussian first: M = T.V3x3.J, dM = 2 M G, dVJ = T^T dM ->
+    (J [N,3,2], dVJ [N,3,2])."""
+    V3 = np.asarray(view, dt).reshape(4, 4)[:3, :3]
+    G = np.moveaxis(np.asarray(G, dt), -1, 0)                                      # [N,2,2]
+    J = np.moveaxis(np.asarray(inter["J"][0], dt), -1, 0)[:, :, :2]                # [N,3,2]
+    T = np.moveaxis(np.asarray(inter["T"], dt), -1, 0)                             # [N,3,3]
+    M = np.einsum("nak,nkc->nac", T, np.einsum("ak,nkc->nac", V3, J))
+    dM = 2 * np.einsum("nac,ncd->nad", M, G)
+    return J, np.einsum("nak,nac->nkc", T, dM)
+
+
 def camera_backward(params, out, camera, img_hw):
     """Camera gradient of one view from oracle.render_forward_backward's output -> (d_view [4,4], d_proj [4,4]).
 
@@ -94,7 +107,6 @@ def camera_backward(params, out, camera, img_hw):
     N = inter["view_pos"].shape[2]
     pt = np.ones((N, 4), dt)
     pt[:, :3] = params["xyz"][:, ids, :].reshape(3, -1).T.astype(dt)
-    Vm = np.asarray(camera["view"], dt).reshape(4, 4)
     P = np.asarray(camera["proj"], dt).reshape(4, 4)
     v = inter["view_pos"][0].T                                                     # [N,4]
     h = v @ P
@@ -105,15 +117,9 @@ def camera_backward(params, out, camera, img_hw):
     dv = dh @ P.T                                                                  # dv_k = sum_j dh_j P[k][j]
     ndc_view = pt[:, :, None] * dv[:, None, :]
     ndc_proj = v[:, :, None] * dh[:, None, :]
-    # Sigma2 path: G = d cov2d (inverse backward, NaN -> 0), dM = 2 M G, dVJ = T^T dM, dV3 = dVJ J^T
-    Gc = np.nan_to_num(oracle.inv_2x2matrix_backward(inter["inv_cov2d"], out["d_cov"]), nan=0.0)[0]     # [2,2,N]
-    Gc = np.moveaxis(Gc, -1, 0)                                                    # [N,2,2]
-    J = np.moveaxis(inter["J"][0], -1, 0)[:, :, :2]                                # [N,3,2]
-    T = np.moveaxis(inter["T"], -1, 0)                                             # [N,3,3]
-    VJ = np.einsum("ak,nkc->nac", Vm[:3, :3], J)
-    M = np.einsum("nak,nkc->nac", T, VJ)
-    dM = 2 * np.einsum("nac,ncd->nad", M, Gc)
-    dVJ = np.einsum("nak,nac->nkc", T, dM)
+    # Sigma2 path: G = d cov2d (inverse backward, NaN -> 0), dV3 = dVJ J^T
+    G = np.nan_to_num(oracle.inv_2x2matrix_backward(inter["inv_cov2d"], out["d_cov"]), nan=0.0)[0]      # [2,2,N]
+    J, dVJ = sigma_chain(inter, camera["view"], G, dt)
     sigma_view = np.zeros((N, 4, 4), dt)
     sigma_view[:, :3, :3] = np.einsum("nac,nkc->nak", dVJ, J)
     parts = dict(ndc_view=ndc_view, sigma_view=sigma_view, ndc_proj=ndc_proj)

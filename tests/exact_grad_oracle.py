@@ -9,16 +9,10 @@ the default convention drops:
 - through the SH view direction: with d = p - cc, n = 1 / sqrt(|d|^2 + 1e-12) and u = d n, g_u = sum_k w_k d b_k / du with
   w_k = sum_c sh[k][c] dcol_c, and g_d = n (g_u - u (u . g_u)); d xyz += g_d and d cc = -g_d.
 
-``render_forward_backward`` wraps ``filter3d_oracle.render_forward_backward`` and adds both terms to the xyz gradient from the
-intermediates that function returns; ``camera_backward`` extends ``aa_oracle.camera_backward`` (itself
-``camera_oracle.camera_backward`` plus the antialiased term) with them.  With ``exact_grad=False`` both return the existing
-composition unchanged.  The oracle library itself has no such mode.
+tests/fused_oracle.py adds both terms to the xyz gradient and to the camera gradient.  The oracle library itself has no such
+mode.
 """
 import numpy as np
-
-import oracle
-from tests import aa_oracle as aa
-from tests import filter3d_oracle as f3
 
 SH_C0 = 0.28209479177387814
 SH_C1 = 0.4886025119029199
@@ -121,70 +115,3 @@ def direction_backward(deg, p, Vm, sh, dcol):
     w = np.einsum("kcn,cn->kn", sh, dcol)
     gu = sh_basis_grad(deg, u, w)
     return n * (gu - u * (u * gu).sum(axis=0))
-
-
-def _terms(params, out, camera, img_hw, sh_degree):
-    """Per-Gaussian terms of the mode: (dv_J [3,N] view space, d p00 [N], d p11 [N], g_d [3,N], p [3,N]) in fp64."""
-    H, W = img_hw
-    inter = out["inter"]
-    Vm = np.asarray(camera["view"], np.float64).reshape(4, 4)
-    P = np.asarray(camera["proj"], np.float64).reshape(4, 4)
-    ids = out["visible_chunk_id"]
-    p = params["xyz"][:, ids, :].reshape(3, -1).astype(np.float64)
-    N = p.shape[1]
-    # J term: G the whole d cov2d (the antialiased term included), dM = 2 M G, dVJ = T^T dM, dJ = V3^T dVJ
-    Gc = np.nan_to_num(oracle.inv_2x2matrix_backward(inter["inv_cov2d"], out["d_cov"]), nan=0.0)[0] + out["G_aa"]
-    Gc = np.moveaxis(Gc.astype(np.float64), -1, 0)                                 # [N,2,2]
-    J = np.moveaxis(inter["J"][0].astype(np.float64), -1, 0)[:, :, :2]             # [N,3,2]
-    T = np.moveaxis(inter["T"].astype(np.float64), -1, 0)                          # [N,3,3]
-    VJ = np.einsum("ak,nkc->nac", Vm[:3, :3], J)
-    M = np.einsum("nak,nkc->nac", T, VJ)
-    dM = 2 * np.einsum("nac,ncd->nad", M, Gc)
-    dVJ = np.einsum("nak,nac->nkc", T, dM)
-    dJ = np.einsum("ak,nac->nkc", Vm[:3, :3], dVJ)                                 # [N,3,2]
-    v = inter["view_pos"][0, :3].astype(np.float64)
-    dvJ, dp00, dp11 = J_backward(v, P[0, 0], P[1, 1], H, W, dJ[:, 0, 0], dJ[:, 1, 1], dJ[:, 2, 0], dJ[:, 2, 1])
-    # SH direction term
-    gd = np.zeros((3, N))
-    if sh_degree > 0:
-        K = (sh_degree + 1) ** 2
-        sh = np.concatenate([params["sh_0"][:, :, ids, :], params["sh_rest"][:K - 1, :, ids, :]]).reshape(K, 3, N)
-        gd = direction_backward(sh_degree, p, Vm, sh.astype(np.float64), out["d_col"][0].astype(np.float64))
-    return dvJ, dp00, dp11, gd, p
-
-
-def render_forward_backward(params, chunk_aabb, camera, img_hw, tile_hw, sh_degree, d_img_fn, true_sigmoid_grad=False,
-                            antialiased=False, filter_3d=None, exact_grad=False, lists=None, freeze=None):
-    """filter3d_oracle.render_forward_backward; with exact_grad the xyz gradient also carries the J and SH direction terms (added
-    in fp64 and rounded to the gradient's dtype).  Returns its dict, with "exact_terms" (see _terms) when exact_grad."""
-    out = f3.render_forward_backward(params, chunk_aabb, camera, img_hw, tile_hw, sh_degree, d_img_fn, true_sigmoid_grad=true_sigmoid_grad,
-                                     antialiased=antialiased, filter_3d=filter_3d, lists=lists, freeze=freeze)
-    if not exact_grad:
-        return out
-    dvJ, dp00, dp11, gd, p = terms = _terms(params, out, camera, img_hw, sh_degree)
-    Vm = np.asarray(camera["view"], np.float64).reshape(4, 4)
-    gx = out["grads"]["xyz"]
-    extra = (Vm[:3, :3] @ dvJ + gd).reshape(gx.shape)
-    out["grads"] = dict(out["grads"], xyz=(gx.astype(np.float64) + extra).astype(gx.dtype))
-    out["exact_terms"] = terms
-    return out
-
-
-def camera_backward(params, out, camera, img_hw, sh_degree=None, exact_grad=False):
-    """aa_oracle.camera_backward, plus with exact_grad the J and SH direction terms -> (d_view [4,4], d_proj [4,4]).  out is
-    render_forward_backward's dict (with exact_grad it needs sh_degree, or the "exact_terms" that call left in it)."""
-    d_view, d_proj = aa.camera_backward(params, out, camera, img_hw)
-    if not exact_grad:
-        return d_view, d_proj
-    dvJ, dp00, dp11, gd, p = out.get("exact_terms") or _terms(params, out, camera, img_hw, sh_degree)
-    Vm = np.asarray(camera["view"], np.float64).reshape(4, 4)
-    d_view = d_view.astype(np.float64)
-    d_proj = d_proj.astype(np.float64)
-    d_view[:3, :3] += p @ dvJ.T                     # d V[k][j] += p~_k dv_j
-    d_view[3, :3] += dvJ.sum(axis=1)
-    g = gd.sum(axis=1)
-    d_view[3, :3] += Vm[:3, :3].T @ g               # d V[3][k] += sum_m g_d[m] V[m][k]
-    d_view[:3, :3] += np.outer(g, Vm[3, :3])        # d V[m][k] += g_d[m] V[3][k]
-    d_proj[0, 0] += dp00.sum()
-    d_proj[1, 1] += dp11.sum()
-    return d_view, d_proj

@@ -5,17 +5,11 @@ view-space normal of Gaussian i's shortest axis.  That is the oracle's own compo
 keeps the composite below the min(c, 1) clamp, and scaling by 2 is exact.  Both use the same weights, so the backward is the sum
 of the colour backward and the same backward of that normal-as-colour image; its colour gradient is dL/dn (times 1/2), which then
 reaches the rotations (row a of the rotation-matrix gradient) and the camera (d view[k][j] += n_w[k] dn_c[j]).
-
-``render_forward_backward`` runs exact_grad_oracle's composition (and, with render_depth, depth_oracle's stages) with
-``oracle.rasterize_backward`` intercepted for the duration of the call, as depth_oracle does.  The oracle library itself is not
-changed, and with ``render_normal=False`` the call is depth_oracle's.
+tests/fused_oracle.py renders N and adds that backward.  The oracle library itself has no normal mode.
 """
-import contextlib
-
 import numpy as np
 
 import oracle
-from tests import depth_oracle as dp
 
 
 def quat_R(qn):
@@ -72,42 +66,6 @@ def normal_forward(sorted_pid, ranges, ndc, inv_cov2d, opacity, n, H, W, th, tw,
     return img * 2
 
 
-@contextlib.contextmanager
-def _normal_stages(frame_fn, d_normal_fn, rec):
-    backward0 = oracle.rasterize_backward
-
-    def rasterize_backward(sorted_pid, ranges, ndc, inv, color, opacity, tiles, T, last, d_img, d_trans, scaler, H, W, th, tw, **kw):
-        if "frame" in rec:               # depth_oracle's depth-as-colour pass (after the colour pass): nothing to add
-            return backward0(sorted_pid, ranges, ndc, inv, color, opacity, tiles, T, last, d_img, d_trans, scaler, H, W, th, tw, **kw)
-        fr = frame_fn(ndc.dtype)
-        rec["frame"] = fr
-        coln = normal_colour(fr["n"], ndc.dtype)
-        Nimg = normal_forward(sorted_pid, ranges, ndc, inv, opacity, fr["n"], H, W, th, tw, tiles)
-        rec["normal"] = Nimg
-        gn = gt = None
-        if d_normal_fn is not None:
-            gn, gt = d_normal_fn(Nimg[..., :H, :W], T[..., :H, :W])
-        s = 1.0 if scaler is None else float(np.asarray(scaler).reshape(-1)[0])
-        if gt is not None:
-            gt = (dp._pad(np.asarray(gt, T.dtype), T.shape) / s).astype(T.dtype)
-            d_trans = gt if d_trans is None else d_trans + gt
-        out = list(backward0(sorted_pid, ranges, ndc, inv, color, opacity, tiles, T, last, d_img, d_trans, scaler, H, W, th, tw, **kw))
-        rec["dn"] = np.zeros(fr["n"].shape, ndc.dtype)
-        if gn is not None:
-            dn_img = (dp._pad(np.asarray(gn, d_img.dtype), (1, 3, *T.shape[-2:])) * 2).astype(d_img.dtype)
-            nn, nc_, ncol, nop, _, _ = backward0(sorted_pid, ranges, ndc, inv, coln, opacity, tiles, T, last, dn_img, None, None,
-                                                 H, W, th, tw)
-            out[0], out[1], out[3] = out[0] + nn, out[1] + nc_, out[3] + nop
-            rec["dn"] = ncol[0] * 0.5
-        return tuple(out)
-
-    oracle.rasterize_backward = rasterize_backward
-    try:
-        yield
-    finally:
-        oracle.rasterize_backward = backward0
-
-
 def project_normal_backward(params, ids, camera, frame, dn):
     """The normal term of the project backward in fp64: (d rot [4,A,S] of the raw quaternion, d_view [4,4])."""
     C, S = params["xyz"].shape[-2:]
@@ -126,51 +84,3 @@ def project_normal_backward(params, ids, camera, frame, dn):
     d_view = np.zeros((4, 4))
     d_view[:3, :3] = frame["nw"].astype(np.float64) @ dnc.T
     return dq.reshape(4, len(ids), S), d_view
-
-
-def render_forward_backward(params, chunk_aabb, camera, img_hw, tile_hw, sh_degree, d_img_fn, render_normal=False, d_normal_fn=None,
-                            render_depth=False, d_depth_fn=None, normal_freeze=None, **kw):
-    """depth_oracle.render_forward_backward (kw as there), plus with render_normal the normal N ("normal" [V,3,H,W],
-    "normal_padded"), the per-Gaussian frame ("frame": a, nw, nc, sg, n [3,N]) and, when d_normal_fn(N, T) -> (dL/dN, dL/dT or
-    None) is given, the normal loss's gradients added to every parameter gradient; "dn" [3,N] is dL/dn of each visible Gaussian.
-    normal_freeze: an earlier "frame" whose shortest axes and facing signs are kept."""
-    if not render_normal:
-        return dp.render_forward_backward(params, chunk_aabb, camera, img_hw, tile_hw, sh_degree, d_img_fn, render_depth=render_depth,
-                                          d_depth_fn=d_depth_fn, **kw)
-    _, _, ids = oracle.frustum_culling_aabb(chunk_aabb[0], chunk_aabb[1], camera["frustumplane"])
-    rec_n, rec_p = {}, {}
-
-    def frame_fn(dt):
-        s_raw = params["scale"][:, ids, :].reshape(3, -1).astype(dt)
-        q_raw = params["rot"][:, ids, :].reshape(4, -1).astype(dt)
-        return normal_frame(s_raw, q_raw, np.asarray(camera["view"]).reshape(4, 4), rec_p["inter"]["view_pos"][0].astype(dt),
-                            freeze=normal_freeze)
-
-    project0 = oracle.project
-
-    def project(*a, **k):
-        rec_p["inter"] = project0(*a, **k)
-        return rec_p["inter"]
-
-    oracle.project = project
-    try:
-        with _normal_stages(frame_fn, d_normal_fn, rec_n):
-            out = dp.render_forward_backward(params, chunk_aabb, camera, img_hw, tile_hw, sh_degree, d_img_fn, render_depth=render_depth,
-                                             d_depth_fn=d_depth_fn, **kw)
-    finally:
-        oracle.project = project0
-    H, W = img_hw
-    dq, _ = project_normal_backward(params, ids, camera, rec_n["frame"], rec_n["dn"])
-    gr = out["grads"]["rot"]
-    out["grads"] = dict(out["grads"], rot=(gr.astype(np.float64) + dq).astype(gr.dtype))
-    out.update(normal=rec_n["normal"][..., :H, :W], normal_padded=rec_n["normal"], dn=rec_n["dn"], frame=rec_n["frame"])
-    return out
-
-
-def camera_backward(params, out, camera, img_hw, sh_degree=None, exact_grad=False):
-    """depth_oracle.camera_backward plus the normal term d view[k][j] += sum_i n_w[k] dn_c[j] (fp64) -> (d_view, d_proj)."""
-    d_view, d_proj = dp.camera_backward(params, out, camera, img_hw, sh_degree=sh_degree, exact_grad=exact_grad)
-    if "dn" not in out:
-        return d_view, d_proj
-    _, dv = project_normal_backward(params, out["visible_chunk_id"], camera, out["frame"], out["dn"])
-    return np.array(d_view, np.float64) + dv, np.array(d_proj, np.float64)

@@ -7,29 +7,21 @@ import numpy as np
 import pytest
 import torch
 
-from litegs_b200 import _lib, pipeline, render, scene
+from litegs_b200 import pipeline, render, scene
 from litegs_b200.arguments import PipelineParams
 from litegs_b200.dist import GradAccumulator
-from tests import aa_oracle as aa
-from tests.test_gpu_pipeline import _to_torch
-from tests.test_oracle_antialias import single_splat
-from tests.util import PARAM_KEYS, differing_tiles, scaled_err, small_scene
+from tests import fused_oracle as fo
+from tests.util import (PARAM_KEYS, as_f64, deterministic, differing_tiles, restatement_mask, scaled_err, single_splat,
+                        small_scene, to_torch)
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture
-def deterministic():
-    _lib.call("lgs_set_deterministic", 1)
-    yield
-    _lib.call("lgs_set_deterministic", 0)
 
 
 def _aa_case(n, hw, tile, deg, seed, view=0, scale_range=(0.003, 0.05)):
     """Scene with many sub-pixel splats; the loss weight is zero on the oracle's fragile pixels."""
     params, aabb, cam = small_scene(n=n, hw=hw, tile=tile, sh_degree=3, seed=seed, view=view, log_scale_range=scale_range)
     w = np.random.default_rng(seed + 100).normal(size=(1, 3, hw[0], hw[1])).astype(np.float32)
-    o0 = aa.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, antialiased=True)
+    o0 = fo.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, antialiased=True)
     return params, aabb, cam, w, o0
 
 
@@ -44,21 +36,14 @@ def test_fused_path_matches_oracle(cuda, deg, tile):
     hw = (96, 128)
     params, aabb, cam, w, o0 = _aa_case(4000, hw, tile, deg, seed=11)
     assert o0["rho"][o0["rho"] > 0].min() < 0.2                       # the mode is exercised
-    P, A, C = _to_torch(params, aabb, cam, cuda)
+    P, A, C = to_torch(params, aabb, cam, cuda)
     _, st, _ = _forward(P, A, C, deg, hw, tile, True)
     D = o0["sorted_pid"].shape[1]
-    bad, npairs = differing_tiles(st.ranges.cpu().numpy(), st.sorted_pid.cpu().numpy(), o0["ranges"], o0["sorted_pid"])
-    print(f"AA deg {deg} tile {tile}: {D} pairs (ours {st.n_pairs}), {len(bad)} tiles / {npairs} pairs differ")
-    assert abs(st.n_pairs - D) <= max(2, 1e-4 * D) and len(bad) <= 2
-    frag = o0["fragile"][:, :hw[0], :hw[1]].copy()
-    gx = -(-hw[1] // tile[1])
-    for t in bad:
-        ty, tx = divmod(int(t), gx)
-        frag[:, ty * tile[0]:(ty + 1) * tile[0], tx * tile[1]:(tx + 1) * tile[1]] = True
-    lc = st.last.cpu().numpy()[:, 0, :hw[0], :hw[1]].astype(np.uint16)
-    assert np.array_equal(lc[~frag], o0["last"][:, 0, :hw[0], :hw[1]].astype(np.uint16)[~frag])
+    frag = restatement_mask(st, o0, hw, tile)
+    print(f"AA deg {deg} tile {tile}: {D} pairs (ours {st.n_pairs})")
+    assert abs(st.n_pairs - D) <= max(2, 1e-4 * D)
     w = w * (~frag)[:, None]
-    ref = aa.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, antialiased=True)
+    ref = fo.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, antialiased=True)
     pp = PipelineParams(tile_size=tile, antialiased=True)
     img = render.render_view(A[0], A[1], C["frustumplane"], C["view"], C["proj"], P["xyz"], P["scale"], P["rot"], P["sh_0"], P["sh_rest"],
                              P["opacity"], deg, hw, pp)[0]
@@ -80,7 +65,7 @@ def test_off_is_the_default_bit_for_bit(cuda, deterministic):
     w = torch.from_numpy(np.random.default_rng(1).normal(size=(1, 3, *hw)).astype(np.float32)).to(cuda)
     outs = []
     for kw in ({}, {"antialiased": False}, {"antialiased": True}):
-        P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+        P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
         img, st, _ = pipeline.render_view_forward(P, A[0], A[1], C["frustumplane"], C["view"], C["proj"], 3, hw, tile, clamp_zero=True, **kw)
         d = torch.zeros_like(img)
         d[..., :hw[0], :hw[1]] = w
@@ -98,7 +83,7 @@ def test_deterministic_backward_and_pair_count(cuda, deterministic):
     w = torch.from_numpy(np.random.default_rng(2).normal(size=(1, 3, *hw)).astype(np.float32)).to(cuda)
     runs = []
     for _ in range(2):
-        P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+        P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
         img, st, _ = pipeline.render_view_forward(P, A[0], A[1], C["frustumplane"], C["view"], C["proj"], 3, hw, tile, clamp_zero=True,
                                                   antialiased=True)
         d = torch.zeros_like(img)
@@ -116,7 +101,7 @@ def test_deterministic_backward_and_pair_count(cuda, deterministic):
 def test_integrated_alpha_on_the_gpu(cuda, std_px):
     hw = (64, 64)
     params, aabb, cam = single_splat(std_px, hw, chunk=32, dt=np.float32)
-    P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+    P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
     _, st, _ = _forward(P, A, C, 0, hw, (16, 16), True)
     got = float((1 - st.T[..., :hw[0], :hw[1]]).double().sum())
     o = 0.8
@@ -228,11 +213,10 @@ def test_camera_gradient_matches_oracle(cuda, deterministic, deg, view):
     params, aabb, cam, w, o0 = _aa_case(4000, hw, tile, deg, seed=12, view=view)
     frag = o0["fragile"][:, :hw[0], :hw[1]]
     w = w * (~frag)[:, None]
-    ref = aa.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, antialiased=True)
-    ref64 = dict(ref, inter={k: v.astype(np.float64) for k, v in ref["inter"].items()}, d_ndc=ref["d_ndc"].astype(np.float64),
-                 d_cov=ref["d_cov"].astype(np.float64), G_aa=ref["G_aa"].astype(np.float64))
-    d_view, d_proj = aa.camera_backward(params, ref64, cam, hw)
-    P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+    ref = fo.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, antialiased=True)
+    ref64 = as_f64(ref)
+    d_view, d_proj = fo.camera_backward(params, ref64, cam, hw)
+    P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
     _, st, _ = _forward(P, A, C, deg, hw, tile, True)
     bad, _ = differing_tiles(st.ranges.cpu().numpy(), st.sorted_pid.cpu().numpy(), ref["ranges"], ref["sorted_pid"])
     assert len(bad) == 0
@@ -279,10 +263,10 @@ def test_c2_one_view_matches_oracle(cuda):
     aabb = (p["cluster_origin"], p["cluster_extend"])
     cam = scene.make_camera(0, 64, W, H)
     w = np.random.default_rng(7).normal(size=(1, 3, H, W)).astype(np.float32)
-    o0 = aa.render_forward_backward(params, aabb, cam, (H, W), tile, deg, lambda img: w, antialiased=True)
+    o0 = fo.render_forward_backward(params, aabb, cam, (H, W), tile, deg, lambda img: w, antialiased=True)
     frag = o0["fragile"][:, :H, :W].copy()
     assert frag.mean() < 0.10
-    P, A, C = _to_torch(params, aabb, cam, cuda)
+    P, A, C = to_torch(params, aabb, cam, cuda)
     _, st, _ = _forward(P, A, C, deg, (H, W), tile, True)
     D = o0["sorted_pid"].shape[1]
     bad, npairs = differing_tiles(st.ranges.cpu().numpy(), st.sorted_pid.cpu().numpy(), o0["ranges"], o0["sorted_pid"])
@@ -303,7 +287,7 @@ def test_c2_one_view_matches_oracle(cuda):
           f"{int((lc[~frag] != lo[~frag]).sum()) == 0}; {frag.mean() * 100:.2f} % fragile in all")
     assert np.array_equal(lc[~frag], lo[~frag])
     w = w * (~frag)[:, None]
-    ref = aa.render_forward_backward(params, aabb, cam, (H, W), tile, deg, lambda img: w, antialiased=True)
+    ref = fo.render_forward_backward(params, aabb, cam, (H, W), tile, deg, lambda img: w, antialiased=True)
     pp = PipelineParams(tile_size=tile, antialiased=True)
     img = render.render_view(A[0], A[1], C["frustumplane"], C["view"], C["proj"], P["xyz"], P["scale"], P["rot"], P["sh_0"], P["sh_rest"],
                              P["opacity"], deg, (H, W), pp)[0]
@@ -321,7 +305,7 @@ def test_c2_one_view_matches_oracle(cuda):
 def test_level_a_refuses_the_mode(cuda):
     hw, tile = (48, 64), (8, 16)
     params, aabb, cam = small_scene(n=500, hw=hw, tile=tile, seed=1)
-    P, A, C = _to_torch(params, aabb, cam, cuda)
+    P, A, C = to_torch(params, aabb, cam, cuda)
     pp = PipelineParams(tile_size=tile, antialiased=True)
     ids, num, cx, cs, cr, col, cop = render.render_preprocess(A[0], A[1], C["frustumplane"], C["view"], P["xyz"], P["scale"], P["rot"],
                                                               P["sh_0"], P["sh_rest"], P["opacity"], None, None, pp, 3)

@@ -7,32 +7,15 @@ import numpy as np
 import pytest
 import torch
 
-from litegs_b200 import _lib, colmap, fused, pipeline, render, scene, wrapper
+from litegs_b200 import fused, pipeline, render, scene, wrapper
 from litegs_b200.arguments import PipelineParams
 from litegs_b200.dist import GradAccumulator
 from tests import camera_oracle as co
-from tests.test_gpu_pipeline import _case, _to_torch
-from tests.util import PARAM_KEYS
+from tests.util import PARAM_KEYS, ZF, ZN, as_f64, deterministic, oracle_case, rot_err_deg, to_torch, view_params
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden", "viewproj.npz")
-ZN, ZF = 0.01, 5000.0
-
-
-@pytest.fixture
-def deterministic():
-    """Bit-identity checks need the raster backward's deterministic accumulation (lgs_set_deterministic): its default fp32 atomics
-    make the record gradients, and so every gradient after them, reproducible only to rounding."""
-    _lib.call("lgs_set_deterministic", 1)
-    yield
-    _lib.call("lgs_set_deterministic", 0)
-
-
-def _view_params(cam):
-    """(qw qx qy qz tx ty tz) of a row-vector view matrix [1,4,4]: its 3x3 block is the transpose of the COLMAP rotation."""
-    V = np.asarray(cam["view"], np.float64).reshape(4, 4)
-    return np.concatenate([colmap.rotmat_to_qvec(V[:3, :3].T), V[3, :3]])
 
 
 def test_create_viewproj_matches_oracle_and_reference(cuda):
@@ -69,11 +52,9 @@ def _camera_grad_direct(P, A, C, deg, hw, tile, w, accumulate_into=None):
 @pytest.mark.parametrize("deg,tile,view", [(3, (16, 16), 0), (3, (8, 16), 3), (0, (8, 16), 5), (0, (16, 16), 6)])
 def test_render_view_camera_gradient_matches_oracle(cuda, deterministic, deg, tile, view):
     hw = (96, 128)
-    params, aabb, cam, w, frag, ref = _case(4000, hw, tile, deg, seed=11, view=view)
-    d_view, d_proj, _ = co.camera_backward(params, {**ref, "inter": {k: v.astype(np.float64) for k, v in ref["inter"].items()},
-                                                    "d_ndc": ref["d_ndc"].astype(np.float64), "d_cov": ref["d_cov"].astype(np.float64)},
-                                           cam, hw)
-    P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+    params, aabb, cam, w, frag, ref = oracle_case(4000, hw, tile, deg, seed=11, view=view)
+    d_view, d_proj, _ = co.camera_backward(params, as_f64(ref), cam, hw)
+    P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
     V = C["view"].clone().requires_grad_(True)
     Pm = C["proj"].clone().requires_grad_(True)
     pp = PipelineParams(tile_size=tile)
@@ -204,9 +185,9 @@ def test_workspace_replay_equals_synchronising_path(cuda, deterministic):
 def test_autograd_through_create_viewproj(cuda, deterministic):
     """CreateViewProj.apply -> render_view -> backward fills extr.grad with create_viewproj_backward of the direct d_view/d_proj."""
     hw, tile = (96, 128), (8, 16)
-    params, aabb, cam, w, frag, ref = _case(4000, hw, tile, 3, seed=12, view=2)
-    P, A, _ = _to_torch(params, aabb, cam, cuda, grad=False)
-    extr = torch.tensor(np.stack([_view_params(cam)]), dtype=torch.float32, device=cuda).requires_grad_(True)
+    params, aabb, cam, w, frag, ref = oracle_case(4000, hw, tile, 3, seed=12, view=2)
+    P, A, _ = to_torch(params, aabb, cam, cuda, grad=False)
+    extr = torch.tensor(np.stack([view_params(cam)]), dtype=torch.float32, device=cuda).requires_grad_(True)
     intr = torch.tensor([float(cam["proj"][0, 0, 0])], dtype=torch.float32, device=cuda).requires_grad_(True)
     pp = PipelineParams(tile_size=tile)
     view, proj, _, planes = wrapper.CreateViewProj.apply(extr, intr, hw[0], hw[1], ZN, ZF)
@@ -221,11 +202,6 @@ def test_autograd_through_create_viewproj(cuda, deterministic):
     assert float(extr.grad.abs().max()) > 0
 
 
-def _rot_err_deg(a, b):
-    qa, qb = a[:4] / np.linalg.norm(a[:4]), b[:4] / np.linalg.norm(b[:4])
-    return float(np.degrees(2 * np.arccos(min(1.0, abs(float(np.dot(qa, qb)))))))
-
-
 def test_pose_recovery(cuda):
     """Gaussians at ground truth, 4 cameras perturbed by 1 degree of rotation and 2 % of their distance in translation; Adam on the
     extrinsics alone with an L1 loss brings every camera's rotation and translation errors below 25 % of their initial values."""
@@ -235,7 +211,7 @@ def test_pose_recovery(cuda):
     P = {k: torch.from_numpy(p[k]).to(cuda) for k in PARAM_KEYS}
     A = [torch.from_numpy(p[k]).to(cuda) for k in ("cluster_origin", "cluster_extend")]
     n = 4
-    true = np.stack([_view_params(scene.make_camera(v, n, W, H)) for v in range(n)])
+    true = np.stack([view_params(scene.make_camera(v, n, W, H)) for v in range(n)])
     recp = torch.tensor([float(scene.make_camera(0, n, W, H)["proj"][0, 0, 0])], device=cuda)
     pp = PipelineParams(tile_size=tile)
     rng = np.random.default_rng(1)
@@ -254,7 +230,7 @@ def test_pose_recovery(cuda):
         gts = [render.render_view(A[0], A[1], tpl[v:v + 1], tv[v:v + 1], tp[v:v + 1], P["xyz"], P["scale"], P["rot"], P["sh_0"], P["sh_rest"],
                                   P["opacity"], 3, hw, pp)[0] for v in range(n)]
     extr = torch.tensor(noisy, dtype=torch.float32, device=cuda).requires_grad_(True)
-    rot0 = [_rot_err_deg(noisy[v], true[v]) for v in range(n)]
+    rot0 = [rot_err_deg(noisy[v], true[v]) for v in range(n)]
     tr0 = [float(np.linalg.norm(noisy[v, 4:] - true[v, 4:])) for v in range(n)]
     steps = 300
     opt = torch.optim.Adam([extr], lr=3e-3)
@@ -271,7 +247,7 @@ def test_pose_recovery(cuda):
         opt.step()
         sched.step()
     est = extr.detach().double().cpu().numpy()
-    rot1 = [_rot_err_deg(est[v], true[v]) for v in range(n)]
+    rot1 = [rot_err_deg(est[v], true[v]) for v in range(n)]
     tr1 = [float(np.linalg.norm(est[v, 4:] - true[v, 4:])) for v in range(n)]
     print("pose recovery: rotation error (deg)", [f"{a:.3f} -> {b:.4f}" for a, b in zip(rot0, rot1)],
           "translation error", [f"{a:.4f} -> {b:.5f}" for a, b in zip(tr0, tr1)])

@@ -12,20 +12,12 @@ import torch
 from litegs_b200 import _lib, pipeline, render, scene
 from litegs_b200.arguments import PipelineParams
 from litegs_b200.dist import GradAccumulator
-from tests import depth_oracle as dp
 from tests import filter3d_oracle as f3
-from tests.test_gpu_exact_grad import _lattice
-from tests.test_gpu_pipeline import _to_torch
-from tests.util import PARAM_KEYS, differing_tiles, scaled_err, small_scene
+from tests import fused_oracle as fo
+from tests.util import (PARAM_KEYS, as_f64, deterministic, differing_tiles, lattice_cameras, restatement_mask, scaled_err,
+                        small_scene, to_torch)
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture
-def deterministic():
-    _lib.call("lgs_set_deterministic", 1)
-    yield
-    _lib.call("lgs_set_deterministic", 0)
 
 
 def _weights(hw, seed):
@@ -40,34 +32,25 @@ CASES = [(deg, tile, aa, f) for deg in (0, 3) for tile in ((8, 16), (16, 16)) fo
 def test_fused_path_matches_restatement(cuda, deg, tile, antialiased, filtered):
     hw = (96, 128)
     params, aabb, cam = small_scene(n=4000, hw=hw, tile=tile, sh_degree=3, seed=40 + deg, log_scale_range=(0.003, 0.05))
-    filt = f3.compute_filter(params["xyz"], *_lattice(24, (36, 48)))[None] if filtered else None
+    filt = f3.compute_filter(params["xyz"], *lattice_cameras(24, (36, 48)))[None] if filtered else None
     if filtered:
         aabb = scene.cluster_aabb(params["xyz"], params["scale"], params["rot"], filter_3d=filt)
     w, u = _weights(hw, deg)
     kw = dict(antialiased=antialiased, filter_3d=filt)
-    o0 = dp.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, render_depth=True, **kw)
-    P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+    o0 = fo.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, render_depth=True, **kw)
+    P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
     F = None if filt is None else torch.from_numpy(filt).to(cuda)
     img, st, _ = pipeline.render_view_forward(P, A[0], A[1], C["frustumplane"], C["view"], C["proj"], deg, hw, tile, clamp_zero=True,
                                               antialiased=antialiased, filter_3d=F, render_depth=True)
-    bad, _ = differing_tiles(st.ranges.cpu().numpy(), st.sorted_pid.cpu().numpy(), o0["ranges"], o0["sorted_pid"])
-    assert len(bad) <= 2
-    frag = o0["fragile"][:, :hw[0], :hw[1]].copy()
-    gx = -(-hw[1] // tile[1])
-    for t in bad:
-        ty, tx = divmod(int(t), gx)
-        frag[:, ty * tile[0]:(ty + 1) * tile[0], tx * tile[1]:(tx + 1) * tile[1]] = True
+    frag = restatement_mask(st, o0, hw, tile)
     ok = ~frag[:, None]
-    last = st.last.cpu().numpy()[..., :hw[0], :hw[1]]
-    assert np.array_equal(last[ok], o0["last"][..., :hw[0], :hw[1]][ok])
     errs = {"img": np.abs(img.cpu().numpy()[..., :hw[0], :hw[1]] - o0["img"])[np.broadcast_to(ok, o0["img"].shape)].max(),
             "D": np.abs(st.depth.cpu().numpy()[..., :hw[0], :hw[1]] - o0["depth"])[ok].max() / np.abs(o0["depth"]).max()}
     w, u = w * ok, u * ok
-    ref = dp.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, render_depth=True, d_depth_fn=lambda D, T: (u, None),
+    ref = fo.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, render_depth=True, d_depth_fn=lambda D, T: (u, None),
                                      **kw)
-    ref64 = dict(ref, inter={k: v.astype(np.float64) for k, v in ref["inter"].items()}, d_ndc=ref["d_ndc"].astype(np.float64),
-                 d_cov=ref["d_cov"].astype(np.float64), G_aa=ref["G_aa"].astype(np.float64))
-    d_view, d_proj = dp.camera_backward(params, ref64, cam, hw, sh_degree=deg)
+    ref64 = as_f64(ref)
+    d_view, d_proj = fo.camera_backward(params, ref64, cam, hw, sh_degree=deg)
     nvis = int(ref["visible_chunk_id"].shape[0])
     d = torch.zeros_like(img)
     d[..., :hw[0], :hw[1]] = torch.from_numpy(w).to(cuda)
@@ -87,7 +70,7 @@ def test_weights_sum_to_one_minus_T(cuda):
     D / (1 - T) is a weighted mean of the depths."""
     hw, tile = (96, 128), (8, 16)
     params, aabb, cam = small_scene(n=4000, hw=hw, tile=tile, seed=3, log_scale_range=(0.003, 0.05))
-    P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+    P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
     img, st, _ = pipeline.render_view_forward(P, A[0], A[1], C["frustumplane"], C["view"], C["proj"], 3, hw, tile, clamp_zero=True,
                                               render_depth=True)
     packed = st.packed.clone()
@@ -110,7 +93,7 @@ def test_weights_sum_to_one_minus_T(cuda):
 
 def _render_grads(cuda, params, aabb, cam, hw, tile, pp, deg=3, u=None):
     """render_view + backward (a colour loss, plus sum u D when u is given) with the matrices as leaves -> dict of outputs."""
-    P, A, C = _to_torch(params, aabb, cam, cuda)
+    P, A, C = to_torch(params, aabb, cam, cuda)
     view, proj = C["view"].clone().requires_grad_(True), C["proj"].clone().requires_grad_(True)
     img, _, depth, _, last = render.render_view(A[0], A[1], C["frustumplane"], view, proj, P["xyz"], P["scale"], P["rot"], P["sh_0"],
                                                 P["sh_rest"], P["opacity"], deg, hw, pp)
@@ -235,7 +218,7 @@ def test_deterministic_and_statistics_modes(cuda, deterministic):
     D, the gradients, the camera gradient and the depth slot equal the statistics-off run to 1e-6 of their maximum."""
     hw, tile = (96, 128), (16, 16)
     params, aabb, cam = small_scene(n=4000, hw=hw, tile=tile, seed=11, log_scale_range=(0.003, 0.05))
-    P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+    P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
     w, u = (torch.from_numpy(x).to(cuda) for x in _weights(hw, 1))
     a = _one_view(cuda, P, A, C, hw, tile, u, w)
     b = _one_view(cuda, P, A, C, hw, tile, u, w)
@@ -282,7 +265,7 @@ def test_non_default_raster_variants_refuse_depth(cuda):
     the entry point returns an error instead of dropping the depth."""
     hw, tile = (96, 128), (8, 16)
     params, aabb, cam = small_scene(n=2000, hw=hw, tile=tile, seed=2)
-    P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+    P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
     fwd = lambda: pipeline.render_view_forward(P, A[0], A[1], C["frustumplane"], C["view"], C["proj"], 3, hw, tile, clamp_zero=True,
                                                render_depth=True)
     img, st, _ = fwd()
@@ -331,7 +314,7 @@ def test_depth_slot_reaches_view_column_2_and_not_proj(cuda):
     (by p~_k dz summed over the Gaussians, within fp32 rounding of the fp64 sum); d_proj and the other gradients keep their bits."""
     hw, tile = (96, 128), (8, 16)
     params, aabb, cam = small_scene(n=4000, hw=hw, tile=tile, seed=12, log_scale_range=(0.003, 0.05))
-    P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+    P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
     w, u = (torch.from_numpy(x).to(cuda) for x in _weights(hw, 2))
     img, st, _ = pipeline.render_view_forward(P, A[0], A[1], C["frustumplane"], C["view"], C["proj"], 3, hw, tile, clamp_zero=True,
                                               render_depth=True)
@@ -398,10 +381,10 @@ def test_c2_one_view_matches_restatement(cuda):
     cam = scene.make_camera(0, 64, W, H)
     g = np.random.default_rng(7)
     w, u = g.normal(size=(1, 3, H, W)).astype(np.float32), g.normal(size=(1, 1, H, W)).astype(np.float32)
-    o0 = dp.render_forward_backward(params, aabb, cam, (H, W), tile, deg, lambda img: w, render_depth=True)
+    o0 = fo.render_forward_backward(params, aabb, cam, (H, W), tile, deg, lambda img: w, render_depth=True)
     frag = o0["fragile"][:, :H, :W].copy()
     assert frag.mean() < 0.10
-    P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+    P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
     img, st, _ = pipeline.render_view_forward(P, A[0], A[1], C["frustumplane"], C["view"], C["proj"], deg, (H, W), tile, clamp_zero=True,
                                               render_depth=True)
     bad, npairs = differing_tiles(st.ranges.cpu().numpy(), st.sorted_pid.cpu().numpy(), o0["ranges"], o0["sorted_pid"])
@@ -419,11 +402,10 @@ def test_c2_one_view_matches_restatement(cuda):
     errs = {"img": np.abs(img.cpu().numpy()[..., :H, :W] - o0["img"])[np.broadcast_to(ok, o0["img"].shape)].max(),
             "D": np.abs(st.depth.cpu().numpy()[..., :H, :W] - o0["depth"])[ok].max() / np.abs(o0["depth"]).max()}
     w, u = w * ok, u * ok
-    ref = dp.render_forward_backward(params, aabb, cam, (H, W), tile, deg, lambda img: w, render_depth=True,
+    ref = fo.render_forward_backward(params, aabb, cam, (H, W), tile, deg, lambda img: w, render_depth=True,
                                      d_depth_fn=lambda D_, T_: (u, None))
-    ref64 = dict(ref, inter={k: v.astype(np.float64) for k, v in ref["inter"].items()}, d_ndc=ref["d_ndc"].astype(np.float64),
-                 d_cov=ref["d_cov"].astype(np.float64), G_aa=ref["G_aa"].astype(np.float64))
-    d_view, d_proj = dp.camera_backward(params, ref64, cam, (H, W), sh_degree=deg)
+    ref64 = as_f64(ref)
+    d_view, d_proj = fo.camera_backward(params, ref64, cam, (H, W), sh_degree=deg)
     d = torch.zeros_like(img)
     d[..., :H, :W] = torch.from_numpy(w).to(cuda)
     cg = torch.empty((2, 4, 4), device=cuda)

@@ -8,28 +8,15 @@ import numpy as np
 import pytest
 import torch
 
-from litegs_b200 import _lib, fused, pipeline, render, scene, wrapper
+from litegs_b200 import fused, pipeline, render, scene, wrapper
 from litegs_b200.arguments import PipelineParams
 from litegs_b200.dist import GradAccumulator
-from tests import exact_grad_oracle as ex
 from tests import filter3d_oracle as f3
-from tests.test_gpu_camera import ZF, ZN, _rot_err_deg, _view_params
-from tests.test_gpu_pipeline import _to_torch
-from tests.util import PARAM_KEYS, differing_tiles, scaled_err, small_scene
+from tests import fused_oracle as fo
+from tests.util import (PARAM_KEYS, ZF, ZN, as_f64, deterministic, lattice_cameras, restatement_mask, rot_err_deg, scaled_err,
+                        small_scene, to_torch, view_params)
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture
-def deterministic():
-    _lib.call("lgs_set_deterministic", 1)
-    yield
-    _lib.call("lgs_set_deterministic", 0)
-
-
-def _lattice(n, hw):
-    cams = [scene.make_camera(i, n, hw[1], hw[0]) for i in range(n)]
-    return np.concatenate([c["view"] for c in cams]), np.concatenate([c["proj"] for c in cams]), np.array([hw] * n, np.int32)
 
 
 def _reference(cuda, params, aabb, cam, hw, tile, deg, antialiased, filt, seed):
@@ -37,23 +24,16 @@ def _reference(cuda, params, aabb, cam, hw, tile, deg, antialiased, filt, seed):
     from ours) zeroed -> (w, ref, d_view, d_proj); the camera gradient is summed in fp64."""
     w = np.random.default_rng(seed).normal(size=(1, 3, *hw)).astype(np.float32)
     kw = dict(antialiased=antialiased, filter_3d=filt)
-    o0 = ex.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, **kw)
-    P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+    o0 = fo.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, **kw)
+    P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
     F = None if filt is None else torch.from_numpy(filt).to(cuda)
     _, st, _ = pipeline.render_view_forward(P, A[0], A[1], C["frustumplane"], C["view"], C["proj"], deg, hw, tile, clamp_zero=True,
                                             antialiased=antialiased, filter_3d=F)
-    bad, _ = differing_tiles(st.ranges.cpu().numpy(), st.sorted_pid.cpu().numpy(), o0["ranges"], o0["sorted_pid"])
-    assert len(bad) <= 2
-    frag = o0["fragile"][:, :hw[0], :hw[1]].copy()
-    gx = -(-hw[1] // tile[1])
-    for t in bad:
-        ty, tx = divmod(int(t), gx)
-        frag[:, ty * tile[0]:(ty + 1) * tile[0], tx * tile[1]:(tx + 1) * tile[1]] = True
+    frag = restatement_mask(st, o0, hw, tile)
     w = w * (~frag)[:, None]
-    ref = ex.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, exact_grad=True, **kw)
-    ref64 = dict(ref, inter={k: v.astype(np.float64) for k, v in ref["inter"].items()}, d_ndc=ref["d_ndc"].astype(np.float64),
-                 d_cov=ref["d_cov"].astype(np.float64), G_aa=ref["G_aa"].astype(np.float64))
-    d_view, d_proj = ex.camera_backward(params, ref64, cam, hw, exact_grad=True)
+    ref = fo.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, exact_grad=True, **kw)
+    ref64 = as_f64(ref)
+    d_view, d_proj = fo.camera_backward(params, ref64, cam, hw, exact_grad=True)
     return w, ref, d_view, d_proj
 
 
@@ -66,11 +46,11 @@ def test_fused_path_matches_restatement(cuda, deg, antialiased, filtered):
     hw = (96, 128)
     tile = (8, 16) if (deg + antialiased + filtered) % 2 == 0 else (16, 16)
     params, aabb, cam = small_scene(n=4000, hw=hw, tile=tile, sh_degree=3, seed=20 + deg, log_scale_range=(0.003, 0.05))
-    filt = f3.compute_filter(params["xyz"], *_lattice(24, (36, 48)))[None] if filtered else None
+    filt = f3.compute_filter(params["xyz"], *lattice_cameras(24, (36, 48)))[None] if filtered else None
     if filtered:
         aabb = scene.cluster_aabb(params["xyz"], params["scale"], params["rot"], filter_3d=filt)
     w, ref, d_view, d_proj = _reference(cuda, params, aabb, cam, hw, tile, deg, antialiased, filt, seed=deg)
-    P, A, C = _to_torch(params, aabb, cam, cuda)
+    P, A, C = to_torch(params, aabb, cam, cuda)
     F = None if filt is None else torch.from_numpy(filt).to(cuda)
     nvis = int(ref["visible_chunk_id"].shape[0])
     # autograd, no camera gradient (CAM = false)
@@ -107,7 +87,7 @@ def test_degree_0_model_on_the_autograd_and_workspace_paths(cuda, deterministic)
     w, ref, d_view, d_proj = _reference(cuda, params, aabb, cam, hw, tile, 0, False, None, seed=31)
     ids = ref["visible_chunk_id"]
     nvis = int(ids.shape[0])
-    P, A, C = _to_torch(params, aabb, cam, cuda)
+    P, A, C = to_torch(params, aabb, cam, cuda)
     pp = PipelineParams(tile_size=tile, exact_grad=True)
     view, proj = C["view"].clone().requires_grad_(True), C["proj"].clone().requires_grad_(True)
     img = render.render_view(A[0], A[1], C["frustumplane"], view, proj, P["xyz"], P["scale"], P["rot"], P["sh_0"], P["sh_rest"],
@@ -171,7 +151,7 @@ def test_chunk_size_beyond_the_exact_kernels_limit_is_refused(cuda):
 
 def _render_grads(cuda, params, aabb, cam, hw, tile, pp, deg=3):
     """render_view + backward with the view and projection matrices as leaves -> (img, T, last, dense grads, d view, d proj)."""
-    P, A, C = _to_torch(params, aabb, cam, cuda)
+    P, A, C = to_torch(params, aabb, cam, cuda)
     view, proj = C["view"].clone().requires_grad_(True), C["proj"].clone().requires_grad_(True)
     img, _, _, _, last = render.render_view(A[0], A[1], C["frustumplane"], view, proj, P["xyz"], P["scale"], P["rot"], P["sh_0"],
                                             P["sh_rest"], P["opacity"], deg, hw, pp)
@@ -309,7 +289,7 @@ def _pose_recovery(cuda, exact_grad):
     P = {k: torch.from_numpy(p[k]).to(cuda) for k in PARAM_KEYS}
     A = [torch.from_numpy(p[k]).to(cuda) for k in ("cluster_origin", "cluster_extend")]
     n = 4
-    true = np.stack([_view_params(scene.make_camera(v, n, W, H)) for v in range(n)])
+    true = np.stack([view_params(scene.make_camera(v, n, W, H)) for v in range(n)])
     recp = torch.tensor([float(scene.make_camera(0, n, W, H)["proj"][0, 0, 0])], device=cuda)
     pp = PipelineParams(tile_size=tile, exact_grad=exact_grad)
     rng = np.random.default_rng(1)
@@ -328,7 +308,7 @@ def _pose_recovery(cuda, exact_grad):
         gts = [render.render_view(A[0], A[1], tpl[v:v + 1], tv[v:v + 1], tp[v:v + 1], P["xyz"], P["scale"], P["rot"], P["sh_0"], P["sh_rest"],
                                   P["opacity"], 3, hw, pp)[0] for v in range(n)]
     extr = torch.tensor(noisy, dtype=torch.float32, device=cuda).requires_grad_(True)
-    rot0 = [_rot_err_deg(noisy[v], true[v]) for v in range(n)]
+    rot0 = [rot_err_deg(noisy[v], true[v]) for v in range(n)]
     tr0 = [float(np.linalg.norm(noisy[v, 4:] - true[v, 4:])) for v in range(n)]
     steps = 300
     opt = torch.optim.Adam([extr], lr=3e-3)
@@ -345,7 +325,7 @@ def _pose_recovery(cuda, exact_grad):
         opt.step()
         sched.step()
     est = extr.detach().double().cpu().numpy()
-    rot1 = [_rot_err_deg(est[v], true[v]) for v in range(n)]
+    rot1 = [rot_err_deg(est[v], true[v]) for v in range(n)]
     tr1 = [float(np.linalg.norm(est[v, 4:] - true[v, 4:])) for v in range(n)]
     return rot0, rot1, tr0, tr1
 

@@ -8,27 +8,15 @@ import numpy as np
 import pytest
 import torch
 
-from litegs_b200 import _lib, pipeline, render, scene
+from litegs_b200 import pipeline, render, scene
 from litegs_b200.arguments import PipelineParams
 from litegs_b200.dist import GradAccumulator
-from tests import aa_oracle as aa
 from tests import filter3d_oracle as f3
-from tests.test_gpu_pipeline import _to_torch
-from tests.util import PARAM_KEYS, differing_tiles, scaled_err, small_scene
+from tests import fused_oracle as fo
+from tests.util import (PARAM_KEYS, as_f64, deterministic, differing_tiles, lattice_cameras, restatement_mask, scaled_err,
+                        small_scene, to_torch)
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture
-def deterministic():
-    _lib.call("lgs_set_deterministic", 1)
-    yield
-    _lib.call("lgs_set_deterministic", 0)
-
-
-def _lattice(n, hw, radius=3.0, fov=60.0):
-    cams = [scene.make_camera(i, n, hw[1], hw[0], radius=radius, fov_x_deg=fov) for i in range(n)]
-    return np.concatenate([c["view"] for c in cams]), np.concatenate([c["proj"] for c in cams]), np.array([hw] * n, np.int32)
 
 
 def _device_filter(xyz, views, projs, hws, cuda, out=None):
@@ -49,11 +37,11 @@ def _kernel_cases():
         c = scene.make_camera(i, 8, w, h, fov_x_deg=fov)
         mixed_v.append(c["view"]); mixed_p.append(c["proj"]); mixed_hw.append((h, w))
     mixed = (np.concatenate(mixed_v), np.concatenate(mixed_p), np.array(mixed_hw, np.int32))
-    v1 = _lattice(1, (90, 160))
+    v1 = lattice_cameras(1, (90, 160))
     # the camera at z = -3 looks towards -z: every point is behind it
     cam_behind = (np.stack([scene.look_at_view_matrix(np.array([0.0, 0.0, -3.0]), target=(0.0, 0.0, -10.0))]),
                   scene.proj_matrix(64, 64)[None], np.array([[64, 64]], np.int32))
-    return {"V=1": (xyz, *v1), "V=1000": (far, *(x[:1000] for x in _lattice(2000, (72, 96)))), "mixed sizes": (far, *mixed),
+    return {"V=1": (xyz, *v1), "V=1000": (far, *(x[:1000] for x in lattice_cameras(2000, (72, 96)))), "mixed sizes": (far, *mixed),
             "none seen": (xyz, *cam_behind)}
 
 
@@ -78,10 +66,10 @@ def test_filter_kernel_matches_restatement_bit_for_bit(cuda, case):
 def _case(n, hw, tile, deg, seed, antialiased, view=0, scale_range=(0.003, 0.05)):
     """Scene with sub-pixel splats and a filter from 24 low-resolution lattice cameras, strong enough that rho3 < 0.5 occurs."""
     params, aabb, cam = small_scene(n=n, hw=hw, tile=tile, sh_degree=3, seed=seed, view=view, log_scale_range=scale_range)
-    filt = f3.compute_filter(params["xyz"], *_lattice(24, (36, 48)))[None]
+    filt = f3.compute_filter(params["xyz"], *lattice_cameras(24, (36, 48)))[None]
     aabb = scene.cluster_aabb(params["xyz"], params["scale"], params["rot"], filter_3d=filt)
     w = np.random.default_rng(seed + 100).normal(size=(1, 3, hw[0], hw[1])).astype(np.float32)
-    o0 = f3.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, antialiased=antialiased, filter_3d=filt)
+    o0 = fo.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, antialiased=antialiased, filter_3d=filt)
     return params, aabb, cam, filt, w, o0
 
 
@@ -97,22 +85,15 @@ def test_fused_path_matches_oracle(cuda, deg, tile, antialiased):
     hw = (96, 128)
     params, aabb, cam, filt, w, o0 = _case(4000, hw, tile, deg, 11, antialiased)
     assert o0["rho3"].min() < 0.5
-    P, A, C = _to_torch(params, aabb, cam, cuda)
+    P, A, C = to_torch(params, aabb, cam, cuda)
     F = torch.from_numpy(filt).to(cuda)
     _, st, _ = _forward(P, A, C, deg, hw, tile, antialiased, F)
     D = o0["sorted_pid"].shape[1]
-    bad, npairs = differing_tiles(st.ranges.cpu().numpy(), st.sorted_pid.cpu().numpy(), o0["ranges"], o0["sorted_pid"])
-    print(f"F3D aa={antialiased} deg {deg} tile {tile}: {D} pairs (ours {st.n_pairs}), {len(bad)} tiles / {npairs} pairs differ")
-    assert abs(st.n_pairs - D) <= max(2, 1e-4 * D) and len(bad) <= 2
-    frag = o0["fragile"][:, :hw[0], :hw[1]].copy()
-    gx = -(-hw[1] // tile[1])
-    for t in bad:
-        ty, tx = divmod(int(t), gx)
-        frag[:, ty * tile[0]:(ty + 1) * tile[0], tx * tile[1]:(tx + 1) * tile[1]] = True
-    lc = st.last.cpu().numpy()[:, 0, :hw[0], :hw[1]].astype(np.uint16)
-    assert np.array_equal(lc[~frag], o0["last"][:, 0, :hw[0], :hw[1]].astype(np.uint16)[~frag])
+    frag = restatement_mask(st, o0, hw, tile)
+    print(f"F3D aa={antialiased} deg {deg} tile {tile}: {D} pairs (ours {st.n_pairs})")
+    assert abs(st.n_pairs - D) <= max(2, 1e-4 * D)
     w = w * (~frag)[:, None]
-    ref = f3.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, antialiased=antialiased, filter_3d=filt)
+    ref = fo.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, antialiased=antialiased, filter_3d=filt)
     pp = PipelineParams(tile_size=tile, antialiased=antialiased)
     img = render.render_view(A[0], A[1], C["frustumplane"], C["view"], C["proj"], P["xyz"], P["scale"], P["rot"], P["sh_0"], P["sh_rest"],
                              P["opacity"], deg, hw, pp, filter_3d=F)[0]
@@ -137,7 +118,7 @@ def test_no_filter_is_the_default_and_zero_filter_is_no_filter(cuda, determinist
     some = torch.full((1, C_, S_), 0.01, device=cuda)
     outs = []
     for kw in ({}, {"filter_3d": None}, {"filter_3d": zero}, {"filter_3d": some}):
-        P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+        P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
         img, st, _ = pipeline.render_view_forward(P, A[0], A[1], C["frustumplane"], C["view"], C["proj"], 3, hw, tile, clamp_zero=True,
                                                   antialiased=antialiased, **kw)
         d = torch.zeros_like(img)
@@ -156,11 +137,11 @@ def test_deterministic_backward_and_fewer_pairs(cuda, deterministic):
     shorter."""
     hw, tile = (96, 128), (8, 16)
     params, aabb, cam = small_scene(n=4000, hw=hw, tile=tile, seed=4, log_scale_range=(0.003, 0.05))
-    filt = torch.from_numpy(f3.compute_filter(params["xyz"], *_lattice(24, (36, 48)))[None]).to(cuda)
+    filt = torch.from_numpy(f3.compute_filter(params["xyz"], *lattice_cameras(24, (36, 48)))[None]).to(cuda)
     w = torch.from_numpy(np.random.default_rng(2).normal(size=(1, 3, *hw)).astype(np.float32)).to(cuda)
     runs = []
     for _ in range(2):
-        P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+        P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
         img, st, _ = pipeline.render_view_forward(P, A[0], A[1], C["frustumplane"], C["view"], C["proj"], 3, hw, tile, clamp_zero=True,
                                                   filter_3d=filt)
         d = torch.zeros_like(img)
@@ -181,7 +162,7 @@ def _setup_views(cuda, n=8000, hw=(72, 96), seed=6):
     A = [torch.from_numpy(p[k]).to(cuda) for k in ("cluster_origin", "cluster_extend")]
     cams = [{k: torch.from_numpy(x).to(cuda) for k, x in scene.make_camera(v, 12, hw[1], hw[0]).items()} for v in range(12)]
     w = torch.from_numpy(np.random.default_rng(0).normal(size=(1, 3, *hw)).astype(np.float32)).to(cuda)
-    views, projs, hws = (torch.from_numpy(a).to(cuda) for a in _lattice(12, (24, 32)))
+    views, projs, hws = (torch.from_numpy(a).to(cuda) for a in lattice_cameras(12, (24, 32)))
     F = scene.filter_3d_device(P["xyz"], views, projs, hws)
     return P, A, cams, w, F, (views, projs, hws)
 
@@ -296,11 +277,10 @@ def test_camera_gradient_matches_oracle(cuda, deterministic, deg, view, antialia
     params, aabb, cam, filt, w, o0 = _case(4000, hw, tile, deg, 12, antialiased, view=view)
     frag = o0["fragile"][:, :hw[0], :hw[1]]
     w = w * (~frag)[:, None]
-    ref = f3.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, antialiased=antialiased, filter_3d=filt)
-    ref64 = dict(ref, inter={k: v.astype(np.float64) for k, v in ref["inter"].items()}, d_ndc=ref["d_ndc"].astype(np.float64),
-                 d_cov=ref["d_cov"].astype(np.float64), G_aa=ref["G_aa"].astype(np.float64))
-    d_view, d_proj = aa.camera_backward(params, ref64, cam, hw)
-    P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+    ref = fo.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, antialiased=antialiased, filter_3d=filt)
+    ref64 = as_f64(ref)
+    d_view, d_proj = fo.camera_backward(params, ref64, cam, hw)
+    P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
     F = torch.from_numpy(filt).to(cuda)
     img, st, _ = pipeline.render_view_forward(P, A[0], A[1], C["frustumplane"], C["view"], C["proj"], deg, hw, tile, clamp_zero=True,
                                               antialiased=antialiased, filter_3d=F)
@@ -318,7 +298,7 @@ def test_camera_gradient_matches_oracle(cuda, deterministic, deg, view, antialia
 
 def _c2(cuda):
     p = scene.make_scene(1_000_000, sh_degree=3, seed=0, log_scale_range=(0.002, 0.02))
-    views, projs, hws = _lattice(24, (1080, 1920))
+    views, projs, hws = lattice_cameras(24, (1080, 1920))
     filt = f3.compute_filter(p["xyz"], views, projs, hws)[None]
     return p, filt
 
@@ -352,17 +332,17 @@ def test_c2_one_view_matches_oracle(cuda):
     H, W, tile, deg = 1080, 1920, (8, 16), 3
     p, filt = _c2(cuda)
     params = {k: p[k] for k in PARAM_KEYS}
-    got = _device_filter(p["xyz"], *_lattice(24, (H, W)), cuda).cpu().numpy()
+    got = _device_filter(p["xyz"], *lattice_cameras(24, (H, W)), cuda).cpu().numpy()
     assert np.array_equal(got.view(np.uint32), filt.view(np.uint32))
     aabb = scene.cluster_aabb(p["xyz"], p["scale"], p["rot"], filter_3d=filt)
     cam = scene.make_camera(0, 64, W, H)
     w = np.random.default_rng(7).normal(size=(1, 3, H, W)).astype(np.float32)
-    o0 = f3.render_forward_backward(params, aabb, cam, (H, W), tile, deg, lambda img: w, filter_3d=filt)
+    o0 = fo.render_forward_backward(params, aabb, cam, (H, W), tile, deg, lambda img: w, filter_3d=filt)
     print(f"C2 filter: f in [{filt.min():.2e}, {filt.max():.2e}], rho3 min {o0['rho3'].min():.3f}, "
           f"{(o0['rho3'] < 0.9).mean() * 100:.1f} % of the visible Gaussians below 0.9")
     frag = o0["fragile"][:, :H, :W].copy()
     assert frag.mean() < 0.10
-    P, A, C = _to_torch(params, aabb, cam, cuda)
+    P, A, C = to_torch(params, aabb, cam, cuda)
     F = torch.from_numpy(filt).to(cuda)
     _, st, _ = _forward(P, A, C, deg, (H, W), tile, False, F)
     D = o0["sorted_pid"].shape[1]
@@ -380,7 +360,7 @@ def test_c2_one_view_matches_oracle(cuda):
     frag |= on_stop(st.T.cpu().numpy()) | on_stop(o0["T"])
     assert np.array_equal(lc[~frag], lo[~frag])
     w = w * (~frag)[:, None]
-    ref = f3.render_forward_backward(params, aabb, cam, (H, W), tile, deg, lambda img: w, filter_3d=filt)
+    ref = fo.render_forward_backward(params, aabb, cam, (H, W), tile, deg, lambda img: w, filter_3d=filt)
     pp = PipelineParams(tile_size=tile)
     img = render.render_view(A[0], A[1], C["frustumplane"], C["view"], C["proj"], P["xyz"], P["scale"], P["rot"], P["sh_0"], P["sh_rest"],
                              P["opacity"], deg, (H, W), pp, filter_3d=F)[0]

@@ -13,19 +13,11 @@ from litegs_b200 import _lib, pipeline, render, scene
 from litegs_b200.arguments import PipelineParams
 from litegs_b200.dist import GradAccumulator
 from tests import filter3d_oracle as f3
-from tests import normal_oracle as nm
-from tests.test_gpu_exact_grad import _lattice
-from tests.test_gpu_pipeline import _to_torch
-from tests.util import PARAM_KEYS, differing_tiles, scaled_err, small_scene
+from tests import fused_oracle as fo
+from tests.util import (PARAM_KEYS, as_f64, deterministic, differing_tiles, lattice_cameras, restatement_mask, scaled_err,
+                        small_scene, to_torch)
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture
-def deterministic():
-    _lib.call("lgs_set_deterministic", 1)
-    yield
-    _lib.call("lgs_set_deterministic", 0)
 
 
 def _weights(hw, seed):
@@ -44,13 +36,13 @@ def test_fused_path_matches_restatement(cuda, deg, tile, antialiased, filtered):
     hw = (96, 128)
     depth = (deg == 3) == antialiased
     params, aabb, cam = small_scene(n=4000, hw=hw, tile=tile, sh_degree=3, seed=40 + deg, log_scale_range=(0.003, 0.05))
-    filt = f3.compute_filter(params["xyz"], *_lattice(24, (36, 48)))[None] if filtered else None
+    filt = f3.compute_filter(params["xyz"], *lattice_cameras(24, (36, 48)))[None] if filtered else None
     if filtered:
         aabb = scene.cluster_aabb(params["xyz"], params["scale"], params["rot"], filter_3d=filt)
     w, u, uz = _weights(hw, deg)
     kw = dict(antialiased=antialiased, filter_3d=filt, render_depth=depth)
-    o0 = nm.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, render_normal=True, **kw)
-    P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+    o0 = fo.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, render_normal=True, **kw)
+    P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
     F = None if filt is None else torch.from_numpy(filt).to(cuda)
     img, st, _ = pipeline.render_view_forward(P, A[0], A[1], C["frustumplane"], C["view"], C["proj"], deg, hw, tile, clamp_zero=True,
                                               antialiased=antialiased, filter_3d=F, render_depth=depth, render_normal=True)
@@ -66,24 +58,15 @@ def test_fused_path_matches_restatement(cuda, deg, tile, antialiased, filtered):
     assert clear.sum() > 0.9 * clear.size and np.array_equal(sg_gpu[clear], fr["sg"][clear])
     errs = {"normal_rec": np.abs(rec[:nvis * S, :3] - fr["n"].T)[clear].max()}
     assert not np.any(rec[:, 3]) and not np.any(rec[nvis * S:])
-    bad, _ = differing_tiles(st.ranges.cpu().numpy(), st.sorted_pid.cpu().numpy(), o0["ranges"], o0["sorted_pid"])
-    assert len(bad) <= 2
-    frag = o0["fragile"][:, :hw[0], :hw[1]].copy()
-    gx = -(-hw[1] // tile[1])
-    for t in bad:
-        ty, tx = divmod(int(t), gx)
-        frag[:, ty * tile[0]:(ty + 1) * tile[0], tx * tile[1]:(tx + 1) * tile[1]] = True
+    frag = restatement_mask(st, o0, hw, tile)
     ok = ~frag[:, None]
-    last = st.last.cpu().numpy()[..., :hw[0], :hw[1]]
-    assert np.array_equal(last[ok], o0["last"][..., :hw[0], :hw[1]][ok])
     ok3 = np.broadcast_to(ok, o0["normal"].shape)
     errs["N"] = np.abs(st.normal.cpu().numpy()[..., :hw[0], :hw[1]] - o0["normal"])[ok3].max()
     w, u, uz = w * ok, u * ok, uz * ok
-    ref = nm.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, render_normal=True,
+    ref = fo.render_forward_backward(params, aabb, cam, hw, tile, deg, lambda img: w, render_normal=True,
                                      d_normal_fn=lambda N, T: (u, None), d_depth_fn=(lambda D, T: (uz, None)) if depth else None, **kw)
-    ref64 = dict(ref, inter={k: x.astype(np.float64) for k, x in ref["inter"].items()}, d_ndc=ref["d_ndc"].astype(np.float64),
-                 d_cov=ref["d_cov"].astype(np.float64), G_aa=ref["G_aa"].astype(np.float64))
-    d_view, d_proj = nm.camera_backward(params, ref64, cam, hw, sh_degree=deg)
+    ref64 = as_f64(ref)
+    d_view, d_proj = fo.camera_backward(params, ref64, cam, hw, sh_degree=deg)
     d = torch.zeros_like(img)
     d[..., :hw[0], :hw[1]] = torch.from_numpy(w).to(cuda)
     cg = torch.empty((2, 4, 4), device=cuda)
@@ -101,7 +84,7 @@ def test_fused_path_matches_restatement(cuda, deg, tile, antialiased, filtered):
 
 def _render_grads(cuda, params, aabb, cam, hw, tile, pp, deg=3, u=None):
     """render_view + backward (a colour loss, plus sum u N when u is given) with the matrices as leaves -> dict of outputs."""
-    P, A, C = _to_torch(params, aabb, cam, cuda)
+    P, A, C = to_torch(params, aabb, cam, cuda)
     view, proj = C["view"].clone().requires_grad_(True), C["proj"].clone().requires_grad_(True)
     img, _, _, normal, last = render.render_view(A[0], A[1], C["frustumplane"], view, proj, P["xyz"], P["scale"], P["rot"], P["sh_0"],
                                                  P["sh_rest"], P["opacity"], deg, hw, pp)
@@ -243,7 +226,7 @@ def test_deterministic_and_statistics_modes(cuda, deterministic):
     N, the gradients and the camera gradient equal the statistics-off run to 1e-6 of their maximum."""
     hw, tile = (96, 128), (16, 16)
     params, aabb, cam = small_scene(n=4000, hw=hw, tile=tile, seed=11, log_scale_range=(0.003, 0.05))
-    P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+    P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
     w, u, _ = (torch.from_numpy(x).to(cuda) for x in _weights(hw, 1))
     a = _one_view(cuda, P, A, C, hw, tile, u, w)
     b = _one_view(cuda, P, A, C, hw, tile, u, w)
@@ -288,7 +271,7 @@ def test_refusals(cuda):
     Level A's render() refuses the flag; d_normal after a forward without normals is refused by the pipeline and the workspace."""
     hw, tile = (96, 128), (8, 16)
     params, aabb, cam = small_scene(n=2000, hw=hw, tile=tile, seed=2)
-    P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+    P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
     fwd = lambda: pipeline.render_view_forward(P, A[0], A[1], C["frustumplane"], C["view"], C["proj"], 3, hw, tile, clamp_zero=True,
                                                render_normal=True)
     img, st, _ = fwd()
@@ -331,7 +314,7 @@ def test_workspace_clears_stale_normal_gradient_padding(cuda, deterministic):
     so a stale padded [Hp,Wp] gradient of an earlier call does not leak into the next backward."""
     hw, tile = (90, 120), (16, 16)
     params, aabb, cam = small_scene(n=3000, hw=hw, tile=tile, seed=8)
-    P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+    P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
     ws = pipeline.ViewWorkspace(P, hw, tile, pair_capacity=1 << 20, use_graphs=False)
     acc = GradAccumulator(P)
     w = torch.randn((1, 3, *hw), device=cuda)
@@ -420,10 +403,10 @@ def test_c2_one_view_matches_restatement(cuda):
     g = np.random.default_rng(7)
     w, u, uz = (g.normal(size=(1, 3, H, W)).astype(np.float32), g.normal(size=(1, 3, H, W)).astype(np.float32),
                 g.normal(size=(1, 1, H, W)).astype(np.float32))
-    o0 = nm.render_forward_backward(params, aabb, cam, (H, W), tile, deg, lambda img: w, render_normal=True, render_depth=True)
+    o0 = fo.render_forward_backward(params, aabb, cam, (H, W), tile, deg, lambda img: w, render_normal=True, render_depth=True)
     frag = o0["fragile"][:, :H, :W].copy()
     assert frag.mean() < 0.10
-    P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+    P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
     img, st, _ = pipeline.render_view_forward(P, A[0], A[1], C["frustumplane"], C["view"], C["proj"], deg, (H, W), tile, clamp_zero=True,
                                               render_depth=True, render_normal=True)
     bad, npairs = differing_tiles(st.ranges.cpu().numpy(), st.sorted_pid.cpu().numpy(), o0["ranges"], o0["sorted_pid"])
@@ -449,16 +432,15 @@ def test_c2_one_view_matches_restatement(cuda):
     freeze = dict(a=fr["a"], sg=sg_gpu)
     ok = ~frag[:, None]
     w, u, uz = w * ok, u * ok, uz * ok
-    ref = nm.render_forward_backward(params, aabb, cam, (H, W), tile, deg, lambda img: w, render_normal=True, render_depth=True,
+    ref = fo.render_forward_backward(params, aabb, cam, (H, W), tile, deg, lambda img: w, render_normal=True, render_depth=True,
                                      d_normal_fn=lambda N_, T_: (u, None), d_depth_fn=lambda D_, T_: (uz, None), normal_freeze=freeze)
     ok3 = np.broadcast_to(ok, ref["normal"].shape)
     errs = {"img": np.abs(img.cpu().numpy()[..., :H, :W] - ref["img"])[np.broadcast_to(ok, ref["img"].shape)].max(),
             "normal_rec": np.abs(rec - ref["frame"]["n"].T).max(),
             "N": np.abs(st.normal.cpu().numpy()[..., :H, :W] - ref["normal"])[ok3].max(),
             "D": np.abs(st.depth.cpu().numpy()[..., :H, :W] - ref["depth"])[ok].max() / np.abs(ref["depth"]).max()}
-    ref64 = dict(ref, inter={k: x.astype(np.float64) for k, x in ref["inter"].items()}, d_ndc=ref["d_ndc"].astype(np.float64),
-                 d_cov=ref["d_cov"].astype(np.float64), G_aa=ref["G_aa"].astype(np.float64))
-    d_view, d_proj = nm.camera_backward(params, ref64, cam, (H, W), sh_degree=deg)
+    ref64 = as_f64(ref)
+    d_view, d_proj = fo.camera_backward(params, ref64, cam, (H, W), sh_degree=deg)
     d = torch.zeros_like(img)
     d[..., :H, :W] = torch.from_numpy(w).to(cuda)
     cg = torch.empty((2, 4, 4), device=cuda)

@@ -8,7 +8,7 @@ import torch
 
 import oracle
 from litegs_b200 import fused
-from tests.util import oracle_projected, rel_err, scaled_err, small_scene
+from tests.util import oracle_projected, raster_case, rel_err, scaled_err, small_scene
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-4
@@ -119,37 +119,7 @@ def test_binning_bit_exact(cuda, proj, tile):
     assert np.array_equal(rng_.cpu().numpy(), oracle.tileRange(okeys, gx * gy, fix_last=True))
 
 
-def _raster_case(cuda, proj, tile, staging):
-    from litegs_b200 import _lib
-    _lib.call("lgs_set_staging", 1 if staging == "bulk" else 0)
-    o, hw = proj["o"], proj["hw"]
-    th, tw = tile
-    ranges, sorted_pid, _, _ = oracle.binning(o["ndc"], o["view_pos"][:, 2], o["inv_cov2d"], o["opacity"], None, hw, tile)
-    oimg, oT, olast, _, _, fragile = oracle.rasterize_forward(sorted_pid, ranges, o["ndc"], o["inv_cov2d"], o["color"], o["opacity"], None,
-                                                               hw[0], hw[1], th, tw, fragile_eps=2e-6)
-    out = fused.rasterize_forward(T(sorted_pid, cuda), T(ranges, cuda), T(o["ndc"], cuda), T(o["inv_cov2d"], cuda), T(o["color"], cuda),
-                                  T(o["opacity"], cuda), None, hw[0], hw[1], th, tw, False, False, False)
-    img, Tr, _, last, packed, _, _ = out
-    ok = ~fragile
-    assert fragile.mean() < 0.02
-    assert np.array_equal(last.cpu().numpy()[:, 0][ok], olast[:, 0][ok])
-    m3 = np.broadcast_to(ok[:, None], oimg.shape)
-    assert rel_err(img.cpu().numpy()[m3], oimg[m3]) < TOL
-    assert rel_err(Tr.cpu().numpy()[:, 0][ok], oT[:, 0][ok]) < TOL
-    # backward, fed with the ORACLE's forward state so that only the backward kernel is under test
-    rng = np.random.default_rng(1)
-    g = rng.normal(size=oimg.shape).astype(np.float32)
-    g[np.broadcast_to(fragile[:, None], g.shape)] = 0.0
-    gmax = np.abs(g).max()
-    ref = oracle.rasterize_backward(sorted_pid, ranges, o["ndc"], o["inv_cov2d"], o["color"], o["opacity"], None, oT, olast,
-                                    g / gmax, None, gmax, hw[0], hw[1], th, tw)
-    got = fused.rasterize_backward(T(sorted_pid, cuda), T(ranges, cuda), packed, None, T(oT, cuda), T(olast, cuda), T(g / gmax, cuda),
-                                   None, None, torch.tensor([gmax], device=cuda), hw[0], hw[1], th, tw, False)
-    for a, b, name in zip(got[:4], ref[:4], ("d_ndc", "d_cov2d_inv", "d_color", "d_opacity")):
-        assert scaled_err(a.cpu().numpy(), b) < TOL, (name, scaled_err(a.cpu().numpy(), b))
-
-
 @pytest.mark.parametrize("staging", ["bulk", "cpasync"])
 @pytest.mark.parametrize("tile", [(16, 16), (8, 16), (12, 16), (8, 8)])
 def test_raster_forward_backward(cuda, proj, tile, staging):
-    _raster_case(cuda, proj, tile, staging)
+    raster_case(cuda, proj, tile, staging)

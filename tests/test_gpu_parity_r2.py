@@ -9,7 +9,7 @@ import torch
 import oracle
 from litegs_b200 import _lib, fused, render, wrapper
 from litegs_b200.arguments import PipelineParams
-from tests.util import PARAM_KEYS, oracle_projected, rel_err, scaled_err, small_scene
+from tests.util import PARAM_KEYS, oracle_projected, raster_case, rel_err, scaled_err, small_scene
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-4
@@ -176,10 +176,9 @@ def _lists(proj, tile):
 @pytest.mark.parametrize("tile", [(8, 16), (16, 16), (12, 16), (8, 8)])
 def test_raster_backward_kernels_default_flags(cuda, proj, tile, bwd):
     """Both backward kernels (scalar v1, packed-pair v2) against the oracle on the oracle's own forward state."""
-    from tests.test_gpu_ops import _raster_case
     _lib.call("lgs_set_backward_kernel", bwd)
     try:
-        _raster_case(cuda, proj, tile, "cpasync")
+        raster_case(cuda, proj, tile, "cpasync")
     finally:
         _lib.call("lgs_set_backward_kernel", 2)
 

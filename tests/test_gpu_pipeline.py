@@ -8,29 +8,10 @@ import torch
 import oracle
 from litegs_b200 import fused, render
 from litegs_b200.arguments import PipelineParams
-from tests.util import PARAM_KEYS, scaled_err, small_scene
+from tests.util import PARAM_KEYS, oracle_case, scaled_err, small_scene, to_torch
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-4
-
-
-def _to_torch(params, aabb, cam, dev, grad=True):
-    P = {k: torch.from_numpy(params[k]).to(dev).requires_grad_(grad) for k in PARAM_KEYS}
-    A = [torch.from_numpy(a).to(dev) for a in aabb]
-    C = {k: torch.from_numpy(v).to(dev) for k, v in cam.items()}
-    return P, A, C
-
-
-def _case(n, hw, tile, sh_degree, seed, view=0, scale_range=(0.02, 0.08)):
-    params, aabb, cam = small_scene(n=n, hw=hw, tile=tile, sh_degree=3, seed=seed, view=view, log_scale_range=scale_range)
-    rng = np.random.default_rng(seed + 100)
-    w = rng.normal(size=(1, 3, hw[0], hw[1])).astype(np.float32)
-    # first pass to find fragile pixels, then zero the loss weight there
-    o0 = oracle.render_forward_backward(params, aabb, cam, hw, tile, sh_degree, lambda img: w)
-    frag = o0["fragile"][:, : hw[0], : hw[1]]
-    w = w * (~frag)[:, None]
-    ref = oracle.render_forward_backward(params, aabb, cam, hw, tile, sh_degree, lambda img: w)
-    return params, aabb, cam, w, frag, ref
 
 
 def _check(img, grads, nvis, ref, frag, what):
@@ -48,13 +29,13 @@ def _check(img, grads, nvis, ref, frag, what):
                                                  # BASELINE.json configs[0] ("C1"): 10k Gaussians, 256 x 256, one view
                                                  ((8, 16), 3, 10000, (256, 256)), ((12, 16), 3, 10000, (256, 256))])
 def test_level_a_and_b_match_oracle(cuda, tile, sh_degree, n, hw):
-    params, aabb, cam, w, frag, ref = _case(n, hw, tile, sh_degree, seed=11)
+    params, aabb, cam, w, frag, ref = oracle_case(n, hw, tile, sh_degree, seed=11)
     nvis = int(ref["visible_chunk_id"].shape[0])
     pp = PipelineParams(tile_size=tile)
     wt = torch.from_numpy(w).to(cuda)
 
     # Level A
-    P, A, C = _to_torch(params, aabb, cam, cuda)
+    P, A, C = to_torch(params, aabb, cam, cuda)
     ids, num, cx, cs, cr, col, cop = render.render_preprocess(A[0], A[1], C["frustumplane"], C["view"], P["xyz"], P["scale"], P["rot"],
                                                               P["sh_0"], P["sh_rest"], P["opacity"], None, None, pp, sh_degree)
     assert int(num.item()) == nvis and np.array_equal(ids.cpu().numpy()[:nvis], ref["visible_chunk_id"])
@@ -64,7 +45,7 @@ def test_level_a_and_b_match_oracle(cuda, tile, sh_degree, n, hw):
     _check(img.detach().cpu().numpy(), grads, nvis, ref, frag, "levelA")
 
     # Level B
-    P2, A2, C2 = _to_torch(params, aabb, cam, cuda)
+    P2, A2, C2 = to_torch(params, aabb, cam, cuda)
     img2, _, _, _, last2 = render.render_view(A2[0], A2[1], C2["frustumplane"], C2["view"], C2["proj"], P2["xyz"], P2["scale"], P2["rot"],
                                               P2["sh_0"], P2["sh_rest"], P2["opacity"], sh_degree, hw, pp)
     (img2 * wt).sum().backward()
@@ -83,7 +64,7 @@ def test_fused_pairs_match_oracle_lists(cuda, hw, tile, n, scales):
     """The fused pipeline's per-tile splat lists equal the oracle's (identical order) on a seeded scene."""
     from litegs_b200 import pipeline
     params, aabb, cam = small_scene(n=n, hw=hw, seed=3, log_scale_range=scales)
-    P, A, C = _to_torch(params, aabb, cam, cuda, grad=False)
+    P, A, C = to_torch(params, aabb, cam, cuda, grad=False)
     img, st, _ = pipeline.render_view_forward(P, A[0], A[1], C["frustumplane"], C["view"], C["proj"], 3, hw, tile)
     from tests.util import oracle_projected
     o = oracle_projected(params, aabb, cam, hw, 3)
@@ -105,7 +86,7 @@ def test_partially_visible_scene_dense_grads(cuda):
     w = torch.from_numpy(np.random.default_rng(0).normal(size=(1, 3, *hw)).astype(np.float32)).to(cuda)
     out = []
     for level in ("A", "B"):
-        P, A, C = _to_torch(params, aabb, cam, cuda)
+        P, A, C = to_torch(params, aabb, cam, cuda)
         if level == "A":
             ids, num, cx, cs, cr, col, cop = render.render_preprocess(A[0], A[1], C["frustumplane"], C["view"], P["xyz"], P["scale"], P["rot"],
                                                                       P["sh_0"], P["sh_rest"], P["opacity"], None, None, pp, 1)
@@ -130,7 +111,7 @@ def test_empty_view_renders_black(cuda):
     Pm = scene.proj_matrix(hw[1], hw[0])
     cam = dict(view=V[None], proj=Pm[None], frustumplane=scene.frustum_planes(V, Pm)[None])
     params = {k: p[k] for k in PARAM_KEYS}
-    P, A, C = _to_torch(params, (p["cluster_origin"], p["cluster_extend"]), cam, cuda)
+    P, A, C = to_torch(params, (p["cluster_origin"], p["cluster_extend"]), cam, cuda)
     pp = PipelineParams(tile_size=tile, sparse_grad=False)
     img = render.render_view(A[0], A[1], C["frustumplane"], C["view"], C["proj"], P["xyz"], P["scale"], P["rot"], P["sh_0"], P["sh_rest"],
                              P["opacity"], 0, hw, pp)[0]
@@ -150,7 +131,7 @@ def test_accumulate_into_dense_buffers_equals_sum_of_views(cuda):
     aabb = (p["cluster_origin"], p["cluster_extend"])
     pp = PipelineParams(tile_size=tile, sparse_grad=True)
     w = torch.from_numpy(np.random.default_rng(0).normal(size=(1, 3, *hw)).astype(np.float32)).to(cuda)
-    P, A, _ = _to_torch(params, aabb, scene.make_camera(0, 8, hw[1], hw[0]), cuda)
+    P, A, _ = to_torch(params, aabb, scene.make_camera(0, 8, hw[1], hw[0]), cuda)
     acc = GradAccumulator(P)
     dense_ref = {k: torch.zeros_like(P[k]) for k in PARAM_KEYS}
     for v in (0, 3, 5):
@@ -179,7 +160,7 @@ def test_render_views_streams_match_serial(cuda):
     p = scene.make_scene(8000, sh_degree=3, cube=1.5, seed=6, log_scale_range=(0.02, 0.08))
     params = {k: p[k] for k in PARAM_KEYS}
     pp = PipelineParams(tile_size=tile)
-    P, A, _ = _to_torch(params, (p["cluster_origin"], p["cluster_extend"]), scene.make_camera(0, 8, hw[1], hw[0]), cuda)
+    P, A, _ = to_torch(params, (p["cluster_origin"], p["cluster_extend"]), scene.make_camera(0, 8, hw[1], hw[0]), cuda)
     cams = [{k: torch.from_numpy(x).to(cuda) for k, x in scene.make_camera(v, 8, hw[1], hw[0]).items()} for v in range(6)]
     w = torch.from_numpy(np.random.default_rng(0).normal(size=(1, 3, *hw)).astype(np.float32)).to(cuda)
     res = []

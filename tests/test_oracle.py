@@ -6,28 +6,18 @@ import pytest
 
 import oracle
 from litegs_b200 import scene
-from tests.util import PARAM_KEYS, oracle_projected, small_scene
+from tests.util import f64_arrays, oracle_projected, small_scene, tiny_scene
 
 
-def _f64(d):
-    return {k: (v.astype(np.float64) if isinstance(v, np.ndarray) and v.dtype == np.float32 else v) for k, v in d.items()}
-
-
-def _tiny(seed=3, n=48, hw=(32, 32), chunk=16, deg=2):
-    p = scene.make_scene(n, sh_degree=deg, chunk=chunk, log_scale_range=(0.05, 0.2), seed=seed)
-    cam = _f64(scene.make_camera(1, 8, hw[1], hw[0]))
-    P = {k: p[k].astype(np.float64) for k in PARAM_KEYS}
-    P["opacity"] = np.clip(P["opacity"], -1, 1.5)       # keep away from the 255/256 clamp
-    P["sh_0"] *= 0.3; P["sh_rest"] *= 0.3               # keep colours inside (0,1): min(c,1) is not differentiable
-    aabb = (p["cluster_origin"].astype(np.float64), p["cluster_extend"].astype(np.float64))
-    return P, aabb, cam
+def _tiny(seed=3):
+    return tiny_scene(seed=seed, log_scale_range=(0.05, 0.2))
 
 
 def test_dense_numpy_rasterizer_agrees():
     """Per-pixel front-to-back compositing written independently in numpy (Appendix A items 12)."""
     hw, tile = (24, 32), (8, 8)
     params, aabb, cam = small_scene(n=300, hw=hw, tile=tile, sh_degree=1, seed=2, log_scale_range=(0.05, 0.15))
-    o = oracle_projected(_f64(params), tuple(a.astype(np.float64) for a in aabb), _f64(cam), hw, 1)
+    o = oracle_projected(f64_arrays(params), tuple(a.astype(np.float64) for a in aabb), f64_arrays(cam), hw, 1)
     ranges, pid, _, _ = oracle.binning(o["ndc"], o["view_pos"][:, 2], o["inv_cov2d"], o["opacity"], None, hw, tile)
     img, T, last, *_ = oracle.rasterize_forward(pid, ranges, o["ndc"], o["inv_cov2d"], o["color"], o["opacity"], None, hw[0], hw[1], *tile)
     H, W = hw
@@ -115,7 +105,7 @@ def test_fp32_and_fp64_oracles_agree():
     params, aabb, cam = small_scene(n=800, hw=hw, seed=4)
     w = np.random.default_rng(0).normal(size=(1, 3, *hw))
     a = oracle.render_forward_backward(params, aabb, cam, hw, tile, 3, lambda img: w.astype(np.float32))
-    b = oracle.render_forward_backward(_f64(params), tuple(x.astype(np.float64) for x in aabb), _f64(cam), hw, tile, 3, lambda img: w)
+    b = oracle.render_forward_backward(f64_arrays(params), tuple(x.astype(np.float64) for x in aabb), f64_arrays(cam), hw, tile, 3, lambda img: w)
     if a["sorted_pid"].shape == b["sorted_pid"].shape and np.array_equal(a["sorted_pid"], b["sorted_pid"]):
         ok = ~(a["fragile"] | b["fragile"])[:, None, : hw[0], : hw[1]]
         ok = np.broadcast_to(ok, a["img"].shape)

@@ -1,5 +1,6 @@
-"""The antialiased mode on the CPU (fp64 restatement in tests/aa_oracle.py): its gradients against central finite differences,
-the off switch, the range of rho, the integrated alpha of one splat and the consistency of renders across resolutions."""
+"""The antialiased mode on the CPU (fp64 restatement in tests/aa_oracle.py, composed by tests/fused_oracle.py): its gradients
+against central finite differences, the off switch, the range of rho, the integrated alpha of one splat and the consistency of
+renders across resolutions."""
 import math
 
 import numpy as np
@@ -9,22 +10,8 @@ import oracle
 from litegs_b200 import scene
 from tests import aa_oracle as aa
 from tests import camera_oracle as co
-from tests.util import PARAM_KEYS, small_scene
-
-
-def _f64(d):
-    return {k: (v.astype(np.float64) if isinstance(v, np.ndarray) and v.dtype == np.float32 else v) for k, v in d.items()}
-
-
-def _tiny(seed=3, n=48, hw=(32, 32), chunk=16, deg=2):
-    """Like test_oracle's tiny scene, with scales down to a third of a pixel so that rho ranges widely."""
-    p = scene.make_scene(n, sh_degree=deg, chunk=chunk, log_scale_range=(0.03, 0.2), seed=seed)
-    cam = _f64(scene.make_camera(1, 8, hw[1], hw[0]))
-    P = {k: p[k].astype(np.float64) for k in PARAM_KEYS}
-    P["opacity"] = np.clip(P["opacity"], -1, 1.5)       # keep away from the 0.99 clamp
-    P["sh_0"] *= 0.3; P["sh_rest"] *= 0.3               # keep colours inside (0,1): min(c,1) is not differentiable
-    aabb = (p["cluster_origin"].astype(np.float64), p["cluster_extend"].astype(np.float64))
-    return P, aabb, cam
+from tests import fused_oracle as fo
+from tests.util import PARAM_KEYS, f64_arrays, single_splat, small_scene, tiny_scene
 
 
 HW, TILE, DEG = (32, 32), (8, 8), 2
@@ -35,14 +22,14 @@ def test_fp64_finite_differences_with_frozen_lists(true_sigmoid):
     """scale, rot, sh and opacity: the analytic gradients of the antialiased render equal fp64 central differences of the same
     render with the tile lists frozen.  Under the reference's convention (true_sigmoid False) the opacity gradient is the true
     one divided by 1 - sigma (SURVEY Q15), and the check divides it out."""
-    P, aabb, cam = _tiny()
+    P, aabb, cam = tiny_scene()
     rng = np.random.default_rng(1)
     w = rng.normal(size=(1, 3, *HW))
-    out = aa.render_forward_backward(P, aabb, cam, HW, TILE, DEG, lambda img: w, true_sigmoid_grad=true_sigmoid, antialiased=True)
+    out = fo.render_forward_backward(P, aabb, cam, HW, TILE, DEG, lambda img: w, true_sigmoid_grad=true_sigmoid, antialiased=True)
     assert out["rho"].min() < 0.5 and out["rho"].max() > 0.8           # sub-pixel and larger splats both present
     lists = (out["ranges"], out["sorted_pid"])
     ids = out["visible_chunk_id"]
-    run = lambda Q: (aa.render_forward_backward(Q, aabb, cam, HW, TILE, DEG, lambda img: w, antialiased=True, lists=lists)["img"] * w).sum()
+    run = lambda Q: (fo.render_forward_backward(Q, aabb, cam, HW, TILE, DEG, lambda img: w, antialiased=True, lists=lists)["img"] * w).sum()
     sig = 1 / (1 + np.exp(-P["opacity"]))
     checked = 0
     for name in ("scale", "rot", "sh_0", "sh_rest", "opacity"):
@@ -65,17 +52,17 @@ def test_fp64_finite_differences_with_frozen_lists(true_sigmoid):
 def test_fp64_finite_differences_xyz_with_frozen_J_and_dirs():
     """xyz: with J, the SH directions and the tile lists frozen, the analytic d xyz of the antialiased render equals central
     differences.  J frozen makes Sigma2 and so rho independent of the position: the gradient flows through the NDC mean only."""
-    P, aabb, cam = _tiny(seed=5)
+    P, aabb, cam = tiny_scene(seed=5)
     rng = np.random.default_rng(2)
     w = rng.normal(size=(1, 3, *HW))
-    out = aa.render_forward_backward(P, aabb, cam, HW, TILE, DEG, lambda img: w, true_sigmoid_grad=True, antialiased=True)
+    out = fo.render_forward_backward(P, aabb, cam, HW, TILE, DEG, lambda img: w, true_sigmoid_grad=True, antialiased=True)
     freeze = dict(J=out["inter"]["J"], color=out["color"])
     lists = (out["ranges"], out["sorted_pid"])
     ids = out["visible_chunk_id"]
     g = out["grads"]["xyz"]
 
     def loss(Q):
-        return (aa.render_forward_backward(Q, aabb, cam, HW, TILE, DEG, lambda img: w, antialiased=True, lists=lists,
+        return (fo.render_forward_backward(Q, aabb, cam, HW, TILE, DEG, lambda img: w, antialiased=True, lists=lists,
                                            freeze=freeze)["img"] * w).sum()
 
     for _ in range(10):
@@ -88,18 +75,18 @@ def test_fp64_finite_differences_xyz_with_frozen_J_and_dirs():
 
 
 def test_camera_gradient_matches_finite_differences_with_frozen_J_and_dirs():
-    """The camera gradient with the antialiasing term (aa_oracle.camera_backward) against central differences of the view and
+    """The camera gradient with the antialiasing term (fused_oracle.camera_backward) against central differences of the view and
     projection matrices, J, SH directions and tile lists frozen."""
-    P, aabb, cam = _tiny(seed=5)
+    P, aabb, cam = tiny_scene(seed=5)
     w = np.random.default_rng(2).normal(size=(1, 3, *HW))
-    out = aa.render_forward_backward(P, aabb, cam, HW, TILE, DEG, lambda img: w, true_sigmoid_grad=True, antialiased=True)
+    out = fo.render_forward_backward(P, aabb, cam, HW, TILE, DEG, lambda img: w, true_sigmoid_grad=True, antialiased=True)
     freeze = dict(J=out["inter"]["J"], color=out["color"])
     lists = (out["ranges"], out["sorted_pid"])
-    d_view, d_proj = aa.camera_backward(P, out, cam, HW)
+    d_view, d_proj = fo.camera_backward(P, out, cam, HW)
 
     def loss(view, proj):
         c = dict(cam, view=view, proj=proj)
-        return (aa.render_forward_backward(P, aabb, c, HW, TILE, DEG, lambda img: w, antialiased=True, lists=lists,
+        return (fo.render_forward_backward(P, aabb, c, HW, TILE, DEG, lambda img: w, antialiased=True, lists=lists,
                                            freeze=freeze)["img"] * w).sum()
 
     h = 1e-6
@@ -121,18 +108,18 @@ def test_camera_gradient_matches_finite_differences_with_frozen_J_and_dirs():
 
 @pytest.mark.parametrize("dt", [np.float32, np.float64])
 def test_off_means_unchanged(dt):
-    """antialiased=False: the composition in aa_oracle returns the oracle's own outputs bit for bit.  One oracle thread: the
+    """antialiased=False: the composition in fused_oracle returns the oracle's own outputs bit for bit.  One oracle thread: the
     raster backward's per-splat sums are run-to-run reproducible only then."""
     hw, tile = (48, 64), (16, 16)
     params, aabb, cam = small_scene(n=800, hw=hw, seed=4)
     if dt == np.float64:
-        params, aabb, cam = _f64(params), tuple(a.astype(np.float64) for a in aabb), _f64(cam)
+        params, aabb, cam = f64_arrays(params), tuple(a.astype(np.float64) for a in aabb), f64_arrays(cam)
     w = np.random.default_rng(0).normal(size=(1, 3, *hw)).astype(dt)
     nt = oracle.num_threads()
     oracle.set_num_threads(1)
     try:
         a = oracle.render_forward_backward(params, aabb, cam, hw, tile, 3, lambda img: w, true_sigmoid_grad=True)
-        b = aa.render_forward_backward(params, aabb, cam, hw, tile, 3, lambda img: w, true_sigmoid_grad=True, antialiased=False)
+        b = fo.render_forward_backward(params, aabb, cam, hw, tile, 3, lambda img: w, true_sigmoid_grad=True, antialiased=False)
     finally:
         oracle.set_num_threads(nt)
     for k in ("img", "T", "last", "fragile", "ranges", "sorted_pid", "d_ndc", "d_cov", "d_col", "d_op"):
@@ -168,26 +155,6 @@ def test_rho_range():
     assert rho[0] == 0 and d_o[0, 0] == 0 and np.all(G == 0)
 
 
-def single_splat(std_px, hw=(64, 64), opacity=0.8, chunk=16, dt=np.float64):
-    """One splat on the optical axis, isotropic with the given standard deviation in pixels before the filter, plus chunk - 1
-    invisible companions (opacity far below 1/255).  -> (params, aabb, cam)."""
-    H, W = hw
-    recp = 1.0 / math.tan(math.radians(30.0))
-    view, proj, _, planes = co.create_viewproj_forward(np.array([[1.0, 0, 0, 0, 0, 0, 0]]), np.array([recp]), H, W, 0.01, 100.0)
-    z = 5.0
-    fx = recp * W * 0.5
-    s = std_px * z / fx
-    n = chunk
-    xyz = np.zeros((3, 1, n)); xyz[2] = z
-    P = dict(xyz=xyz, scale=np.full((3, 1, n), math.log(s)), rot=np.tile(np.array([1.0, 0, 0, 0])[:, None, None], (1, 1, n)),
-             sh_0=np.full((1, 3, 1, n), 0.5), sh_rest=np.zeros((0, 3, 1, n)), opacity=np.full((1, 1, n), -30.0))
-    P["opacity"][0, 0, 0] = math.log(opacity / (1 - opacity))
-    P = {k: v.astype(dt) for k, v in P.items()}
-    aabb = (np.array([[0.0], [0.0], [z]], dt), np.full((3, 1), 10 * s, dt))
-    cam = dict(view=view.astype(dt), proj=proj.astype(dt), frustumplane=planes.astype(dt))
-    return P, aabb, cam
-
-
 @pytest.mark.parametrize("std_px", [0.35, 0.7, 1.5, 3.0])
 def test_integrated_alpha_of_one_splat(std_px):
     """With the compensation, a splat's alpha summed over the pixels equals the integral of the unfiltered Gaussian, o 2 pi
@@ -196,7 +163,7 @@ def test_integrated_alpha_of_one_splat(std_px):
     hw = (64, 64)
     P, aabb, cam = single_splat(std_px, hw)
     for on in (True, False):
-        out = aa.render_forward_backward(P, aabb, cam, hw, (16, 16), 0, lambda img: np.zeros_like(img), antialiased=on)
+        out = fo.render_forward_backward(P, aabb, cam, hw, (16, 16), 0, lambda img: np.zeros_like(img), antialiased=on)
         o_act = 1 / (1 + np.exp(-P["opacity"].reshape(1, -1)))
         _, rho, f = aa.antialias_forward(aa.cov_M(out["inter"], cam["view"]), o_act)
         o, oe = float(o_act[0, 0]), float(o_act[0, 0] * rho[0])
@@ -225,7 +192,7 @@ def test_resolution_consistency():
         imgs = {}
         for hw in (lo, hi):
             cam = scene.make_camera(0, 8, hw[1], hw[0])
-            out = aa.render_forward_backward(P, aabb, cam, hw, (16, 16), 0, lambda img: np.zeros_like(img), antialiased=on)
+            out = fo.render_forward_backward(P, aabb, cam, hw, (16, 16), 0, lambda img: np.zeros_like(img), antialiased=on)
             imgs[hw] = out["img"][0].astype(np.float64)
         pooled = imgs[hi].reshape(3, lo[0], k, lo[1], k).mean(axis=(2, 4))
         err[on] = float(np.abs(pooled - imgs[lo]).mean())

@@ -9,7 +9,7 @@ import pytest
 import oracle
 from litegs_b200 import colmap, scene
 from tests import camera_oracle as co
-from tests.test_oracle import _tiny
+from tests.util import tiny_scene
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "viewproj.npz")
 ZN, ZF = 0.01, 5000.0
@@ -95,7 +95,7 @@ def test_oracle_matches_the_reference_fixture():
 
 
 def _render_case(seed=5):
-    P, aabb, cam = _tiny(seed=seed)
+    P, aabb, cam = tiny_scene(seed=seed, log_scale_range=(0.05, 0.2))
     hw, tile = (32, 32), (8, 8)
     w = np.random.default_rng(2).normal(size=(1, 3, 32, 32))
     out = oracle.render_forward_backward(P, aabb, cam, hw, tile, 2, lambda img: w, true_sigmoid_grad=True)

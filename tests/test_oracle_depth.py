@@ -1,13 +1,14 @@
-"""The depth mode on the CPU (numpy restatement in tests/depth_oracle.py): the gradients of a loss in D and of a loss in the
-expected depth ED = D / (1 - T) against fp64 central differences with the tile lists frozen, in the default convention (J and the
-SH directions frozen as well) and in the exact mode (nothing else frozen); what the mode leaves unchanged."""
+"""The depth mode on the CPU (numpy restatement in tests/depth_oracle.py, composed by tests/fused_oracle.py): the gradients of a
+loss in D and of a loss in the expected depth ED = D / (1 - T) against fp64 central differences with the tile lists frozen, in the
+default convention (J and the SH directions frozen as well) and in the exact mode (nothing else frozen); what the mode leaves
+unchanged."""
 import numpy as np
 import pytest
 
 import oracle
-from tests import aa_oracle as aa
 from tests import depth_oracle as dp
-from tests.test_oracle_antialias import _tiny
+from tests import fused_oracle as fo
+from tests.util import tiny_scene
 
 HW, TILE = (32, 32), (8, 8)
 TOL = 1e-4
@@ -18,7 +19,7 @@ def _close(fd, g):
 
 
 def _scene(deg, filtered):
-    P, aabb, cam = _tiny(seed=5, deg=max(deg, 1))
+    P, aabb, cam = tiny_scene(seed=5, deg=max(deg, 1))
     if deg == 0:
         P["sh_rest"] = P["sh_rest"][:0]
     filt = np.random.default_rng(1).uniform(0.02, 0.12, (1, *P["xyz"].shape[-2:])) if filtered else None
@@ -51,7 +52,7 @@ def test_fp64_finite_differences(deg, antialiased, filtered, kind):
     u = rng.normal(size=(1, 1, *HW))
     true_sigmoid = bool(antialiased)
     kw = dict(antialiased=antialiased, filter_3d=filt)
-    base = dp.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, render_depth=True, **kw)
+    base = fo.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, render_depth=True, **kw)
     mask = (1 - base["T"][..., :HW[0], :HW[1]]) > 0.2
     dloss, dgrad = _losses(kind, u, mask)
     lists = (base["ranges"], base["sorted_pid"])
@@ -59,11 +60,11 @@ def test_fp64_finite_differences(deg, antialiased, filtered, kind):
     assert np.abs(base["depth"]).max() > 1.0           # no clamp: depths well above 1 are present
 
     def run(Q, c=cam, freeze=None):
-        o = dp.render_forward_backward(Q, aabb, c, HW, TILE, deg, lambda img: w, render_depth=True, lists=lists, freeze=freeze, **kw)
+        o = fo.render_forward_backward(Q, aabb, c, HW, TILE, deg, lambda img: w, render_depth=True, lists=lists, freeze=freeze, **kw)
         return (o["img"] * w).sum() + dloss(o["depth"], o["T"][..., :HW[0], :HW[1]])
 
     h = 1e-6
-    out = dp.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, render_depth=True, d_depth_fn=dgrad,
+    out = fo.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, render_depth=True, d_depth_fn=dgrad,
                                      true_sigmoid_grad=true_sigmoid, **kw)
     assert np.abs(out["dz"]).max() > 0
     sig = 1 / (1 + np.exp(-P["opacity"]))
@@ -80,7 +81,7 @@ def test_fp64_finite_differences(deg, antialiased, filtered, kind):
             want = g[idx] * ((1 - sig[full]) if name == "opacity" and not true_sigmoid else 1.0)
             assert _close(fd, want), (name, idx, fd, want)
     for exact in (False, True):
-        o = dp.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, render_depth=True, d_depth_fn=dgrad,
+        o = fo.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, render_depth=True, d_depth_fn=dgrad,
                                        true_sigmoid_grad=True, exact_grad=exact, **kw)
         freeze = None if exact else dict(J=o["inter"]["J"], color=o["color"])
         g = o["grads"]["xyz"]
@@ -90,7 +91,7 @@ def test_fp64_finite_differences(deg, antialiased, filtered, kind):
             Pm = {k: v.copy() for k, v in P.items()}; Pm["xyz"][c, ids[a], s] -= h
             fd = (run(Pp, freeze=freeze) - run(Pm, freeze=freeze)) / (2 * h)
             assert _close(fd, g[c, a, s]), ("xyz", exact, fd, g[c, a, s])
-        d_view, d_proj = dp.camera_backward(P, o, cam, HW, sh_degree=deg, exact_grad=exact)
+        d_view, d_proj = fo.camera_backward(P, o, cam, HW, sh_degree=deg, exact_grad=exact)
         assert np.all(d_proj[:, 2] == 0)
         for k in range(4):
             for j in range(4):
@@ -108,7 +109,7 @@ def test_depth_of_one_opaque_splat_is_its_z():
     keep[0, 0, 0] = True
     P["opacity"] = np.where(keep, 6.0, -40.0)
     P["scale"] = np.where(keep[None], np.log(0.5), P["scale"])
-    out = dp.render_forward_backward(P, aabb, cam, HW, TILE, 0, lambda img: np.zeros_like(img), render_depth=True)
+    out = fo.render_forward_backward(P, aabb, cam, HW, TILE, 0, lambda img: np.zeros_like(img), render_depth=True)
     a = 1 - out["T"][..., :HW[0], :HW[1]]
     m = a > 1e-3
     assert m.sum() > 50
@@ -119,7 +120,8 @@ def test_depth_of_one_opaque_splat_is_its_z():
 
 
 def test_off_and_depth_without_loss_are_the_existing_composition():
-    """render_depth=False returns the existing composition's bits; depth on with no depth loss changes no output either."""
+    """render_depth=False returns the oracle's own composition's bits where the other modes allow it; depth on with no depth loss
+    changes no output either."""
     nt = oracle.num_threads()
     oracle.set_num_threads(1)               # the oracle's raster backward sums are reproducible with one thread
     try:
@@ -133,10 +135,10 @@ def _off_and_on_without_loss():
         P, aabb, cam, filt = _scene(deg, filtered)
         w = np.random.default_rng(3).normal(size=(1, 3, *HW))
         kw = dict(true_sigmoid_grad=True, antialiased=aa_on, filter_3d=filt)
-        ref = aa.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, antialiased=aa_on,
-                                         true_sigmoid_grad=True) if filt is None else None
-        off = dp.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, **kw)
-        on = dp.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, render_depth=True, **kw)
+        ref = None if aa_on or filtered else oracle.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w,
+                                                                             true_sigmoid_grad=True)
+        off = fo.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, **kw)
+        on = fo.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, render_depth=True, **kw)
         for k in ("img", "T", "last", "ranges", "sorted_pid", "d_ndc", "d_cov", "d_op"):
             assert np.array_equal(on[k], off[k]), k
             if ref is not None:
@@ -151,7 +153,7 @@ def _off_and_on_without_loss():
 def test_weights_sum_to_one_minus_T():
     """sum w = 1 - T (the identity that makes D / (1 - T) the expected depth), from the oracle's composite of z = 1."""
     P, aabb, cam, _ = _scene(3, False)
-    out = dp.render_forward_backward(P, aabb, cam, HW, TILE, 3, lambda img: np.zeros_like(img), render_depth=True)
+    out = fo.render_forward_backward(P, aabb, cam, HW, TILE, 3, lambda img: np.zeros_like(img), render_depth=True)
     inter = out["inter"]
     ones = np.ones(inter["view_pos"].shape[-1])
     sw = dp.depth_forward(out["sorted_pid"], out["ranges"], inter["ndc"], inter["inv_cov2d"], out["opacity"], ones, *HW, *TILE)

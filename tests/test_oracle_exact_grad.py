@@ -1,15 +1,16 @@
-"""The exact gradient mode on the CPU (numpy restatement in tests/exact_grad_oracle.py): the J backward and the SH direction
-backward on their own against fp64 central differences, the position and camera gradients of a render against central
-differences of the real function (only the tile lists frozen; J and the colours follow the perturbation), the default convention
-failing that check on the same scenes, and what the mode leaves unchanged."""
+"""The exact gradient mode on the CPU (numpy restatement in tests/exact_grad_oracle.py, composed by tests/fused_oracle.py): the J
+backward and the SH direction backward on their own against fp64 central differences, the position and camera gradients of a
+render against central differences of the real function (only the tile lists frozen; J and the colours follow the perturbation),
+the default convention failing that check on the same scenes, and what the mode leaves unchanged."""
 import numpy as np
 import pytest
 
 import oracle
 from litegs_b200 import scene
-from tests import aa_oracle as aa
+from tests import camera_oracle as co
 from tests import exact_grad_oracle as ex
-from tests.test_oracle_antialias import _tiny
+from tests import fused_oracle as fo
+from tests.util import PARAM_KEYS, tiny_scene
 
 HW, TILE = (32, 32), (8, 8)
 TOL = 1e-4
@@ -99,7 +100,7 @@ def test_direction_backward_matches_finite_differences(deg):
 
 
 def _scene(deg, filtered):
-    P, aabb, cam = _tiny(seed=5, deg=max(deg, 1))
+    P, aabb, cam = tiny_scene(seed=5, deg=max(deg, 1))
     if deg == 0:
         P["sh_rest"] = P["sh_rest"][:0]
     filt = np.random.default_rng(1).uniform(0.02, 0.12, (1, *P["xyz"].shape[-2:])) if filtered else None
@@ -117,13 +118,13 @@ def test_fp64_finite_differences_xyz_and_camera(deg, antialiased, filtered):
     rng = np.random.default_rng(2)
     w = rng.normal(size=(1, 3, *HW))
     kw = dict(antialiased=antialiased, filter_3d=filt)
-    out = ex.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, true_sigmoid_grad=True, exact_grad=True, **kw)
-    off = ex.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, true_sigmoid_grad=True, **kw)
+    out = fo.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, true_sigmoid_grad=True, exact_grad=True, **kw)
+    off = fo.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, true_sigmoid_grad=True, **kw)
     lists = (out["ranges"], out["sorted_pid"])
     ids = out["visible_chunk_id"]
 
     def loss(Q, c=cam):
-        return (ex.render_forward_backward(Q, aabb, c, HW, TILE, deg, lambda img: w, lists=lists, **kw)["img"] * w).sum()
+        return (fo.render_forward_backward(Q, aabb, c, HW, TILE, deg, lambda img: w, lists=lists, **kw)["img"] * w).sum()
 
     h = 1e-6
     worst = miss = 0.0
@@ -135,8 +136,8 @@ def test_fp64_finite_differences_xyz_and_camera(deg, antialiased, filtered):
         fd = (loss(Pp) - loss(Pm)) / (2 * h)
         assert _close(fd, g[c, a, s]), ("xyz", fd, g[c, a, s])
         worst, miss = max(worst, _ratio(fd, g[c, a, s])), max(miss, _ratio(fd, g0[c, a, s]))
-    d_view, d_proj = ex.camera_backward(P, out, cam, HW, exact_grad=True)
-    v0, p0 = aa.camera_backward(P, off, cam, HW)
+    d_view, d_proj = fo.camera_backward(P, out, cam, HW, exact_grad=True)
+    v0, p0 = fo.camera_backward(P, off, cam, HW)
     for which, gc, gd in (("view", d_view, v0), ("proj", d_proj, p0)):
         for k in range(4):
             for j in range(4):
@@ -157,7 +158,8 @@ def test_fp64_finite_differences_xyz_and_camera(deg, antialiased, filtered):
 
 def test_mode_changes_only_xyz_and_keeps_the_translation_identity():
     """Exact on vs off: the same image, lists and scale, rot, opacity, sh gradients (the mode only adds to d xyz);
-    sum_i d xyz_i = V3x3 . d_view[3, :3] to 1e-9 in fp64, with the antialiased mode and the filter on as well."""
+    sum_i d xyz_i = V3x3 . d_view[3, :3] to 1e-9 in fp64, with the antialiased mode and the filter on as well.  With the other
+    modes off as well, off is the oracle's own composition and camera_oracle's camera gradient, bit for bit."""
     for deg, aa_on, filtered in ((3, False, False), (3, True, True), (1, True, False)):
         P, aabb, cam, filt = _scene(deg, filtered)
         w = np.random.default_rng(3).normal(size=(1, 3, *HW))
@@ -165,8 +167,10 @@ def test_mode_changes_only_xyz_and_keeps_the_translation_identity():
         nt = oracle.num_threads()
         oracle.set_num_threads(1)               # the oracle's raster backward sums are reproducible with one thread
         try:
-            on = ex.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, exact_grad=True, **kw)
-            off = ex.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, **kw)
+            on = fo.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, exact_grad=True, **kw)
+            off = fo.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, **kw)
+            ref = None if aa_on or filtered else oracle.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w,
+                                                                                 true_sigmoid_grad=True)
         finally:
             oracle.set_num_threads(nt)
         for k in ("img", "ranges", "sorted_pid", "T", "last"):
@@ -174,15 +178,20 @@ def test_mode_changes_only_xyz_and_keeps_the_translation_identity():
         for k in ("scale", "rot", "opacity", "sh_0", "sh_rest"):
             assert np.array_equal(on["grads"][k], off["grads"][k]), k
         assert not np.array_equal(on["grads"]["xyz"], off["grads"]["xyz"])
-        d_view, _ = ex.camera_backward(P, on, cam, HW, exact_grad=True)
+        d_view, _ = fo.camera_backward(P, on, cam, HW, exact_grad=True)
         s = on["grads"]["xyz"].reshape(3, -1).sum(axis=1)
         rhs = cam["view"][0, :3, :3] @ d_view[3, :3]
         assert np.abs(s).max() > 0
         assert np.abs(s - rhs).max() <= 1e-9 * np.abs(s).max(), (s, rhs)
-        # off: the existing composition, unchanged
-        v0, p0 = ex.camera_backward(P, off, cam, HW)
-        va, pa = aa.camera_backward(P, off, cam, HW)
-        assert np.array_equal(v0, va) and np.array_equal(p0, pa)
+        # off: the oracle's own composition, unchanged
+        if ref is not None:
+            for k in ("img", "T", "last", "ranges", "sorted_pid", "d_ndc", "d_cov", "d_op"):
+                assert np.array_equal(ref[k], off[k]), k
+            for k in PARAM_KEYS:
+                assert np.array_equal(ref["grads"][k], off["grads"][k]), k
+            v0, p0 = fo.camera_backward(P, off, cam, HW)
+            va, pa, _ = co.camera_backward(P, ref, cam, HW)
+            assert np.array_equal(v0, va) and np.array_equal(p0, pa)
 
 
 def test_level_a_render_refuses_the_flag():

@@ -9,10 +9,9 @@ import pytest
 
 import oracle
 from litegs_b200 import ply, scene
-from tests import aa_oracle as aa
 from tests import filter3d_oracle as f3
-from tests.test_oracle_antialias import _tiny
-from tests.util import PARAM_KEYS, small_scene
+from tests import fused_oracle as fo
+from tests.util import PARAM_KEYS, f64_arrays, small_scene, tiny_scene
 
 HW, TILE, DEG = (32, 32), (8, 8), 2
 
@@ -111,16 +110,16 @@ def _filter_for(P, seed=0, lo=0.02, hi=0.12):
 def test_fp64_finite_differences_with_frozen_lists(true_sigmoid, antialiased):
     """scale, rot, sh and opacity of a filtered render (f held constant) equal fp64 central differences with the tile lists
     frozen.  Under the reference's sigmoid convention the opacity gradient is the true one divided by 1 - sigma."""
-    P, aabb, cam = _tiny()
+    P, aabb, cam = tiny_scene()
     filt = _filter_for(P)
     rng = np.random.default_rng(1)
     w = rng.normal(size=(1, 3, *HW))
     kw = dict(antialiased=antialiased, filter_3d=filt)
-    out = f3.render_forward_backward(P, aabb, cam, HW, TILE, DEG, lambda img: w, true_sigmoid_grad=true_sigmoid, **kw)
+    out = fo.render_forward_backward(P, aabb, cam, HW, TILE, DEG, lambda img: w, true_sigmoid_grad=true_sigmoid, **kw)
     assert out["rho3"].min() < 0.5 and out["rho3"].max() > 0.8
     lists = (out["ranges"], out["sorted_pid"])
     ids = out["visible_chunk_id"]
-    run = lambda Q: (f3.render_forward_backward(Q, aabb, cam, HW, TILE, DEG, lambda img: w, lists=lists, **kw)["img"] * w).sum()
+    run = lambda Q: (fo.render_forward_backward(Q, aabb, cam, HW, TILE, DEG, lambda img: w, lists=lists, **kw)["img"] * w).sum()
     sig = 1 / (1 + np.exp(-P["opacity"]))
     checked = 0
     for name in ("scale", "rot", "sh_0", "sh_rest", "opacity"):
@@ -144,18 +143,18 @@ def test_fp64_finite_differences_with_frozen_lists(true_sigmoid, antialiased):
 def test_fp64_finite_differences_xyz_and_camera_with_frozen_J_and_dirs(antialiased):
     """xyz and the camera (view and projection matrices) of a filtered render, with J, the SH directions and the tile lists
     frozen: the analytic gradients equal central differences."""
-    P, aabb, cam = _tiny(seed=5)
+    P, aabb, cam = tiny_scene(seed=5)
     filt = _filter_for(P, seed=1)
     rng = np.random.default_rng(2)
     w = rng.normal(size=(1, 3, *HW))
     kw = dict(antialiased=antialiased, filter_3d=filt)
-    out = f3.render_forward_backward(P, aabb, cam, HW, TILE, DEG, lambda img: w, true_sigmoid_grad=True, **kw)
+    out = fo.render_forward_backward(P, aabb, cam, HW, TILE, DEG, lambda img: w, true_sigmoid_grad=True, **kw)
     freeze = dict(J=out["inter"]["J"], color=out["color"])
     lists = (out["ranges"], out["sorted_pid"])
     ids = out["visible_chunk_id"]
 
     def loss(Q, c=cam):
-        return (f3.render_forward_backward(Q, aabb, c, HW, TILE, DEG, lambda img: w, lists=lists, freeze=freeze, **kw)["img"] * w).sum()
+        return (fo.render_forward_backward(Q, aabb, c, HW, TILE, DEG, lambda img: w, lists=lists, freeze=freeze, **kw)["img"] * w).sum()
 
     g = out["grads"]["xyz"]
     h = 1e-6
@@ -165,7 +164,7 @@ def test_fp64_finite_differences_xyz_and_camera_with_frozen_J_and_dirs(antialias
         Pm = {k: v.copy() for k, v in P.items()}; Pm["xyz"][c, ids[a], s] -= h
         fd = (loss(Pp) - loss(Pm)) / (2 * h)
         assert abs(fd - g[c, a, s]) <= 1e-4 * max(1e-3, abs(fd), abs(g[c, a, s])), (fd, g[c, a, s])
-    d_view, d_proj = aa.camera_backward(P, out, cam, HW)
+    d_view, d_proj = fo.camera_backward(P, out, cam, HW)
     for which, gc in (("view", d_view), ("proj", d_proj)):
         for k in range(4):
             for j in range(4):
@@ -179,35 +178,31 @@ def test_fp64_finite_differences_xyz_and_camera_with_frozen_J_and_dirs(antialias
                 assert abs(fd - gc[k, j]) <= 1e-4 * max(1e-3, abs(fd), abs(gc[k, j])), (which, k, j, fd, gc[k, j])
 
 
-def _f64(d):
-    return {k: (v.astype(np.float64) if isinstance(v, np.ndarray) and v.dtype == np.float32 else v) for k, v in d.items()}
-
-
 @pytest.mark.parametrize("antialiased", [False, True])
 @pytest.mark.parametrize("dt", [np.float32, np.float64])
 def test_zero_filter_and_no_filter_are_the_same_bits(dt, antialiased):
-    """f = 0 gives the unfiltered render bit for bit, forward and gradients; no filter gives aa_oracle's composition (and so, with
-    the antialiased mode off, the oracle's own).  One oracle thread: the raster backward's sums are reproducible only then."""
+    """f = 0 gives the unfiltered render bit for bit, forward and gradients; with the antialiased mode off as well, both are the
+    oracle's own composition.  One oracle thread: the raster backward's sums are reproducible only then."""
     hw, tile = (48, 64), (16, 16)
     params, aabb, cam = small_scene(n=800, hw=hw, seed=4)
     if dt == np.float64:
-        params, aabb, cam = _f64(params), tuple(a.astype(np.float64) for a in aabb), _f64(cam)
+        params, aabb, cam = f64_arrays(params), tuple(a.astype(np.float64) for a in aabb), f64_arrays(cam)
     w = np.random.default_rng(0).normal(size=(1, 3, *hw)).astype(dt)
     zero = np.zeros((1, *params["xyz"].shape[-2:]), dt)
     nt = oracle.num_threads()
     oracle.set_num_threads(1)
     try:
-        a = aa.render_forward_backward(params, aabb, cam, hw, tile, 3, lambda img: w, true_sigmoid_grad=True, antialiased=antialiased)
-        b = f3.render_forward_backward(params, aabb, cam, hw, tile, 3, lambda img: w, true_sigmoid_grad=True, antialiased=antialiased)
-        c = f3.render_forward_backward(params, aabb, cam, hw, tile, 3, lambda img: w, true_sigmoid_grad=True, antialiased=antialiased,
+        a = oracle.render_forward_backward(params, aabb, cam, hw, tile, 3, lambda img: w, true_sigmoid_grad=True)
+        b = fo.render_forward_backward(params, aabb, cam, hw, tile, 3, lambda img: w, true_sigmoid_grad=True, antialiased=antialiased)
+        c = fo.render_forward_backward(params, aabb, cam, hw, tile, 3, lambda img: w, true_sigmoid_grad=True, antialiased=antialiased,
                                        filter_3d=zero)
     finally:
         oracle.set_num_threads(nt)
-    for other in (b, c):
+    for ref, other in [(b, c)] + ([] if antialiased else [(a, b)]):
         for k in ("img", "T", "last", "fragile", "ranges", "sorted_pid", "d_ndc", "d_cov", "d_col", "d_op", "opacity"):
-            assert np.array_equal(a[k], other[k]), k
+            assert np.array_equal(ref[k], other[k]), k
         for k in PARAM_KEYS:
-            assert np.array_equal(a["grads"][k], other["grads"][k]), k
+            assert np.array_equal(ref["grads"][k], other["grads"][k]), k
     assert np.all(c["rho3"] == 1)
 
 

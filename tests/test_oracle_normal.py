@@ -1,13 +1,13 @@
-"""The normal mode on the CPU (numpy restatement in tests/normal_oracle.py): the gradients of a loss in the colour, the normal N and
-the expected normal N / (1 - T) against fp64 central differences with the tile lists, the shortest axes and the facing signs
-frozen, in the default and the exact convention; the properties of the definition."""
+"""The normal mode on the CPU (numpy restatement in tests/normal_oracle.py, composed by tests/fused_oracle.py): the gradients of a
+loss in the colour, the normal N and the expected normal N / (1 - T) against fp64 central differences with the tile lists, the
+shortest axes and the facing signs frozen, in the default and the exact convention; the properties of the definition."""
 import numpy as np
 import pytest
 
 import oracle
-from tests import depth_oracle as dp
+from tests import fused_oracle as fo
 from tests import normal_oracle as nm
-from tests.test_oracle_antialias import _tiny
+from tests.util import tiny_scene
 
 HW, TILE = (32, 32), (8, 8)
 TOL = 1e-4
@@ -18,7 +18,7 @@ def _close(fd, g):
 
 
 def _scene(deg, filtered):
-    P, aabb, cam = _tiny(seed=5, deg=max(deg, 1))
+    P, aabb, cam = tiny_scene(seed=5, deg=max(deg, 1))
     if deg == 0:
         P["sh_rest"] = P["sh_rest"][:0]
     filt = np.random.default_rng(1).uniform(0.02, 0.12, (1, *P["xyz"].shape[-2:])) if filtered else None
@@ -50,7 +50,7 @@ def test_fp64_finite_differences(deg, antialiased, filtered, depth):
     uz = rng.normal(size=(1, 1, *HW))
     true_sigmoid = bool(antialiased)
     kw = dict(antialiased=antialiased, filter_3d=filt, render_depth=depth)
-    base = nm.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, render_normal=True, **kw)
+    base = fo.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, render_normal=True, **kw)
     mask = (1 - base["T"][..., :HW[0], :HW[1]]) > 0.2
     nloss, ngrad = _normal_loss(u, v, mask)
     dz_fn = (lambda D, T: (uz, None)) if depth else None
@@ -60,13 +60,13 @@ def test_fp64_finite_differences(deg, antialiased, filtered, depth):
     assert np.abs(base["normal"]).max() > 0.1
 
     def run(Q, c=cam, freeze=None):
-        o = nm.render_forward_backward(Q, aabb, c, HW, TILE, deg, lambda img: w, render_normal=True, lists=lists, freeze=freeze,
+        o = fo.render_forward_backward(Q, aabb, c, HW, TILE, deg, lambda img: w, render_normal=True, lists=lists, freeze=freeze,
                                        normal_freeze=frame, **kw)
         T = o["T"][..., :HW[0], :HW[1]]
         return (o["img"] * w).sum() + nloss(o["normal"], T) + ((uz * o["depth"]).sum() if depth else 0.0)
 
     h = 1e-6
-    out = nm.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, render_normal=True, d_normal_fn=ngrad,
+    out = fo.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, render_normal=True, d_normal_fn=ngrad,
                                      d_depth_fn=dz_fn, true_sigmoid_grad=true_sigmoid, **kw)
     assert np.abs(out["dn"]).max() > 0
     sig = 1 / (1 + np.exp(-P["opacity"]))
@@ -83,7 +83,7 @@ def test_fp64_finite_differences(deg, antialiased, filtered, depth):
             want = g[idx] * ((1 - sig[full]) if name == "opacity" and not true_sigmoid else 1.0)
             assert _close(fd, want), (name, idx, fd, want)
     for exact in (False, True):
-        o = nm.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, render_normal=True, d_normal_fn=ngrad,
+        o = fo.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, render_normal=True, d_normal_fn=ngrad,
                                        d_depth_fn=dz_fn, true_sigmoid_grad=True, exact_grad=exact, **kw)
         freeze = None if exact else dict(J=o["inter"]["J"], color=o["color"])
         g = o["grads"]["xyz"]
@@ -93,8 +93,8 @@ def test_fp64_finite_differences(deg, antialiased, filtered, depth):
             Pm = {k: x.copy() for k, x in P.items()}; Pm["xyz"][c, ids[a], s] -= h
             fd = (run(Pp, freeze=freeze) - run(Pm, freeze=freeze)) / (2 * h)
             assert _close(fd, g[c, a, s]), ("xyz", exact, fd, g[c, a, s])
-        d_view, d_proj = nm.camera_backward(P, o, cam, HW, sh_degree=deg, exact_grad=exact)
-        d_view0, d_proj0 = dp.camera_backward(P, o, cam, HW, sh_degree=deg, exact_grad=exact)
+        d_view, d_proj = fo.camera_backward(P, o, cam, HW, sh_degree=deg, exact_grad=exact)
+        d_view0, d_proj0 = fo.camera_backward(P, dict(o, dn=None), cam, HW, sh_degree=deg, exact_grad=exact)
         assert np.array_equal(d_proj, np.asarray(d_proj0, np.float64))      # the normal term adds nothing to d_proj
         for k in range(4):
             for j in range(4):
@@ -119,7 +119,7 @@ def test_opaque_tilted_splat_gives_its_normal():
     """One large opaque tilted splat: N / (1 - T) equals its n wherever it was blended, |n| = 1 and n faces the camera."""
     P, aabb, cam, _ = _scene(0, False)
     Q = _opaque_tilted(P, np.array([0.9, 0.3, -0.2, 0.1]))
-    out = nm.render_forward_backward(Q, aabb, cam, HW, TILE, 0, lambda img: np.zeros_like(img), render_normal=True)
+    out = fo.render_forward_backward(Q, aabb, cam, HW, TILE, 0, lambda img: np.zeros_like(img), render_normal=True)
     a = 1 - out["T"][..., :HW[0], :HW[1]]
     m = a[0, 0] > 1e-3
     assert m.sum() > 50
@@ -151,8 +151,8 @@ def test_rotation_about_the_shortest_axis_leaves_N_unchanged():
         q2 = np.array([r2 * r1 - v2 @ v1, *(r2 * v1 + r1 * v2 + np.cross(v2, v1))])
         R2 = nm.quat_R(q2[:, None])[:, 0].reshape(3, 3)
     assert np.allclose(R2[2], R[2], atol=1e-12) and not np.allclose(R2[0], R[0], atol=1e-3)
-    o1 = nm.render_forward_backward(_opaque_tilted(P, q), aabb, cam, HW, TILE, 0, lambda img: np.zeros_like(img), render_normal=True)
-    o2 = nm.render_forward_backward(_opaque_tilted(P, q2), aabb, cam, HW, TILE, 0, lambda img: np.zeros_like(img), render_normal=True)
+    o1 = fo.render_forward_backward(_opaque_tilted(P, q), aabb, cam, HW, TILE, 0, lambda img: np.zeros_like(img), render_normal=True)
+    o2 = fo.render_forward_backward(_opaque_tilted(P, q2), aabb, cam, HW, TILE, 0, lambda img: np.zeros_like(img), render_normal=True)
     # the ellipse turns with the long axes, so compare the expected normal where both renders blended the splat (it is the only
     # one the alpha test lets through)
     a1, a2 = 1 - o1["T"][0, 0, :HW[0], :HW[1]], 1 - o2["T"][0, 0, :HW[0], :HW[1]]
@@ -211,16 +211,17 @@ def test_translation_identity():
     rng = np.random.default_rng(9)
     w, u = rng.normal(size=(1, 3, *HW)), rng.normal(size=(1, 3, *HW))
     for exact in (False, True):
-        o = nm.render_forward_backward(P, aabb, cam, HW, TILE, 3, lambda img: w, render_normal=True,
+        o = fo.render_forward_backward(P, aabb, cam, HW, TILE, 3, lambda img: w, render_normal=True,
                                        d_normal_fn=lambda N, T: (u, None), true_sigmoid_grad=True, exact_grad=exact)
-        d_view, _ = nm.camera_backward(P, o, cam, HW, sh_degree=3, exact_grad=exact)
+        d_view, _ = fo.camera_backward(P, o, cam, HW, sh_degree=3, exact_grad=exact)
         V3 = np.asarray(cam["view"], np.float64).reshape(4, 4)[:3, :3]
         gsum = o["grads"]["xyz"].astype(np.float64).reshape(3, -1).sum(1)
         assert np.abs(gsum - V3 @ d_view[3, :3]).max() <= 1e-9 * max(1.0, np.abs(gsum).max()), (exact, gsum, V3 @ d_view[3, :3])
 
 
 def test_off_and_normals_without_loss_are_the_existing_composition():
-    """render_normal=False returns depth_oracle's bits; normals on with no normal loss change no output either."""
+    """render_normal=False returns the oracle's own composition's bits where the other modes allow it; normals on with no normal
+    loss change no output either."""
     nt = oracle.num_threads()
     oracle.set_num_threads(1)
     try:
@@ -228,13 +229,14 @@ def test_off_and_normals_without_loss_are_the_existing_composition():
             P, aabb, cam, filt = _scene(deg, filtered)
             w = np.random.default_rng(3).normal(size=(1, 3, *HW))
             kw = dict(true_sigmoid_grad=True, antialiased=aa_on, filter_3d=filt, render_depth=depth)
-            ref = dp.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, **kw)
-            off = nm.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, **kw)
-            on = nm.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, render_normal=True, **kw)
+            ref = None if aa_on or filtered or depth else oracle.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w,
+                                                                                          true_sigmoid_grad=True)
+            off = fo.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, **kw)
+            on = fo.render_forward_backward(P, aabb, cam, HW, TILE, deg, lambda img: w, render_normal=True, **kw)
             for k in ("img", "T", "last", "ranges", "sorted_pid", "d_ndc", "d_cov", "d_op"):
-                assert np.array_equal(ref[k], off[k]) and np.array_equal(on[k], off[k]), k
+                assert (ref is None or np.array_equal(ref[k], off[k])) and np.array_equal(on[k], off[k]), k
             for k in on["grads"]:
-                assert np.array_equal(ref["grads"][k], off["grads"][k]) and np.array_equal(on["grads"][k], off["grads"][k]), k
+                assert (ref is None or np.array_equal(ref["grads"][k], off["grads"][k])) and np.array_equal(on["grads"][k], off["grads"][k]), k
             assert not np.any(on["dn"])
     finally:
         oracle.set_num_threads(nt)
