@@ -50,9 +50,11 @@ extern "C" int lgs_get_allocate_size(const float* ndc, const float* view_space_z
     LGS_CUDA(cudaMemsetAsync(allocate_size, 0, sizeof(int) * (size_t)V * N, st));
     int gx = (width + tile_w - 1) / tile_w, gy = (height + tile_h - 1) / tile_h;
     dim3 grid(lgs_cdiv(N, 256), V);
-    LGS_DISPATCH_TILE(tile_h, tile_w,
-        allocate_size_kernel<TH, TW><<<grid, 256, 0, st>>>(ndc, view_space_z, inv_cov2d, opacity, valid_length, N, height, width,
-                                                          gx, gy, left_up, right_down, allocate_size);)
+    lgs_with_tile(tile_h, tile_w, [&](auto th, auto tw) {
+        allocate_size_kernel<th, tw><<<grid, 256, 0, st>>>(ndc, view_space_z, inv_cov2d, opacity, valid_length, N, height, width,
+                                                          gx, gy, left_up, right_down, allocate_size);
+        return LGS_OK;
+    });
     LGS_CHECK_LAUNCH("allocate_size_kernel");
     return LGS_OK;
 }
@@ -123,9 +125,11 @@ extern "C" int lgs_create_table(const float* ndc, const float* inv_cov2d, const 
     int gx = (width + tile_w - 1) / tile_w, gy = (height + tile_h - 1) / tile_h;
     if (N > 0) {
         dim3 grid(lgs_cdiv(N, 256), V);
-        LGS_DISPATCH_TILE(tile_h, tile_w,
-            emit_pairs_kernel<TH, TW><<<grid, 256, 0, st>>>(ndc, inv_cov2d, opacity, offset, depth_sorted_pointid, N, cap, height,
-                                                           width, gx, gy, keys, vals);)
+        lgs_with_tile(tile_h, tile_w, [&](auto th, auto tw) {
+            emit_pairs_kernel<th, tw><<<grid, 256, 0, st>>>(ndc, inv_cov2d, opacity, offset, depth_sorted_pointid, N, cap, height,
+                                                           width, gx, gy, keys, vals);
+            return LGS_OK;
+        });
         LGS_CHECK_LAUNCH("emit_pairs_kernel");
     }
     int bits = tile_bits(gx * gy);

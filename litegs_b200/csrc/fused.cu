@@ -317,18 +317,6 @@ __global__ void project_forward_kernel(
     }
 }
 
-// Largest block a NORMAL instantiation of project_forward_kernel can be launched with: the heaviest use 72 registers, which
-// allows 896 threads instead of 1024 (DESIGN.md section 1, "Normals").  Read once per instantiation, on its first (eager) use.
-template <int DEG, int TH, int TW, bool AA, bool F3D>
-static int project_forward_normal_max_threads()
-{
-    static const int n = [] {
-        cudaFuncAttributes a;
-        return cudaFuncGetAttributes(&a, project_forward_kernel<DEG, TH, TW, AA, F3D, true>) == cudaSuccess ? a.maxThreadsPerBlock : 0;
-    }();
-    return n;
-}
-
 // normal_rec f32[A*S,4] or NULL: normal mode, the camera-facing view-space normal of each record (DESIGN.md section 1, "Normals").
 extern "C" int lgs_project_forward(int sh_degree, const int64_t* visible_chunk_id, const int* visible_chunks_num,
                                    const float* view_matrix, const float* proj_matrix, const float* position,
@@ -344,27 +332,21 @@ extern "C" int lgs_project_forward(int sh_degree, const int64_t* visible_chunk_i
     LGS_CUDA(cudaMemsetAsync(totals, 0, 3 * sizeof(int), st));
     if (A == 0) return LGS_OK;
     int gx = (img_w + tile_w - 1) / tile_w, gy = (img_h + tile_h - 1) / tile_h;
-#define PF(D, AA, F3, NM) {                                                                                                         \
-        if constexpr (NM) {                                                                                                         \
-            const int mt = project_forward_normal_max_threads<D, TH, TW, AA, F3>();                                                 \
-            LGS_REQUIRE(S <= mt, "project_forward: normals with this configuration support chunk sizes up to %d, got %d", mt, S); \
-        }                                                                                                                           \
-        project_forward_kernel<D, TH, TW, AA, F3, NM><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num,                        \
-        view_matrix, proj_matrix, position, scale, rotation, sh_base, sh_rest, opacity, C, S, img_h, img_w, gx, gy,                  \
-        (SplatRec*)packed_params, depth_key, iota, tile_count, totals, filter_3d, (float4*)normal_rec); }
-#define PF_DEG(AA, F3, NM) LGS_DISPATCH_TILE(tile_h, tile_w,                                                                        \
-        switch (sh_degree) { case 0: PF(0, AA, F3, NM); break; case 1: PF(1, AA, F3, NM); break; case 2: PF(2, AA, F3, NM); break;   \
-                             default: PF(3, AA, F3, NM); })
-#define PF_MODE(NM)                                                                                                                 \
-    if (filter_3d != nullptr) {                                                                                                     \
-        if (antialiased) { PF_DEG(true, true, NM) } else { PF_DEG(false, true, NM) }                                                \
-    } else {                                                                                                                        \
-        if (antialiased) { PF_DEG(true, false, NM) } else { PF_DEG(false, false, NM) }                                              \
-    }
-    if (normal_rec != nullptr) { PF_MODE(true) } else { PF_MODE(false) }
-#undef PF_MODE
-#undef PF_DEG
-#undef PF
+    const int rc = lgs_with_flags([&](auto nm, auto f3, auto aa) { return lgs_with_tile(tile_h, tile_w, [&](auto th, auto tw) {
+        return lgs_with_degree(sh_degree, [&](auto deg) {
+            constexpr auto kernel = project_forward_kernel<deg, th, tw, aa, f3, nm>;
+            // the heaviest NORMAL instantiations use 72 registers, which allows 896 threads instead of 1024 (DESIGN.md section 1,
+            // "Normals")
+            if constexpr (nm) {
+                const int mt = lgs_max_threads<kernel>();
+                LGS_REQUIRE(S <= mt, "project_forward: normals with this configuration support chunk sizes up to %d, got %d", mt, S);
+            }
+            kernel<<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num, view_matrix, proj_matrix, position, scale, rotation, sh_base,
+                                    sh_rest, opacity, C, S, img_h, img_w, gx, gy, (SplatRec*)packed_params, depth_key, iota, tile_count,
+                                    totals, filter_3d, (float4*)normal_rec);
+            return LGS_OK;
+        }); }); }, normal_rec != nullptr, filter_3d != nullptr, antialiased != 0);
+    if (rc != LGS_OK) return rc;
     LGS_CHECK_LAUNCH("project_forward_kernel");
     return LGS_OK;
 }
@@ -429,9 +411,11 @@ extern "C" int lgs_emit_pairs(const float* packed_params, const int* offset, con
     if (n <= 0 || cap <= 0) return LGS_OK;
     int gx = (img_w + tile_w - 1) / tile_w, gy = (img_h + tile_h - 1) / tile_h;
     cudaStream_t st = (cudaStream_t)stream;
-    LGS_DISPATCH_TILE(tile_h, tile_w,
-        emit_pairs_rec_kernel<TH, TW, int><<<lgs_cdiv(n, LGS_EMIT_WARPS * 32), LGS_EMIT_WARPS * 32, 0, st>>>((const SplatRec*)packed_params, offset, order, n, cap, img_h,
-                                                                           img_w, gx, gy, keys, vals, nullptr, nullptr);)
+    lgs_with_tile(tile_h, tile_w, [&](auto th, auto tw) {
+        emit_pairs_rec_kernel<th, tw, int><<<lgs_cdiv(n, LGS_EMIT_WARPS * 32), LGS_EMIT_WARPS * 32, 0, st>>>(
+            (const SplatRec*)packed_params, offset, order, n, cap, img_h, img_w, gx, gy, keys, vals, nullptr, nullptr);
+        return LGS_OK;
+    });
     LGS_CHECK_LAUNCH("emit_pairs_rec_kernel");
     return LGS_OK;
 }
@@ -445,9 +429,11 @@ extern "C" int lgs_emit_pairs_u16(const float* packed_params, const int* offset,
     int gx = (img_w + tile_w - 1) / tile_w, gy = (img_h + tile_h - 1) / tile_h;
     LGS_REQUIRE(gx * gy + 1 < 65536, "emit_pairs_u16: %d tiles do not fit 16-bit keys", gx * gy);
     cudaStream_t st = (cudaStream_t)stream;
-    LGS_DISPATCH_TILE(tile_h, tile_w,
-        emit_pairs_rec_kernel<TH, TW, unsigned short><<<lgs_cdiv(n, LGS_EMIT_WARPS * 32), LGS_EMIT_WARPS * 32, 0, st>>>((const SplatRec*)packed_params, offset, order, n, cap,
-                                                                                      img_h, img_w, gx, gy, keys, vals, nullptr, nullptr);)
+    lgs_with_tile(tile_h, tile_w, [&](auto th, auto tw) {
+        emit_pairs_rec_kernel<th, tw, unsigned short><<<lgs_cdiv(n, LGS_EMIT_WARPS * 32), LGS_EMIT_WARPS * 32, 0, st>>>(
+            (const SplatRec*)packed_params, offset, order, n, cap, img_h, img_w, gx, gy, keys, vals, nullptr, nullptr);
+        return LGS_OK;
+    });
     LGS_CHECK_LAUNCH("emit_pairs_rec_kernel<u16>");
     return LGS_OK;
 }
@@ -466,15 +452,12 @@ extern "C" int lgs_emit_pairs_dev(const float* packed_params, const int* offset,
     LGS_REQUIRE(key_bits == 32 || gx * gy + 1 < 65536, "emit_pairs_dev: %d tiles do not fit 16-bit keys", gx * gy);
     cudaStream_t st = (cudaStream_t)stream;
     const int grid = lgs_cdiv(n_capacity, LGS_EMIT_WARPS * 32);
-    if (key_bits == 16) {
-        LGS_DISPATCH_TILE(tile_h, tile_w,
-            emit_pairs_rec_kernel<TH, TW, unsigned short><<<grid, LGS_EMIT_WARPS * 32, 0, st>>>((const SplatRec*)packed_params, offset, order, n_capacity,
-                                                                                          cap, img_h, img_w, gx, gy, (unsigned short*)keys, vals, n_dev, valid_pairs);)
-    } else {
-        LGS_DISPATCH_TILE(tile_h, tile_w,
-            emit_pairs_rec_kernel<TH, TW, int><<<grid, LGS_EMIT_WARPS * 32, 0, st>>>((const SplatRec*)packed_params, offset, order, n_capacity, cap,
-                                                                               img_h, img_w, gx, gy, (int*)keys, vals, n_dev, valid_pairs);)
-    }
+    lgs_with_flags([&](auto k16) { return lgs_with_tile(tile_h, tile_w, [&](auto th, auto tw) {
+        using KeyT = std::conditional_t<k16, unsigned short, int>;
+        emit_pairs_rec_kernel<th, tw, KeyT><<<grid, LGS_EMIT_WARPS * 32, 0, st>>>((const SplatRec*)packed_params, offset, order, n_capacity,
+                                                                              cap, img_h, img_w, gx, gy, (KeyT*)keys, vals, n_dev, valid_pairs);
+        return LGS_OK;
+    }); }, key_bits == 16);
     LGS_CHECK_LAUNCH("emit_pairs_rec_kernel(dev)");
     return LGS_OK;
 }
@@ -883,20 +866,6 @@ __global__ void __launch_bounds__(1024) camera_grad_sum_kernel(const float* __re
     }
 }
 
-// Largest block an EXACT or NORMAL instantiation can be launched with.  The kernel has no launch bounds (the default
-// instantiations must keep their code), and the heaviest EXACT ones use up to 168 registers, which allows 384 threads instead of
-// 1024 (DESIGN.md section 1, "Exact gradient mode"); NORMAL instantiations use up to 138 without EXACT (DESIGN.md section 1,
-// "Normals").  Read once per instantiation, on its first (eager) use.
-template <int DEG, bool CAM, bool AA, bool F3D, bool EXACT, bool DEPTH, bool NORMAL>
-static int project_backward_max_threads()
-{
-    static const int n = [] {
-        cudaFuncAttributes a;
-        return cudaFuncGetAttributes(&a, project_backward_kernel<DEG, CAM, AA, F3D, EXACT, DEPTH, NORMAL>) == cudaSuccess ? a.maxThreadsPerBlock : 0;
-    }();
-    return n;
-}
-
 // mode 0: outputs are compacted [..,A,S] and assigned; mode 1: same, cleared first (rows of chunks >= *visible_num and
 // sh_rest rows above the active degree must read as zero); mode 2: outputs are the DENSE [..,C,S] gradient tensors and
 // this view's gradients are accumulated into them (the multi-view / data-parallel path: no compacted round trip).
@@ -937,36 +906,24 @@ extern "C" int lgs_project_backward(int sh_degree, const int64_t* visible_chunk_
         LGS_CUDA(cudaMemsetAsync(g_sh_rest, 0, sizeof(float) * (size_t)rest_dim * 3 * AS, st));
         LGS_CUDA(cudaMemsetAsync(g_opacity, 0, sizeof(float) * AS, st));
     }
-#define PB(D, K, AA, F3, EX, Z, NM) {                                                                                               \
-        if constexpr (EX || NM) {                                                                                                   \
-            const int mt = project_backward_max_threads<D, K, AA, F3, EX, Z, NM>();                                                 \
-            LGS_REQUIRE(S <= mt, "project_backward: %s with this configuration supports chunk sizes up to %d, got %d",            \
-                        EX ? "exact_grad" : "the normal gradient", mt, S);                                                          \
-        }                                                                                                                           \
-        project_backward_kernel<D, K, AA, F3, EX, Z, NM><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num,                     \
-        view_matrix, proj_matrix, position, scale, rotation, opacity, C, S, A, rest_dim, img_h, img_w, true_sigmoid_grad, accumulate,  \
-        packed_grad, grad_inv_scaler, g_position, g_scale, g_rotation, g_sh_base, g_sh_rest, g_opacity, touched, cam_partials,        \
-        filter_3d, sh_rest, (const float4*)grad_normal); }
-#define PB_DEG(K, AA, F3, EX, Z, NM) switch (sh_degree) { case 0: PB(0, K, AA, F3, EX, Z, NM); break; case 1: PB(1, K, AA, F3, EX, Z, NM); break; \
-                                                          case 2: PB(2, K, AA, F3, EX, Z, NM); break; default: PB(3, K, AA, F3, EX, Z, NM); }
-#define PB_CAM(AA, F3, EX, Z, NM) if (cam) { PB_DEG(true, AA, F3, EX, Z, NM) } else { PB_DEG(false, AA, F3, EX, Z, NM) }
-#define PB_MODE(EX, Z, NM)                                                                                                          \
-    if (filter_3d != nullptr) {                                                                                                     \
-        if (antialiased) { PB_CAM(true, true, EX, Z, NM) } else { PB_CAM(false, true, EX, Z, NM) }                                  \
-    } else {                                                                                                                        \
-        if (antialiased) { PB_CAM(true, false, EX, Z, NM) } else { PB_CAM(false, false, EX, Z, NM) }                                \
-    }
-#define PB_DEPTH(EX, NM) if (depth) { PB_MODE(EX, true, NM) } else { PB_MODE(EX, false, NM) }
-    if (grad_normal != nullptr) {
-        if (exact_grad) { PB_DEPTH(true, true) } else { PB_DEPTH(false, true) }
-    } else {
-        if (exact_grad) { PB_DEPTH(true, false) } else { PB_DEPTH(false, false) }
-    }
-#undef PB_DEPTH
-#undef PB_MODE
-#undef PB_CAM
-#undef PB_DEG
-#undef PB
+    const int rc = lgs_with_flags([&](auto nm, auto ex, auto z, auto f3, auto aa, auto k) {
+        return lgs_with_degree(sh_degree, [&](auto deg) {
+            constexpr auto kernel = project_backward_kernel<deg, k, aa, f3, ex, z, nm>;
+            // The kernel has no launch bounds (the default instantiations must keep their code), and the heaviest EXACT ones use up
+            // to 168 registers, which allows 384 threads instead of 1024 (DESIGN.md section 1, "Exact gradient mode"); NORMAL
+            // instantiations use up to 138 without EXACT (DESIGN.md section 1, "Normals").
+            if constexpr (ex || nm) {
+                const int mt = lgs_max_threads<kernel>();
+                LGS_REQUIRE(S <= mt, "project_backward: %s with this configuration supports chunk sizes up to %d, got %d",
+                            ex ? "exact_grad" : "the normal gradient", mt, S);
+            }
+            kernel<<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num, view_matrix, proj_matrix, position, scale, rotation, opacity, C,
+                                    S, A, rest_dim, img_h, img_w, true_sigmoid_grad, accumulate, packed_grad, grad_inv_scaler, g_position,
+                                    g_scale, g_rotation, g_sh_base, g_sh_rest, g_opacity, touched, cam_partials, filter_3d, sh_rest,
+                                    (const float4*)grad_normal);
+            return LGS_OK;
+        }); }, grad_normal != nullptr, exact_grad != 0, depth != 0, filter_3d != nullptr, antialiased != 0, cam);
+    if (rc != LGS_OK) return rc;
     LGS_CHECK_LAUNCH("project_backward_kernel");
     if (cam) {
         camera_grad_sum_kernel<<<1, 1024, 0, st>>>(cam_partials, A, d_cam);

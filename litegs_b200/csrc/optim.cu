@@ -97,8 +97,10 @@ extern "C" int lgs_adam_step_dense(float* const* params, const int* rows_per_par
     }
     LGS_REQUIRE((((uintptr_t)grad | (uintptr_t)exp_avg | (uintptr_t)exp_avg_sq) & 15) == 0, "adam_step_dense: buffers must be 16-byte aligned");
     cudaStream_t st = (cudaStream_t)stream;
-    if (clear_grad) adam_dense_kernel<true><<<C, S / 4, 0, st>>>(G, grad, exp_avg, exp_avg_sq, touched, C, S, (float)b1, (float)b2, (float)eps);
-    else adam_dense_kernel<false><<<C, S / 4, 0, st>>>(G, grad, exp_avg, exp_avg_sq, touched, C, S, (float)b1, (float)b2, (float)eps);
+    lgs_with_flags([&](auto clear) {
+        adam_dense_kernel<clear><<<C, S / 4, 0, st>>>(G, grad, exp_avg, exp_avg_sq, touched, C, S, (float)b1, (float)b2, (float)eps);
+        return LGS_OK;
+    }, clear_grad != 0);
     LGS_CHECK_LAUNCH("adam_dense_kernel");
     return LGS_OK;
 }

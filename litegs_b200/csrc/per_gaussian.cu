@@ -166,10 +166,12 @@ extern "C" int lgs_cull_compact_activate(int sh_degree, const int64_t* visible_c
     LGS_REQUIRE(S >= 1 && S <= 1024 && V >= 1, "cull_compact_activate: chunk size %d / views %d unsupported", S, V);
     if (A == 0) return LGS_OK;
     cudaStream_t st = (cudaStream_t)stream;
-#define LAUNCH(D) activate_forward_kernel<D><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num, view_matrix, V, position, \
-        scale, rotation, sh_base, sh_rest, opacity, C, S, A, act_position, act_scale, act_rotation, color, act_opacity)
-    switch (sh_degree) { case 0: LAUNCH(0); break; case 1: LAUNCH(1); break; case 2: LAUNCH(2); break; default: LAUNCH(3); }
-#undef LAUNCH
+    lgs_with_degree(sh_degree, [&](auto deg) {
+        activate_forward_kernel<deg><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num, view_matrix, V, position, scale, rotation,
+                                                      sh_base, sh_rest, opacity, C, S, A, act_position, act_scale, act_rotation, color,
+                                                      act_opacity);
+        return LGS_OK;
+    });
     LGS_CHECK_LAUNCH("activate_forward_kernel");
     return LGS_OK;
 }
@@ -253,11 +255,13 @@ extern "C" int lgs_activate_backward(int sh_degree, const int64_t* visible_chunk
     // rows of sh_rest above the active degree (and tail chunks) must read as zero, as with the
     // reference's torch::zeros allocation (GR/compact.cu:1107).
     LGS_CUDA(cudaMemsetAsync(g_sh_rest, 0, sizeof(float) * (size_t)rest_dim * 3 * A * S, st));
-#define LAUNCH(D) activate_backward_kernel<D><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num, view_matrix, V, position, \
-        scale, rotation, opacity, C, S, A, rest_dim, true_sigmoid_grad, g_act_position, g_act_scale, g_act_rotation, g_color, \
-        g_act_opacity, g_position, g_scale, g_rotation, g_sh_base, g_sh_rest, g_opacity)
-    switch (sh_degree) { case 0: LAUNCH(0); break; case 1: LAUNCH(1); break; case 2: LAUNCH(2); break; default: LAUNCH(3); }
-#undef LAUNCH
+    lgs_with_degree(sh_degree, [&](auto deg) {
+        activate_backward_kernel<deg><<<A, S, 0, st>>>(visible_chunk_id, visible_chunks_num, view_matrix, V, position, scale, rotation,
+                                                       opacity, C, S, A, rest_dim, true_sigmoid_grad, g_act_position, g_act_scale,
+                                                       g_act_rotation, g_color, g_act_opacity, g_position, g_scale, g_rotation, g_sh_base,
+                                                       g_sh_rest, g_opacity);
+        return LGS_OK;
+    });
     LGS_CHECK_LAUNCH("activate_backward_kernel");
     return LGS_OK;
 }
@@ -646,12 +650,10 @@ extern "C" int lgs_sh2rgb_forward(int degree, const float* sh_base, const float*
     if (N == 0) return LGS_OK;
     dim3 grid(lgs_cdiv(N, 256), V);
     cudaStream_t st = (cudaStream_t)stream;
-    switch (degree) {
-    case 0: sh2rgb_forward_kernel<0><<<grid, 256, 0, st>>>(sh_base, sh_rest, dirs, rgb, N); break;
-    case 1: sh2rgb_forward_kernel<1><<<grid, 256, 0, st>>>(sh_base, sh_rest, dirs, rgb, N); break;
-    case 2: sh2rgb_forward_kernel<2><<<grid, 256, 0, st>>>(sh_base, sh_rest, dirs, rgb, N); break;
-    default: sh2rgb_forward_kernel<3><<<grid, 256, 0, st>>>(sh_base, sh_rest, dirs, rgb, N); break;
-    }
+    lgs_with_degree(degree, [&](auto deg) {
+        sh2rgb_forward_kernel<deg><<<grid, 256, 0, st>>>(sh_base, sh_rest, dirs, rgb, N);
+        return LGS_OK;
+    });
     LGS_CHECK_LAUNCH("sh2rgb_forward_kernel");
     return LGS_OK;
 }
@@ -689,12 +691,10 @@ extern "C" int lgs_sh2rgb_backward(int degree, const float* rgb_grad, int sh_res
     LGS_CUDA(cudaMemsetAsync(sh_rest_grad, 0, sizeof(float) * (size_t)sh_rest_dim * 3 * N, st));
     if (dir_grad) LGS_CUDA(cudaMemsetAsync(dir_grad, 0, sizeof(float) * (size_t)V * 3 * N, st));
     int grid = lgs_cdiv(N, 256);
-    switch (degree) {
-    case 0: sh2rgb_backward_kernel<0><<<grid, 256, 0, st>>>(dirs, rgb_grad, V, N, sh_base_grad, sh_rest_grad); break;
-    case 1: sh2rgb_backward_kernel<1><<<grid, 256, 0, st>>>(dirs, rgb_grad, V, N, sh_base_grad, sh_rest_grad); break;
-    case 2: sh2rgb_backward_kernel<2><<<grid, 256, 0, st>>>(dirs, rgb_grad, V, N, sh_base_grad, sh_rest_grad); break;
-    default: sh2rgb_backward_kernel<3><<<grid, 256, 0, st>>>(dirs, rgb_grad, V, N, sh_base_grad, sh_rest_grad); break;
-    }
+    lgs_with_degree(degree, [&](auto deg) {
+        sh2rgb_backward_kernel<deg><<<grid, 256, 0, st>>>(dirs, rgb_grad, V, N, sh_base_grad, sh_rest_grad);
+        return LGS_OK;
+    });
     LGS_CHECK_LAUNCH("sh2rgb_backward_kernel");
     return LGS_OK;
 }
@@ -818,19 +818,25 @@ extern "C" int lgs_sparse_chunk_op(void* A, const void* B, const int64_t* visibl
     if (alloc_chunks == 0 || ele_num == 0) return LGS_OK;
     dim3 grid(alloc_chunks, ele_num);
     cudaStream_t st = (cudaStream_t)stream;
-#define SC(T, OP) sparse_scatter_kernel<T, OP><<<grid, chunk_size, 0, st>>>((T*)A, (const T*)B, visible_chunk_ids, visible_count, chunks, alloc_chunks)
-#define SCT(T) do { if (op == 0) SC(T, 0); else if (op == 1) SC(T, 1); else SC(T, 2); } while (0)
+    const auto scatter = [&](auto zero) {       // the element type is zero's type
+        using T = decltype(zero);
+        const auto launch = [&](auto o) {
+            sparse_scatter_kernel<T, o><<<grid, chunk_size, 0, st>>>((T*)A, (const T*)B, visible_chunk_ids, visible_count, chunks,
+                                                                      alloc_chunks);
+        };
+        if (op == 0) launch(std::integral_constant<int, 0>{});
+        else if (op == 1) launch(std::integral_constant<int, 1>{});
+        else launch(std::integral_constant<int, 2>{});
+    };
     switch (dtype) {
-        case 0: SCT(float); break;
-        case 1: SCT(int); break;
-        case 2: SCT(double); break;
-        case 3: SCT(long long); break;
-        case 4: SCT(short); break;
-        case 5: SCT(signed char); break;
-        default: SCT(unsigned char); break;
+        case 0: scatter(0.0f); break;
+        case 1: scatter(0); break;
+        case 2: scatter(0.0); break;
+        case 3: scatter(0LL); break;
+        case 4: scatter((short)0); break;
+        case 5: scatter((signed char)0); break;
+        default: scatter((unsigned char)0); break;
     }
-#undef SCT
-#undef SC
     LGS_CHECK_LAUNCH("sparse_scatter_kernel");
     return LGS_OK;
 }

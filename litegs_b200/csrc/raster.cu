@@ -1171,33 +1171,19 @@ extern "C" int lgs_rasterize_forward_packed(const int* sorted_points, const int*
     dim3 grid(lgs_cdiv(nrender, wpb), V), block(32, wpb);
     cudaStream_t st = (cudaStream_t)stream;
     const SplatRec* recs = (const SplatRec*)packed_params;
-#define FWD(S, B) raster_forward_kernel<TH, TW, S, B><<<grid, block, 0, st>>>(sorted_points, start_index, recs, specific_tiles, n_specific, \
-        img, transmittance, (unsigned short*)last_contributor, fragment_count, fragment_weight, tile_work, gx, ntile, cap, N, Hp, Wp, clamp_zero, nullptr, \
-        nullptr, nullptr)
-#define FWDP() raster_forward_kernel<TH, TW, false, false, true><<<grid, block, 0, st>>>(sorted_points, start_index, recs, specific_tiles, \
-        n_specific, img, transmittance, (unsigned short*)last_contributor, fragment_count, fragment_weight, tile_work, gx, ntile, cap, N, Hp, Wp, clamp_zero, nullptr, \
-        nullptr, nullptr)
-#define FWDD(S) raster_forward_kernel<TH, TW, S, false, false, true><<<grid, block, 0, st>>>(sorted_points, start_index, recs, specific_tiles, \
-        n_specific, img, transmittance, (unsigned short*)last_contributor, fragment_count, fragment_weight, tile_work, gx, ntile, cap, N, Hp, Wp, clamp_zero, depth, \
-        nullptr, nullptr)
-#define FWDN(S, Z) raster_forward_kernel<TH, TW, S, false, false, Z, true><<<grid, block, 0, st>>>(sorted_points, start_index, recs,    \
-        specific_tiles, n_specific, img, transmittance, (unsigned short*)last_contributor, fragment_count, fragment_weight, tile_work, gx, \
-        ntile, cap, N, Hp, Wp, clamp_zero, depth, (const float4*)normal_rec, normal)
-    if (normal != nullptr) {
-        LGS_DISPATCH_TILE(tile_h, tile_w,
-            if (depth != nullptr) { if (enable_statistic) FWDN(true, true); else FWDN(false, true); }
-            else { if (enable_statistic) FWDN(true, false); else FWDN(false, false); })
-    } else if (depth != nullptr) {
-        LGS_DISPATCH_TILE(tile_h, tile_w, if (enable_statistic) FWDD(true); else FWDD(false);)
-    } else {
-        LGS_DISPATCH_TILE(tile_h, tile_w,
-            if (enable_statistic) { if (bulk) FWD(true, true); else FWD(true, false); }
-            else { if (bulk) FWD(false, true); else if (forward_pairs()) FWDP(); else FWD(false, false); })
-    }
-#undef FWD
-#undef FWDP
-#undef FWDD
-#undef FWDN
+    // The pixel-pair forward runs without statistics only, and bulk staging wins over it.  Neither renders depth or normals, which
+    // the checks above refuse, so those combinations are not instantiated.
+    const bool pairs = !enable_statistic && !bulk && forward_pairs();
+    const int rc = lgs_with_flags([&](auto nm, auto z, auto stat, auto bk, auto pr) {
+        if constexpr (((bk || pr) && (z || nm)) || (pr && (stat || bk))) return LGS_ERR_ARG;
+        else return lgs_with_tile(tile_h, tile_w, [&](auto th, auto tw) {
+            raster_forward_kernel<th, tw, stat, bk, pr, z, nm><<<grid, block, 0, st>>>(sorted_points, start_index, recs, specific_tiles,
+                n_specific, img, transmittance, (unsigned short*)last_contributor, fragment_count, fragment_weight, tile_work, gx, ntile,
+                cap, N, Hp, Wp, clamp_zero, depth, (const float4*)normal_rec, normal);
+            return LGS_OK;
+        });
+    }, normal != nullptr, depth != nullptr, enable_statistic != 0, bulk, pairs);
+    if (rc != LGS_OK) return rc;
     LGS_CHECK_LAUNCH("raster_forward_kernel");
     return LGS_OK;
 }
@@ -1240,6 +1226,15 @@ extern "C" int lgs_rasterize_backward(const int* sorted_points, const int* start
         const bool trans = d_trans_img != nullptr;
         const bool defer = use_deferred_reduce() && !bulk;
         const unsigned short* lastu = (const unsigned short*)last_contributor;
+        // the pixel-pair kernel, writing the record gradients to grad and the normal gradients to grad_nrm
+        const auto backward_v2 = [&](auto det, float* grad, float* grad_nrm) {
+            return lgs_with_flags([&](auto nm, auto z, auto stat, auto tr) { return lgs_with_tile(tile_h, tile_w, [&](auto th, auto tw) {
+                raster_backward_v2_kernel<th, tw, stat, tr, det, z, nm><<<grid, block, 0, st>>>(sorted_points, start_index, recs,
+                    specific_tiles, n_specific, final_transmittance, lastu, d_img, d_trans_img, clamped_img, grad, gx, ntile, cap, N, Hp,
+                    Wp, g_err_mode, d_depth, (const float4*)normal_rec, d_normal, grad_nrm);
+                return LGS_OK;
+            }); }, nrm, d_depth != nullptr, enable_statistic != 0, trans);
+        };
         if (deterministic()) {
             // integer accumulation in a stream-ordered scratch buffer, converted into packed_grad afterwards
             // (normal mode: the normal rows follow in the same buffer, V*N*4 more slots)
@@ -1247,19 +1242,7 @@ extern "C" int lgs_rasterize_backward(const int* sorted_points, const int* start
             long long* q = nullptr;
             LGS_CUDA(cudaMallocAsync((void**)&q, (nq + nqn) * sizeof(long long), st));
             LGS_CUDA(cudaMemsetAsync(q, 0, (nq + nqn) * sizeof(long long), st));
-#define BWD_DET(S, T, Z, NM) raster_backward_v2_kernel<TH, TW, S, T, true, Z, NM><<<grid, block, 0, st>>>(sorted_points, start_index, \
-        recs, specific_tiles, n_specific, final_transmittance, lastu, d_img, d_trans_img, clamped_img, (float*)q, gx, ntile, cap, N, Hp, Wp, \
-        g_err_mode, d_depth, (const float4*)normal_rec, d_normal, (float*)(q + nq))
-#define BWD_DET_Z(Z, NM) LGS_DISPATCH_TILE(tile_h, tile_w,                                                                \
-                if (enable_statistic) { if (trans) BWD_DET(true, true, Z, NM); else BWD_DET(true, false, Z, NM); }          \
-                else { if (trans) BWD_DET(false, true, Z, NM); else BWD_DET(false, false, Z, NM); })
-            if (nrm) {
-                if (d_depth != nullptr) { BWD_DET_Z(true, true) } else { BWD_DET_Z(false, true) }
-            } else {
-                if (d_depth != nullptr) { BWD_DET_Z(true, false) } else { BWD_DET_Z(false, false) }
-            }
-#undef BWD_DET_Z
-#undef BWD_DET
+            backward_v2(std::true_type{}, (float*)q, (float*)(q + nq));
             LGS_CHECK_LAUNCH("raster_backward_v2_kernel<DET>");
             det_to_float_kernel<<<lgs_cdiv((long long)nq, 256), 256, 0, st>>>(q, packed_grad, nq);
             LGS_CHECK_LAUNCH("det_to_float_kernel");
@@ -1269,32 +1252,21 @@ extern "C" int lgs_rasterize_backward(const int* sorted_points, const int* start
             }
             LGS_CUDA(cudaFreeAsync(q, st));
         } else if (backward_version() == 2 && !bulk) {
-#define BW2(S, T, Z, NM) raster_backward_v2_kernel<TH, TW, S, T, false, Z, NM><<<grid, block, 0, st>>>(sorted_points, start_index, \
-        recs, specific_tiles, n_specific, final_transmittance, lastu, d_img, d_trans_img, clamped_img, packed_grad, gx, ntile, cap, N, Hp, \
-        Wp, g_err_mode, d_depth, (const float4*)normal_rec, d_normal, grad_normal)
-#define BW2_Z(Z, NM) LGS_DISPATCH_TILE(tile_h, tile_w,                                                                     \
-                if (enable_statistic) { if (trans) BW2(true, true, Z, NM); else BW2(true, false, Z, NM); }                  \
-                else { if (trans) BW2(false, true, Z, NM); else BW2(false, false, Z, NM); })
-            if (nrm) {
-                if (d_depth != nullptr) { BW2_Z(true, true) } else { BW2_Z(false, true) }
-            } else {
-                if (d_depth != nullptr) { BW2_Z(true, false) } else { BW2_Z(false, false) }
-            }
-#undef BW2_Z
-#undef BW2
+            backward_v2(std::false_type{}, packed_grad, grad_normal);
             LGS_CHECK_LAUNCH("raster_backward_v2_kernel");
         } else {
-#define BWD(S, T, B) if (defer) BWD2(S, T, false, true); else BWD2(S, T, B, false)
-#define BWD2(S, T, B, D) raster_backward_kernel<TH, TW, S, T, B, D><<<grid, block, 0, st>>>(sorted_points, start_index, recs, specific_tiles, \
-        n_specific, final_transmittance, lastu, d_img, d_trans_img, clamped_img, packed_grad, gx, ntile, cap, N, Hp, Wp)
-        LGS_DISPATCH_TILE(tile_h, tile_w,
-            if (enable_statistic) { if (trans) { if (bulk) BWD(true, true, true); else BWD(true, true, false); }
-                                    else { if (bulk) BWD(true, false, true); else BWD(true, false, false); } }
-            else { if (trans) { if (bulk) BWD(false, true, true); else BWD(false, true, false); }
-                   else { if (bulk) BWD(false, false, true); else BWD(false, false, false); } })
-#undef BWD
-#undef BWD2
-        LGS_CHECK_LAUNCH("raster_backward_kernel");
+            // the scalar kernel; the deferred reduce is off under bulk staging, so that pair is not instantiated
+            const int rc = lgs_with_flags([&](auto stat, auto tr, auto bk, auto df) {
+                if constexpr (bk && df) return LGS_ERR_ARG;
+                else return lgs_with_tile(tile_h, tile_w, [&](auto th, auto tw) {
+                    raster_backward_kernel<th, tw, stat, tr, bk, df><<<grid, block, 0, st>>>(sorted_points, start_index, recs,
+                        specific_tiles, n_specific, final_transmittance, lastu, d_img, d_trans_img, clamped_img, packed_grad, gx, ntile, cap,
+                        N, Hp, Wp);
+                    return LGS_OK;
+                });
+            }, enable_statistic != 0, trans, bulk, defer);
+            if (rc != LGS_OK) return rc;
+            LGS_CHECK_LAUNCH("raster_backward_kernel");
         }
     }
     if (d_ndc != nullptr) {

@@ -452,13 +452,11 @@ int rs_sort(const KeyT* keys_in, KeyT* keys_out, const unsigned* vals_in, unsign
         KeyT* kdst = to_out ? keys_out : ktmp;
         unsigned* vdst = to_out ? vals_out : vtmp;
         const bool vec = ((uintptr_t)ksrc & 15) == 0;
-        if (p.ipt == 16) {
-            if (vec) rs_hist_kernel<KeyT, 16, true><<<p.nblocks, RS_THREADS, 0, st>>>(ksrc, n, bit, nbins, p.nblocks, table, bias, n_dev, bias_dev);
-            else rs_hist_kernel<KeyT, 16, false><<<p.nblocks, RS_THREADS, 0, st>>>(ksrc, n, bit, nbins, p.nblocks, table, bias, n_dev, bias_dev);
-        } else {
-            if (vec) rs_hist_kernel<KeyT, 8, true><<<p.nblocks, RS_THREADS, 0, st>>>(ksrc, n, bit, nbins, p.nblocks, table, bias, n_dev, bias_dev);
-            else rs_hist_kernel<KeyT, 8, false><<<p.nblocks, RS_THREADS, 0, st>>>(ksrc, n, bit, nbins, p.nblocks, table, bias, n_dev, bias_dev);
-        }
+        lgs_with_flags([&](auto ipt16, auto v) {
+            rs_hist_kernel<KeyT, ipt16 ? 16 : 8, v><<<p.nblocks, RS_THREADS, 0, st>>>(ksrc, n, bit, nbins, p.nblocks, table, bias, n_dev,
+                                                                                     bias_dev);
+            return LGS_OK;
+        }, p.ipt == 16, vec);
         LGS_CHECK_LAUNCH("rs_hist_kernel");
         rs_scan_rows_kernel<<<nbins, RS_THREADS, 0, st>>>(table, p.nblocks, totals);
         LGS_CHECK_LAUNCH("rs_scan_rows_kernel");
@@ -466,11 +464,11 @@ int rs_sort(const KeyT* keys_in, KeyT* keys_out, const unsigned* vals_in, unsign
         static const int rank_cap = getenv("LGS_RS_RANK") ? atoi(getenv("LGS_RS_RANK")) : 2;
         int ns = 1;
         while (ns < 4 && ns * 2 <= rank_cap && ns * 2 * RS_WARPS * nbins <= p.tile) ns *= 2;
-#define RS_SCATTER(IPT_, NS_) rs_scatter_kernel<KeyT, IPT_, NS_><<<p.nblocks, RS_THREADS, 0, st>>>(ksrc, vsrc, kdst, vdst, n, bit, nbins, \
-                                                                                             p.nblocks, table, totals, bias, n_dev, bias_dev)
-        if (p.ipt == 16) { if (ns == 4) RS_SCATTER(16, 4); else if (ns == 2) RS_SCATTER(16, 2); else RS_SCATTER(16, 1); }
-        else { if (ns == 4) RS_SCATTER(8, 4); else if (ns == 2) RS_SCATTER(8, 2); else RS_SCATTER(8, 1); }
-#undef RS_SCATTER
+        lgs_with_flags([&](auto ipt16, auto ns4, auto ns2) {
+            rs_scatter_kernel<KeyT, ipt16 ? 16 : 8, ns4 ? 4 : ns2 ? 2 : 1><<<p.nblocks, RS_THREADS, 0, st>>>(
+                ksrc, vsrc, kdst, vdst, n, bit, nbins, p.nblocks, table, totals, bias, n_dev, bias_dev);
+            return LGS_OK;
+        }, p.ipt == 16, ns == 4, ns == 2);
         LGS_CHECK_LAUNCH("rs_scatter_kernel");
         ksrc = kdst; vsrc = vdst;
         bit += dbits;
@@ -513,8 +511,10 @@ int rs_sort_onesweep(const KeyT* keys_in, KeyT* keys_out, const unsigned* vals_i
     }
     LGS_CUDA(cudaMemsetAsync(status, 0, status_words * sizeof(unsigned), st));
     LGS_CUDA(cudaMemsetAsync(ghist, 0, (RS_MAXPASS * RS_MAXBINS + 64) * sizeof(int), st));
-    if (p.ipt == 16) rs_ghist_kernel<KeyT, 16><<<p.nblocks, RS_THREADS, 0, st>>>(keys_in, n, A, ghist, bias, n_dev, bias_dev);
-    else rs_ghist_kernel<KeyT, 8><<<p.nblocks, RS_THREADS, 0, st>>>(keys_in, n, A, ghist, bias, n_dev, bias_dev);
+    lgs_with_flags([&](auto ipt16) {
+        rs_ghist_kernel<KeyT, ipt16 ? 16 : 8><<<p.nblocks, RS_THREADS, 0, st>>>(keys_in, n, A, ghist, bias, n_dev, bias_dev);
+        return LGS_OK;
+    }, p.ipt == 16);
     LGS_CHECK_LAUNCH("rs_ghist_kernel");
     const KeyT* ksrc = keys_in;
     const unsigned* vsrc = vals_in;
@@ -523,12 +523,11 @@ int rs_sort_onesweep(const KeyT* keys_in, KeyT* keys_out, const unsigned* vals_i
         bool to_out = ((p.passes - 1 - pass) & 1) == 0;
         KeyT* kdst = to_out ? keys_out : ktmp;
         unsigned* vdst = to_out ? vals_out : vtmp;
-        if (p.ipt == 16)
-            rs_onesweep_kernel<KeyT, 16><<<p.nblocks, RS_THREADS, 0, st>>>(ksrc, vsrc, kdst, vdst, n, A.shift[pass], A.nbins[pass],
-                                                                          ghist + pass * RS_MAXBINS, status + soff, tickets + pass, bias, n_dev, bias_dev);
-        else
-            rs_onesweep_kernel<KeyT, 8><<<p.nblocks, RS_THREADS, 0, st>>>(ksrc, vsrc, kdst, vdst, n, A.shift[pass], A.nbins[pass],
-                                                                         ghist + pass * RS_MAXBINS, status + soff, tickets + pass, bias, n_dev, bias_dev);
+        lgs_with_flags([&](auto ipt16) {
+            rs_onesweep_kernel<KeyT, ipt16 ? 16 : 8><<<p.nblocks, RS_THREADS, 0, st>>>(ksrc, vsrc, kdst, vdst, n, A.shift[pass],
+                A.nbins[pass], ghist + pass * RS_MAXBINS, status + soff, tickets + pass, bias, n_dev, bias_dev);
+            return LGS_OK;
+        }, p.ipt == 16);
         LGS_CHECK_LAUNCH("rs_onesweep_kernel");
         soff += (size_t)p.nblocks * A.nbins[pass];
         ksrc = kdst; vsrc = vdst;

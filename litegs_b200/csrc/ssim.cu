@@ -261,11 +261,11 @@ extern "C" int lgs_ssim_forward(const float* img1, const float* img2, int B, int
     LGS_REQUIRE(map != nullptr || block_sums != nullptr || train, "ssim_forward: nothing to compute");
     cudaStream_t st = (cudaStream_t)stream;
     dim3 grid((W + CO - 1) / CO, (H + BH - 1) / BH, B * CH);
-#define FWD(L, T) ssim_forward_kernel<L, T><<<grid, CT, 0, st>>>(img1, img2, H, W, C1, C2, ssim_weight, map, dm_dmu1, dm_dsigma1_sq, \
-                                                                 dm_dsigma12, block_sums)
-    if (l1_mode) { if (train) FWD(true, true); else FWD(true, false); }
-    else { if (train) FWD(false, true); else FWD(false, false); }
-#undef FWD
+    lgs_with_flags([&](auto l1, auto tr) {
+        ssim_forward_kernel<l1, tr><<<grid, CT, 0, st>>>(img1, img2, H, W, C1, C2, ssim_weight, map, dm_dmu1, dm_dsigma1_sq, dm_dsigma12,
+                                                         block_sums);
+        return LGS_OK;
+    }, l1_mode != 0, train);
     LGS_CHECK_LAUNCH("ssim_forward_kernel");
     return LGS_OK;
 }
@@ -279,11 +279,11 @@ extern "C" int lgs_ssim_backward(const float* img1, const float* img2, const flo
     LGS_REQUIRE((size_t)B * CH <= 65535, "ssim_backward: B*CH = %d exceeds the grid z limit", B * CH);
     cudaStream_t st = (cudaStream_t)stream;
     dim3 grid((W + CO - 1) / CO, (H + BH - 1) / BH, B * CH);
-#define BWD(L, U) ssim_backward_kernel<L, U><<<grid, CT, 0, st>>>(img1, img2, dL_dmap, uniform_chain, dm_dmu1, dm_dsigma1_sq, dm_dsigma12, H, \
-                                                                  W, ssim_weight, dL_dimg1)
-    if (dL_dmap == nullptr) { if (l1_mode) BWD(true, true); else BWD(false, true); }
-    else { if (l1_mode) BWD(true, false); else BWD(false, false); }
-#undef BWD
+    lgs_with_flags([&](auto uniform, auto l1) {
+        ssim_backward_kernel<l1, uniform><<<grid, CT, 0, st>>>(img1, img2, dL_dmap, uniform_chain, dm_dmu1, dm_dsigma1_sq, dm_dsigma12, H,
+                                                               W, ssim_weight, dL_dimg1);
+        return LGS_OK;
+    }, dL_dmap == nullptr, l1_mode != 0);
     LGS_CHECK_LAUNCH("ssim_backward_kernel");
     return LGS_OK;
 }
