@@ -4,12 +4,15 @@
     python examples/render_ply.py --make /tmp/demo.ply --out /tmp/renders        # writes a synthetic cloud first
     python examples/render_ply.py --ply mip_splatting.ply --filter-3d --antialiased    # a Mip-Splatting checkpoint
     python examples/render_ply.py --make /tmp/demo.ply --out /tmp/renders --depth      # also depth maps (e.g. for TSDF fusion)
+    python examples/render_ply.py --ply point_cloud.ply --depth-normal                  # also the normals of the rendered depth
 
 Cameras: the poses of a COLMAP model when --colmap is given, else the Fibonacci lattice of scene.make_camera.  Forward only
 (the reference's example_metrics.py path): project -> bin -> sort -> composite, no gradients kept.  With --depth each view also
 writes <name>_depth.npy (D = sum w z, the accumulated view-space depth, f32[H,W]) and <name>_alpha.npy (1 - T, f32[H,W]); the
 expected depth is D / alpha where alpha > 0.  With --normal each view also writes <name>_normal.npy, the expected view-space
-normal N / (1 - T) (f32[3,H,W], zero where nothing was blended; DESIGN.md section 1, "Normals").
+normal N / (1 - T) (f32[3,H,W], zero where nothing was blended; DESIGN.md section 1, "Normals").  With --depth-normal each view
+also writes <name>_depth_normal.npy, the unit view-space normal n_d of the surface the expected depth unprojects to (f32[3,H,W],
+zero where it is undefined: the border, 1 - T <= 0.5 at the pixel or a neighbour; DESIGN.md section 1, "Depth-normal consistency").
 """
 import argparse
 import os
@@ -20,7 +23,7 @@ import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from litegs_b200 import colmap, pipeline, ply, scene  # noqa: E402
+from litegs_b200 import colmap, geometry, pipeline, ply, scene  # noqa: E402
 from litegs_b200.dist import PARAM_ORDER  # noqa: E402
 
 
@@ -40,6 +43,7 @@ def main():
                     help="apply the file's filter_3D property (Mip-Splatting's 3D smoothing filter); the file must have it")
     ap.add_argument("--depth", action="store_true", help="also write the accumulated depth D and 1 - T of each view as .npy")
     ap.add_argument("--normal", action="store_true", help="also write the expected view-space normal N / (1 - T) of each view as .npy")
+    ap.add_argument("--depth-normal", action="store_true", help="also write the normal n_d of the rendered expected depth of each view as .npy")
     a = ap.parse_args()
     path = a.ply
     if a.make:
@@ -68,15 +72,15 @@ def main():
         cams = [(scene.make_camera(i, a.views, a.width, a.height), (a.height, a.width), f"view_{i:04d}.png") for i in range(a.views)]
     import PIL.Image
     os.makedirs(a.out, exist_ok=True)
-    imgs, depths, normals = [], [], []
+    imgs, depths, normals, depth_normals = [], [], [], []
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     with torch.no_grad():
         for cam, hw, _ in cams:
             c = {k: torch.from_numpy(v).to(dev) for k, v in cam.items()}
             img, st, _ = pipeline.render_view_forward(P, A[0], A[1], c["frustumplane"], c["view"], c["proj"], a.sh_degree, hw, (8, 16),
-                                                      clamp_zero=True, antialiased=a.antialiased, filter_3d=filt, render_depth=a.depth,
-                                                      render_normal=a.normal)
+                                                      clamp_zero=True, antialiased=a.antialiased, filter_3d=filt,
+                                                      render_depth=a.depth or a.depth_normal, render_normal=a.normal)
             imgs.append(img[0, :, : hw[0], : hw[1]])
             if a.depth:
                 depths.append((st.depth[0, 0, : hw[0], : hw[1]], 1.0 - st.T[0, 0, : hw[0], : hw[1]]))
@@ -84,6 +88,8 @@ def main():
                 alpha = 1.0 - st.T[0, :, : hw[0], : hw[1]]
                 nrm = st.normal[0, :, : hw[0], : hw[1]]
                 normals.append(torch.where(alpha > 0, nrm / alpha.clamp_min(1e-12), torch.zeros_like(nrm)))
+            if a.depth_normal:
+                depth_normals.append(geometry.depth_normal(st.depth[..., : hw[0], : hw[1]], st.T[..., : hw[0], : hw[1]], c["proj"])[0][0])
     torch.cuda.synchronize()
     dt = time.perf_counter() - t0
     for (cam, hw, name), img in zip(cams, imgs):
@@ -94,6 +100,8 @@ def main():
         np.save(os.path.join(a.out, os.path.splitext(name)[0] + "_alpha.npy"), alpha.cpu().numpy())
     for (_, _, name), en in zip(cams, normals):
         np.save(os.path.join(a.out, os.path.splitext(name)[0] + "_normal.npy"), en.cpu().numpy())
+    for (_, _, name), nd in zip(cams, depth_normals):
+        np.save(os.path.join(a.out, os.path.splitext(name)[0] + "_depth_normal.npy"), nd.cpu().numpy())
     print(f"{g['n_points']} Gaussians, {len(cams)} views rendered in {dt * 1e3:.1f} ms ({len(cams) / dt:.0f} views/s forward only) -> {a.out}")
 
 

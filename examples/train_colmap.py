@@ -6,6 +6,7 @@
     python examples/train_colmap.py --make /tmp/noisy --pose-noise 1 0.02 --refine-poses --exact-grad   # ... with the J and SH terms
     python examples/train_colmap.py --make /tmp/synth_depth --depth-weight 0.1     # also supervise the expected depth
     python examples/train_colmap.py --make /tmp/synth_normal --normal-weight 0.1   # also supervise the rendered normals
+    python examples/train_colmap.py --data /path/to/colmap --depth-normal-weight 0.1   # self-supervised depth-normal consistency
 
 Reads ``sparse/0/{cameras,images,points3D}.bin`` and ``images/*`` (litegs_b200.colmap; same files and conventions as the
 reference's ``litegs/io_manager/colmap.py`` + ``litegs/data.py``), initialises Gaussians from the SfM points the way
@@ -17,6 +18,9 @@ ED = D / (1 - T) from the depth mode (DESIGN.md section 1, "Depth").
 With ``--normal-weight W`` and a ``normals/`` directory (``normals/<image stem>.npy``, f32[3,H,W] unit view-space normal, NaN
 where unknown -- ``--make`` writes the hidden scene's N / |N|), the loss gains W * mean(1 - cos(N / |N|, target)) over the known
 pixels, with N from the normal mode (DESIGN.md section 1, "Normals"); it composes with ``--depth-weight``.
+With ``--depth-normal-weight W`` the loss gains W * mean(1 - n_d . N / |N|), n_d the normal of the surface the rendered expected
+depth unprojects to (litegs_b200.geometry, DESIGN.md section 1, "Depth-normal consistency"): it turns depth and normals on and
+needs no ``depths/`` or ``normals/`` directory, so it trains the geometry of a real capture; it composes with every option above.
 """
 import argparse
 import os
@@ -27,7 +31,7 @@ import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from litegs_b200 import colmap, dist as lgs_dist, optimizer, render, scene, ssim  # noqa: E402
+from litegs_b200 import colmap, dist as lgs_dist, geometry, optimizer, render, scene, ssim  # noqa: E402
 from litegs_b200.arguments import PipelineParams  # noqa: E402
 from litegs_b200.dist import PARAM_ORDER  # noqa: E402
 
@@ -153,12 +157,22 @@ def depth_loss_and_grad(depth, trans, target, weight, upstream=1.0):
     return loss, g_ed / a, g_ed * ed / a
 
 
+def depth_normal_angle(depth, trans, normal, proj):
+    """Mean angle in degrees between N / |N| and the depth normal n_d over the pixels where n_d is defined and |N| > 1e-6."""
+    nd, mask = geometry.depth_normal(depth, trans, proj)
+    norm = normal.norm(dim=1, keepdim=True)
+    valid = mask & (norm > 1e-6)
+    cos = (nd * normal / norm.clamp_min(1e-6)).sum(1, keepdim=True).clamp(-1, 1)
+    return float(torch.rad2deg(torch.arccos(cos))[valid].mean()) if bool(valid.any()) else float("nan")
+
+
 def train(root, iters=300, views_per_step=8, log=print, refine_poses=False, antialiased=False, filter_3d=False, exact_grad=False,
-          depth_weight=0.0, metrics=None, normal_weight=0.0):
+          depth_weight=0.0, metrics=None, normal_weight=0.0, depth_normal_weight=0.0):
     """Returns (loss history, PSNR).  depth_weight > 0 adds the expected-depth term (the dataset must have depths/), normal_weight
-    > 0 the normal term (the dataset must have normals/).  metrics (a dict, optional) receives "ed_error": mean |ED - target| over
-    the known pixels of 8 training views, when the dataset has depths, and "normal_angle": their mean angle in degrees between
-    N / |N| and the target, when it has normals."""
+    > 0 the normal term (the dataset must have normals/), depth_normal_weight > 0 the depth-normal consistency term (no targets).
+    metrics (a dict, optional) receives "ed_error": mean |ED - target| over the known pixels of 8 training views, when the dataset
+    has depths, "normal_angle": their mean angle in degrees between N / |N| and the target, when it has normals, and
+    "depth_normal_angle": the mean angle in degrees between N / |N| and n_d where both are defined, with depth_normal_weight > 0."""
     from litegs_b200 import fused
     if refine_poses and int(os.environ.get("WORLD_SIZE", "1")) > 1:
         raise ValueError("--refine-poses runs on one GPU: multi-GPU pose refinement is not supported")
@@ -166,7 +180,7 @@ def train(root, iters=300, views_per_step=8, log=print, refine_poses=False, anti
     fused.CONFIG["true_sigmoid_grad"] = True               # our own loops train with the true sigmoid derivative (SURVEY Q15)
     try:
         return _train(root, iters, views_per_step, log, refine_poses, antialiased, filter_3d, exact_grad, depth_weight, metrics,
-                      normal_weight)
+                      normal_weight, depth_normal_weight)
     finally:
         fused.CONFIG["true_sigmoid_grad"] = keep
 
@@ -204,7 +218,7 @@ class _Poses:
 
 
 def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=False, filter_3d=False, exact_grad=False,
-           depth_weight=0.0, metrics=None, normal_weight=0.0):
+           depth_weight=0.0, metrics=None, normal_weight=0.0, depth_normal_weight=0.0):
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", 0)))
     torch.cuda.set_device(dev)
     frames, xyz, rgb = load_dataset(root, dev=dev)
@@ -216,14 +230,15 @@ def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=Fal
     if normal_weight > 0 and ntargets is None:
         raise ValueError(f"--normal-weight needs unit-normal targets in {os.path.join(root, 'normals')}")
     use_normal = normal_weight > 0
+    use_dn = depth_normal_weight > 0
     H, W = frames[0][2]
     poses = _Poses(frames, (H, W), dev) if refine_poses else None
     extr0 = poses.extr.detach().clone() if poses else None
     cgrads = torch.empty((views_per_step, 2, 4, 4), dtype=torch.float32, device=dev) if poses else None
     g = colmap.gaussians_from_points(xyz, rgb, sh_degree=3)
     P = {k: torch.from_numpy(g[k]).to(dev) for k in PARAM_ORDER}
-    pp = PipelineParams(tile_size=(8, 16), sparse_grad=True, antialiased=antialiased, exact_grad=exact_grad, render_depth=use_depth,
-                        render_normal=use_normal)
+    pp = PipelineParams(tile_size=(8, 16), sparse_grad=True, antialiased=antialiased, exact_grad=exact_grad,
+                        render_depth=use_depth or use_dn, render_normal=use_normal or use_dn)
     acc = lgs_dist.GradAccumulator(P)
     extent = float(np.linalg.norm(xyz.max(0) - xyz.min(0)) * 0.5)
     opt, sched = optimizer.get_optimizer(P, spatial_lr_scale=extent)
@@ -257,10 +272,18 @@ def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=Fal
                 loss, d_img, d_depth, d_trans = colour_and_depth_loss(i, img, depth, trans)
             else:
                 (loss, d_img), d_depth, d_trans = colour_loss(i, img), None, None
-            ln, d_normal, _ = normal_loss_and_grad(normal, ntargets[idx[i]], normal_weight, upstream=1.0 / views_per_step)
-            return loss + ln, d_img, d_depth, d_trans, d_normal
+            d_normal = None
+            if use_normal:
+                ln, d_normal, _ = normal_loss_and_grad(normal, ntargets[idx[i]], normal_weight, upstream=1.0 / views_per_step)
+                loss = loss + ln
+            if use_dn:
+                lc, gd, gt, gn = geometry.depth_normal_loss_and_grad(depth, trans, normal, cams[i]["proj"], depth_normal_weight,
+                                                                     upstream=1.0 / views_per_step)
+                add = lambda a, b: b if a is None else a + b
+                loss, d_depth, d_trans, d_normal = loss + lc, add(d_depth, gd), add(d_trans, gt), add(d_normal, gn)
+            return loss, d_img, d_depth, d_trans, d_normal
 
-        fn = with_normal_loss if use_normal else (colour_and_depth_loss if use_depth else colour_loss)
+        fn = with_normal_loss if (use_normal or use_dn) else (colour_and_depth_loss if use_depth else colour_loss)
         losses = render.render_views(views_per_step, lambda i: cams[i], None, A[0], A[1], P["xyz"], P["scale"], P["rot"],
                                      P["sh_0"], P["sh_rest"], P["opacity"], 3, (H, W), pp, acc.grads(),
                                      loss_and_grad_fn=fn, camera_grads=cgrads, filter_3d=filt)
@@ -273,10 +296,10 @@ def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=Fal
             log(f"iter {it:5d}  loss {hist[-1]:.5f}")
     torch.cuda.synchronize(dev)
     dt = time.perf_counter() - t0
-    pp_eval = PipelineParams(tile_size=(8, 16), sparse_grad=True, antialiased=antialiased, render_depth=targets is not None,
-                             enable_transmitance=targets is not None, render_normal=ntargets is not None)
+    pp_eval = PipelineParams(tile_size=(8, 16), sparse_grad=True, antialiased=antialiased, render_depth=targets is not None or use_dn,
+                             enable_transmitance=targets is not None or use_dn, render_normal=ntargets is not None or use_dn)
     with torch.no_grad():
-        mse, ed_err, n_err = [], [], []
+        mse, ed_err, n_err, dn_err = [], [], [], []
         for j, (cam, gt, _) in enumerate(frames[:8]):
             cam = poses.cameras([j])[0] if poses else cam
             img, trans, depth, normal, _ = render.render_view(A[0], A[1], cam["frustumplane"], cam["view"], cam["proj"], P["xyz"],
@@ -287,6 +310,8 @@ def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=Fal
                 ed_err.append(float(depth_loss_and_grad(depth, trans, targets[j], 1.0)[0]))
             if ntargets is not None:
                 n_err.append(float(normal_loss_and_grad(normal, ntargets[j], 1.0)[2]))
+            if use_dn:
+                dn_err.append(depth_normal_angle(depth, trans, normal, cam["proj"]))
     psnr = -10.0 * np.log10(np.mean(mse))
     if ed_err:
         log(f"expected-depth error over 8 training views: {np.mean(ed_err):.4f}")
@@ -296,6 +321,10 @@ def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=Fal
         log(f"mean angle between N / |N| and the target normals over 8 training views: {np.mean(n_err):.2f} degrees")
         if metrics is not None:
             metrics["normal_angle"] = float(np.mean(n_err))
+    if dn_err:
+        log(f"mean angle between N / |N| and the depth normal n_d over 8 training views: {np.mean(dn_err):.2f} degrees")
+        if metrics is not None:
+            metrics["depth_normal_angle"] = float(np.mean(dn_err))
     log(f"{iters} iterations x {views_per_step} views in {dt:.1f} s ({iters * views_per_step / dt:.0f} views/s incl. loss + optimizer); "
         f"{xyz.shape[0]} Gaussians, PSNR over 8 training views {psnr:.2f} dB")
     if poses:
@@ -320,6 +349,9 @@ if __name__ == "__main__":
     ap.add_argument("--normal-weight", type=float, default=0.0,
                     help="weight of the mean (1 - cos) term between N / |N| and the target normals (needs normals/<image stem>.npy, "
                          "written by --make)")
+    ap.add_argument("--depth-normal-weight", type=float, default=0.0,
+                    help="weight of the mean (1 - cos) term between N / |N| and the normal of the rendered expected depth (needs no "
+                         "targets)")
     ap.add_argument("--pose-noise", type=float, nargs=2, default=None, metavar=("DEG", "FRAC"),
                     help="with --make: perturb the written poses by DEG degrees and FRAC of the camera distance")
     a = ap.parse_args()
@@ -329,5 +361,6 @@ if __name__ == "__main__":
     if root is None:
         ap.error("give --data or --make")
     h, _ = train(root, a.iters, refine_poses=a.refine_poses, antialiased=a.antialiased, filter_3d=a.filter_3d,
-                 exact_grad=a.exact_grad, depth_weight=a.depth_weight, normal_weight=a.normal_weight)
+                 exact_grad=a.exact_grad, depth_weight=a.depth_weight, normal_weight=a.normal_weight,
+                 depth_normal_weight=a.depth_normal_weight)
     assert h[-1] < h[0]

@@ -419,6 +419,26 @@ int lgs_ssim_backward(const float* img1, const float* img2, const float* dL_dmap
                       const float* dm_dsigma1_sq, const float* dm_dsigma12, int B, int CH, int H, int W, int l1_mode,
                       float ssim_weight, float* dL_dimg1, void* stream);
 
+/* ---- depth-normal consistency (ours) --------------------------------------------------------------------------------- */
+
+/* Depth-normal consistency of one view, ours (DESIGN.md section 1, "Depth-normal consistency"; 2DGS, PGSR, RaDe-GS).  Inputs on
+ * the device: the depth mode's D and the transmittance T, f32[H,W] planes with row strides depth_row_stride, trans_row_stride
+ * (elements); the normal mode's N, three f32[H,W] planes with the given row and channel strides (nullable when neither the
+ * loss nor the gradient is asked for); proj f32[4,4] (row-vector), of which P[0][0] and P[1][1] are read on the device.
+ * With alpha = 1 - T, ED = D / alpha, fx = P[0][0] W / 2, fy = P[1][1] H / 2 and r(u,v) = ((u + 0.5 - W/2) / fx,
+ * (v + 0.5 - H/2) / fy, 1), X = ED r: at pixel p, a = X(u+1,v) - X(u-1,v), b = X(u,v+1) - X(u,v-1), n_d = (b x a) / |b x a|,
+ * defined where p is at least one pixel from the border, alpha > alpha_min at p and its four neighbours, and |b x a| > 0.
+ * There, with |N_p| > 1e-6 as well, l_p = 1 - n_d . N_p / |N_p|.  Outputs, contiguous, each optional:
+ *   n_d f32[3,H,W] (zero where n_d is undefined);
+ *   d_depth, d_trans f32[H,W] and d_normal f32[3,H,W], all or none: grad_scale * d(sum_p l_p) / d(D, T, N), the masks held constant
+ *     (grad_scale = weight * upstream / (H W) gives the gradient of L = weight * mean_p l_p);
+ *   block_sums f32[count of lgs_depth_normal_num_block_sums] = sum of l_p over each CTA's tile (sum them in order).
+ * alpha_min in [0, 1).  One kernel, no atomics (bit-reproducible), no host synchronisation. */
+int lgs_depth_normal_num_block_sums(int H, int W, int* count);
+int lgs_depth_normal(const float* depth, int depth_row_stride, const float* trans, int trans_row_stride, const float* normal,
+                     int normal_row_stride, int normal_channel_stride, const float* proj, int H, int W, float alpha_min, float grad_scale,
+                     float* n_d, float* d_depth, float* d_trans, float* d_normal, float* block_sums, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

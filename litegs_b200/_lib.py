@@ -86,6 +86,8 @@ SIGNATURES = {
     "lgs_ssim_num_block_sums": [_I, _I, _I, _I, ctypes.POINTER(_I)],
     "lgs_ssim_forward": [_P, _P, _I, _I, _I, _I, _F, _F, _I, _F, _P, _P, _P, _P, _P, _P],
     "lgs_ssim_backward": [_P, _P, _P, _F, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P, _P],
+    "lgs_depth_normal_num_block_sums": [_I, _I, ctypes.POINTER(_I)],
+    "lgs_depth_normal": [_P, _I, _P, _I, _P, _I, _I, _P, _I, _I, _F, _F, _P, _P, _P, _P, _P, _P],
 }
 NO_STATUS = {"lgs_last_error": ctypes.c_char_p, "lgs_abi_version": ctypes.c_int}
 
