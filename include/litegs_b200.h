@@ -254,8 +254,9 @@ int lgs_set_warps_per_block(int wpb);
 int lgs_set_forward_pairs(int on);
 /* backward kernel: 2 = pixel pairs, branch-free pixel body (default); 1 = scalar kernel.  env LGS_BWD=v1|v2 */
 int lgs_set_backward_kernel(int version);
-/* 1 = deterministic backward: per-(tile, splat) sums accumulated as 64-bit fixed point with integer atomics (associative, so
- * two runs give bit-identical gradients; scratch from the stream-ordered allocator); 0 = fp32 RED atomics (default, faster).
+/* 1 = deterministic backward: per-(tile, splat) sums accumulated as fixed point, two 64-bit words per value (range 3.6e16,
+ * resolution 3.6e-15), with integer atomics (associative, so two runs give bit-identical gradients; scratch from the
+ * stream-ordered allocator); 0 = fp32 RED atomics (default, faster).
  * env LGS_DETERMINISTIC=1 */
 int lgs_set_deterministic(int on);
 /* err_square_sum under enable_statistic: 1 = the reference's lane-running recurrence (GR/raster.cu:779-784, default),

@@ -698,10 +698,21 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_kernel(
 __device__ __forceinline__ float2 bc2(float a) { return make_float2(a, a); }
 
 // DET (deterministic mode, lgs_set_deterministic): the per-(tile, splat) sums -- themselves computed in a fixed order inside the
-// warp -- are accumulated as 64-bit FIXED-POINT integers (scale 2^36) with integer atomics, which are associative: the result no
-// longer depends on the order in which tiles reach a splat, so two runs give bit-identical gradients (SURVEY 7 asks for such a
-// mode next to the fp32 RED default, whose run-to-run spread is ~1e-6 relative).  `grad` then points at i64[N][LGS_GRAD_FLOATS].
-#define LGS_DET_SCALE 68719476736.0                      // 2^36: |value| < 1.3e8, resolution 1.5e-11
+// warp -- are accumulated as FIXED-POINT integers with integer atomics, which are associative: the result no longer depends on the
+// order in which tiles reach a splat, so two runs give bit-identical gradients (SURVEY 7 asks for such a mode next to the fp32 RED
+// default, whose run-to-run spread is ~1e-6 relative).  Each slot is two 64-bit words, summed separately (det_add):
+//   hi = floor(v 2^8)   lo = round((v 2^8 - hi) 2^40)   value = hi 2^-8 + lo 2^-48
+// so a slot's total may reach 2^63 / 2^8 = 3.6e16 (slot 2, sum dx^2 dpw with dx in pixels, passes 1e8 for a screen-sized splat),
+// one contribution may be as large, the resolution is 2^-48 = 3.6e-15, and lo (< 2^40 + 1 per contribution) has room for 2^23
+// contributions per slot.  `grad` then points at i64[N][LGS_GRAD_FLOATS][2].
+#define LGS_DET_HI 256.0                                 // 2^8
+#define LGS_DET_LO 1099511627776.0                       // 2^40
+__device__ __forceinline__ void det_add(unsigned long long* q, float v)
+{
+    const double s = (double)v * LGS_DET_HI, h = floor(s);
+    atomicAdd(&q[0], (unsigned long long)(long long)h);
+    atomicAdd(&q[1], (unsigned long long)__double2ll_rn((s - h) * LGS_DET_LO));
+}
 // DEPTH: d_depth f32[V,1,Hp,Wp] = dL/dD is one more colour channel with "colour" z (the staged pad0): z g_z joins the (c - R) . g
 // dot product, and sum w g_z is reduced into slot LGS_GRAD_DEPTH.  That value is the last row of a parked splat; with STAT it makes
 // 11 rows, so only 2 splats are parked per flush (RG * NV <= 32 lanes).
@@ -741,10 +752,10 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
     const int start = rg[tile_id];
     if (start < 0) return;
     recs += (size_t)b * N;
-    grad += (size_t)b * N * LGS_GRAD_FLOATS * (DET ? 2 : 1);          // DET: 64-bit slots
+    grad += (size_t)b * N * LGS_GRAD_FLOATS * (DET ? 4 : 1);          // DET: two 64-bit words per slot
     if (NORMAL) {
         nrec += (size_t)b * N;
-        grad_normal += (size_t)b * N * 4 * (DET ? 2 : 1);
+        grad_normal += (size_t)b * N * 4 * (DET ? 4 : 1);
     }
     const int* ids = sorted + (size_t)b * cap + start;
 
@@ -810,15 +821,10 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
             const int v = (DEPTH && row == ROW_Z) ? LGS_GRAD_DEPTH : row;         // gradient slot of the row
             const int pid = s_pid[warp][sp];
             if (NORMAL && row >= ROW_N) {                                            // normal rows -> the side array
-                if (DET) {
-                    unsigned long long* gq = reinterpret_cast<unsigned long long*>(grad_normal);
-                    atomicAdd(&gq[(size_t)pid * 4 + (row - ROW_N)], (unsigned long long)__double2ll_rn((double)sum * LGS_DET_SCALE));
-                } else {
-                    atomicAdd(&grad_normal[(size_t)pid * 4 + (row - ROW_N)], sum);
-                }
+                if (DET) det_add(reinterpret_cast<unsigned long long*>(grad_normal) + 2 * ((size_t)pid * 4 + (row - ROW_N)), sum);
+                else atomicAdd(&grad_normal[(size_t)pid * 4 + (row - ROW_N)], sum);
             } else if (DET) {
-                unsigned long long* gq = reinterpret_cast<unsigned long long*>(grad);
-                atomicAdd(&gq[(size_t)pid * LGS_GRAD_FLOATS + v], (unsigned long long)__double2ll_rn((double)sum * LGS_DET_SCALE));
+                det_add(reinterpret_cast<unsigned long long*>(grad) + 2 * ((size_t)pid * LGS_GRAD_FLOATS + v), sum);
             } else {
                 atomicAdd(&grad[(size_t)pid * LGS_GRAD_FLOATS + v], sum);                        // RED.ADD.F32
             }
@@ -954,11 +960,11 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
     st.drain();
 }
 
-// deterministic mode: 64-bit fixed point -> the fp32 gradient record
+// deterministic mode: the two fixed-point words of each slot (det_add) -> the fp32 gradient record
 __global__ void det_to_float_kernel(const long long* __restrict__ q, float* __restrict__ g, size_t n)
 {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) g[i] = (float)((double)q[i] * (1.0 / LGS_DET_SCALE));
+    if (i < n) g[i] = (float)((double)q[2 * i] * (1.0 / LGS_DET_HI) + (double)q[2 * i + 1] * (1.0 / (LGS_DET_HI * LGS_DET_LO)));
 }
 
 // ---- unpack ----------------------------------------------------------------------------------------
@@ -1236,18 +1242,18 @@ extern "C" int lgs_rasterize_backward(const int* sorted_points, const int* start
             }); }, nrm, d_depth != nullptr, enable_statistic != 0, trans);
         };
         if (deterministic()) {
-            // integer accumulation in a stream-ordered scratch buffer, converted into packed_grad afterwards
+            // integer accumulation in a stream-ordered scratch buffer, two words per slot, converted into packed_grad afterwards
             // (normal mode: the normal rows follow in the same buffer, V*N*4 more slots)
             const size_t nq = (size_t)V * N * LGS_GRAD_FLOATS, nqn = nrm ? (size_t)V * N * 4 : 0;
             long long* q = nullptr;
-            LGS_CUDA(cudaMallocAsync((void**)&q, (nq + nqn) * sizeof(long long), st));
-            LGS_CUDA(cudaMemsetAsync(q, 0, (nq + nqn) * sizeof(long long), st));
-            backward_v2(std::true_type{}, (float*)q, (float*)(q + nq));
+            LGS_CUDA(cudaMallocAsync((void**)&q, 2 * (nq + nqn) * sizeof(long long), st));
+            LGS_CUDA(cudaMemsetAsync(q, 0, 2 * (nq + nqn) * sizeof(long long), st));
+            backward_v2(std::true_type{}, (float*)q, (float*)(q + 2 * nq));
             LGS_CHECK_LAUNCH("raster_backward_v2_kernel<DET>");
             det_to_float_kernel<<<lgs_cdiv((long long)nq, 256), 256, 0, st>>>(q, packed_grad, nq);
             LGS_CHECK_LAUNCH("det_to_float_kernel");
             if (nrm) {
-                det_to_float_kernel<<<lgs_cdiv((long long)nqn, 256), 256, 0, st>>>(q + nq, grad_normal, nqn);
+                det_to_float_kernel<<<lgs_cdiv((long long)nqn, 256), 256, 0, st>>>(q + 2 * nq, grad_normal, nqn);
                 LGS_CHECK_LAUNCH("det_to_float_kernel");
             }
             LGS_CUDA(cudaFreeAsync(q, st));
