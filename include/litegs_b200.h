@@ -115,7 +115,8 @@ int lgs_sh2rgb_backward(int degree, const float* rgb_grad, int sh_rest_dim, cons
 /* ---- binning ----------------------------------------------------------------------------------------- */
 
 /* get_allocate_size, GR/binning.cu:289-440 (GR/binning.h:11-15): visibility + exact ellipse/tile overlap
- * count (GR/speedy_splat.cuh:33-149). left_up/right_down i32[V,2,N], allocate_size i32[V,N] (zeroed). */
+ * count (GR/speedy_splat.cuh:33-149). left_up/right_down i32[V,2,N], allocate_size i32[V,N] (zeroed).
+ * The tile rectangle's last row / column follows lgs_set_exact_tile_bound. */
 int lgs_get_allocate_size(const float* ndc, const float* view_space_z, const float* inv_cov2d, const float* opacity,
                           const int* valid_length, int V, int N, int height, int width, int tile_h, int tile_w,
                           int* left_up, int* right_down, int* allocate_size, void* stream);
@@ -123,12 +124,19 @@ int lgs_get_allocate_size(const float* ndc, const float* view_space_z, const flo
 /* create_table, GR/binning.cu:33-226 (GR/binning.h:5-9): emit (tile+1, splat) in depth order at `offset`
  * (inclusive scan, i32[V,N]) then a stable radix sort on the tile bits.  cap = table length; outputs
  * i32[V,cap].  The reference sizes the table from a pinned feedback buffer (GR/binning.cu:137-163);
- * that policy lives in the host mirror, the C entry point takes `cap` explicitly. */
+ * that policy lives in the host mirror, the C entry point takes `cap` explicitly.
+ * The counts in `offset` must have been made under the same lgs_set_exact_tile_bound setting. */
 int lgs_create_table_workspace_bytes(int V, int cap, size_t* bytes);
 int lgs_create_table(const float* ndc, const float* inv_cov2d, const float* opacity, const int* offset,
                      const int64_t* depth_sorted_pointid, int V, int N, int cap, int height, int width, int tile_h,
                      int tile_w, int* sorted_tile_id, int* sorted_point_id, void* workspace, size_t workspace_bytes,
                      void* stream);
+
+/* Tile rectangle of lgs_get_allocate_size / lgs_create_table.  1 (default): it ends after the tile holding bbox_max,
+ * floor((bbox_max + T) / T), so every tile holding a pixel centre where the splat's alpha reaches 1/255 is listed;
+ * 0: the reference's floor((bbox_max + T - 1) / T) (GR/binning.cu:88-91), which drops a tile the ellipse reaches by less
+ * than a pixel (DESIGN.md section 7, D14).  The fused pipeline always uses 1.  Process-wide, like lgs_set_staging. */
+int lgs_set_exact_tile_bound(int on);
 
 /* tileRange, GR/binning.cu:228-287 (GR/binning.h:10). tile_range i32[V,max_tile_id+2], -1 = empty.
  * fix_last=1 closes the last populated tile (the reference leaves it open: SURVEY Q3); 0 = bit-compatible. */

@@ -33,6 +33,7 @@ SIGNATURES = {
     "lgs_get_allocate_size": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P],
     "lgs_create_table_workspace_bytes": [_I, _I, ctypes.POINTER(_Z)],
     "lgs_create_table": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _Z, _P],
+    "lgs_set_exact_tile_bound": [_I],
     "lgs_tile_range": [_P, _I, _I, _I, _I, _P, _P],
     "lgs_tile_range_u16": [_P, _I, _I, _I, _I, _P, _P],
     "lgs_sort_pairs_u16_workspace_bytes": [_I, ctypes.POINTER(_Z)],

@@ -13,13 +13,17 @@
 #include "common.cuh"
 #include "splat_geom.cuh"
 
+// Level A tile rectangle: 1 = floor((bbox_max + T) / T), 0 = the reference's rule (lgs_set_exact_tile_bound, DESIGN.md D14)
+static int g_exact_tile_bound = 1;
+extern "C" int lgs_set_exact_tile_bound(int on) { g_exact_tile_bound = on ? 1 : 0; return LGS_OK; }
+
 // ------------------------------------------------------------------------------------------------
 // per-splat pixel bbox + tile count.                                  replaces GR/binning.cu:289-440
 // ------------------------------------------------------------------------------------------------
 template <int TH, int TW>
 __global__ void __launch_bounds__(256) allocate_size_kernel(
     const float* __restrict__ ndc, const float* __restrict__ viewz, const float* __restrict__ inv_cov,
-    const float* __restrict__ opac, const int* __restrict__ valid_length, int N, int H, int W, int gx, int gy,
+    const float* __restrict__ opac, const int* __restrict__ valid_length, int N, int H, int W, int gx, int gy, bool exact_bound,
     int* __restrict__ left_up, int* __restrict__ right_down, int* __restrict__ alloc)
 {
     int i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
@@ -27,7 +31,7 @@ __global__ void __launch_bounds__(256) allocate_size_kernel(
     size_t o4 = (size_t)b * 4 * N + i, o2 = (size_t)b * 2 * N + i;
     SplatGeom g;
     lgs_splat_setup<TH, TW>(ndc[o4], ndc[o4 + N], viewz[(size_t)b * N + i], inv_cov[o4], inv_cov[o4 + N],
-                            inv_cov[o4 + 3 * (size_t)N], opac[i], H, W, gx, gy, true, g);
+                            inv_cov[o4 + 3 * (size_t)N], opac[i], H, W, gx, gy, true, g, exact_bound);
     if (g.visible) {
         left_up[o2] = lgs_f2i_rz(ceilf(g.bbox_min[0])); left_up[o2 + N] = lgs_f2i_rz(ceilf(g.bbox_min[1]));
         right_down[o2] = lgs_f2i_rz(floorf(g.bbox_max[0])); right_down[o2 + N] = lgs_f2i_rz(floorf(g.bbox_max[1]));
@@ -52,7 +56,7 @@ extern "C" int lgs_get_allocate_size(const float* ndc, const float* view_space_z
     dim3 grid(lgs_cdiv(N, 256), V);
     lgs_with_tile(tile_h, tile_w, [&](auto th, auto tw) {
         allocate_size_kernel<th, tw><<<grid, 256, 0, st>>>(ndc, view_space_z, inv_cov2d, opacity, valid_length, N, height, width,
-                                                          gx, gy, left_up, right_down, allocate_size);
+                                                          gx, gy, g_exact_tile_bound != 0, left_up, right_down, allocate_size);
         return LGS_OK;
     });
     LGS_CHECK_LAUNCH("allocate_size_kernel");
@@ -66,7 +70,7 @@ template <int TH, int TW>
 __global__ void __launch_bounds__(256) emit_pairs_kernel(
     const float* __restrict__ ndc, const float* __restrict__ inv_cov, const float* __restrict__ opac,
     const int* __restrict__ offset /*inclusive scan, depth order*/, const int64_t* __restrict__ sorted_id,
-    int N, int cap, int H, int W, int gx, int gy, int* __restrict__ keys, int* __restrict__ vals)
+    int N, int cap, int H, int W, int gx, int gy, bool exact_bound, int* __restrict__ keys, int* __restrict__ vals)
 {
     int j = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
     if (j >= N) return;
@@ -77,7 +81,7 @@ __global__ void __launch_bounds__(256) emit_pairs_kernel(
     size_t o4 = (size_t)b * 4 * N + i;
     SplatGeom g;
     lgs_splat_setup<TH, TW>(ndc[o4], ndc[o4 + N], 1.0f, inv_cov[o4], inv_cov[o4 + N], inv_cov[o4 + 3 * (size_t)N], opac[i],
-                            H, W, gx, gy, false, g);
+                            H, W, gx, gy, false, g, exact_bound);
     if (g.visible) lgs_process_tiles<TH, TW, true>(g, gx, i, off, cap, keys + (size_t)b * cap, vals + (size_t)b * cap);
 }
 
@@ -127,7 +131,7 @@ extern "C" int lgs_create_table(const float* ndc, const float* inv_cov2d, const 
         dim3 grid(lgs_cdiv(N, 256), V);
         lgs_with_tile(tile_h, tile_w, [&](auto th, auto tw) {
             emit_pairs_kernel<th, tw><<<grid, 256, 0, st>>>(ndc, inv_cov2d, opacity, offset, depth_sorted_pointid, N, cap, height,
-                                                           width, gx, gy, keys, vals);
+                                                           width, gx, gy, g_exact_tile_bound != 0, keys, vals);
             return LGS_OK;
         });
         LGS_CHECK_LAUNCH("emit_pairs_kernel");

@@ -51,9 +51,14 @@ __device__ __forceinline__ void lgs_ellipse_isect(float A, float B, float C, flo
 
 // check_visibility=false reproduces the emit kernel, which trusts the count it was given
 // (GR/binning.cu:63) and skips the ndc / depth tests.
+// exact_bound: the last tile row / column of the rectangle is the one holding bbox_max, floor((bbox_max + T) / T), so a
+// splat whose ellipse reaches pixel centre kT keeps tile k even when bbox_max < kT + 1.  false = the reference's
+// floor((bbox_max + T - 1) / T) (GR/binning.cu:88-91), which treats bbox_max as an integer pixel bound and drops that tile
+// (DESIGN.md section 7, D14).  The count and the emit of one list must use the same rule.
 template <int TH, int TW>
 __device__ __forceinline__ void lgs_splat_setup(float ndcx, float ndcy, float viewz, float A, float B, float C, float o,
-                                                int H, int W, int gx, int gy, bool check_visibility, SplatGeom& g)
+                                                int H, int W, int gx, int gy, bool check_visibility, SplatGeom& g,
+                                                bool exact_bound = true)
 {
     g.A = A; g.B = B; g.C = C;
     g.disc = __fsub_rn(__fmul_rn(B, B), __fmul_rn(A, C));
@@ -83,8 +88,9 @@ __device__ __forceinline__ void lgs_splat_setup(float ndcx, float ndcy, float vi
     lgs_ellipse_isect(A, B, C, g.inv_A, g.inv_C, g.disc, t, g.px, g.py, false, g.argmax[1], lo, hi); g.bbox_max[1] = hi;
     g.rect_min[0] = max(0, min(gx, lgs_f2i_rz(lgs_div_tile<TW>(g.bbox_min[0]))));
     g.rect_min[1] = max(0, min(gy, lgs_f2i_rz(lgs_div_tile<TH>(g.bbox_min[1]))));
-    g.rect_max[0] = max(0, min(gx, lgs_f2i_rz(lgs_div_tile<TW>(__fsub_rn(__fadd_rn(g.bbox_max[0], (float)TW), 1.0f)))));
-    g.rect_max[1] = max(0, min(gy, lgs_f2i_rz(lgs_div_tile<TH>(__fsub_rn(__fadd_rn(g.bbox_max[1], (float)TH), 1.0f)))));
+    const float ex = __fadd_rn(g.bbox_max[0], (float)TW), ey = __fadd_rn(g.bbox_max[1], (float)TH);
+    g.rect_max[0] = max(0, min(gx, lgs_f2i_rz(lgs_div_tile<TW>(exact_bound ? ex : __fsub_rn(ex, 1.0f)))));
+    g.rect_max[1] = max(0, min(gy, lgs_f2i_rz(lgs_div_tile<TH>(exact_bound ? ey : __fsub_rn(ey, 1.0f)))));
 }
 
 // Walks the tile slices of one splat; returns the number of tiles and, when EMIT, writes

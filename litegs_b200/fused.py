@@ -25,7 +25,9 @@ _F32, _I32, _I64 = torch.float32, torch.int32, torch.int64
 
 # Deviations that can be switched back to bit-compatibility with the reference (SURVEY Q3, Q15)
 CONFIG = {
-    "fix_last_tile": True,          # close the last populated tile's range (reference leaves it empty)
+    # close the last populated tile's range (reference leaves it empty, Q3) and keep the tile a splat reaches by less than a
+    # pixel (the reference drops it, DESIGN.md section 7, D14); False = the reference's tile tables bit for bit
+    "fix_last_tile": True,
     "true_sigmoid_grad": False,     # False = reference's d_o * sigma(x) on the cluster path
     "tile_order": os.environ.get("LGS_TILE_ORDER", "1") != "0",   # fused pipeline: backward tiles launched heaviest-first (lgs_tile_order)
 }
@@ -319,6 +321,7 @@ def get_allocate_size(ndc, view_space_z, inv_cov2d, opacity, height, width, tile
     V, N = n.shape[0], n.shape[2]
     dev = n.device
     with torch.cuda.device(dev):
+        _lib.call("lgs_set_exact_tile_bound", int(bool(CONFIG["fix_last_tile"])))
         lu = torch.empty((V, 2, N), dtype=_I32, device=dev)
         rd = torch.empty((V, 2, N), dtype=_I32, device=dev)
         al = torch.empty((V, N), dtype=_I32, device=dev)
@@ -354,6 +357,7 @@ def create_table(ndc, inv_cov2d, opacity, offset, depth_sorted_pointid, feedback
         ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
         keys = torch.empty((V, pred), dtype=_I32, device=dev)
         vals = torch.empty((V, pred), dtype=_I32, device=dev)
+        _lib.call("lgs_set_exact_tile_bound", int(bool(CONFIG["fix_last_tile"])))
         _lib.call("lgs_create_table", _ptr(n), _ptr(c), _ptr(o), _ptr(off), _ptr(sid), V, N, pred, int(height), int(width),
                   int(tile_size_h), int(tile_size_w), _ptr(keys), _ptr(vals), _ptr(ws), ctypes.c_size_t(nbytes.value), _stream(dev))
     return [keys, vals]

@@ -244,22 +244,29 @@ def sh2rgb_backward(degree, rgb_grad, sh_rest_dim, dirs, sh_base=None, sh_rest=N
     return g0, gr, np.zeros_like(dirs)
 
 
-def get_allocate_size(ndc, view_space_z, inv_cov2d, opacity, height, width, tile_h, tile_w, valid_length=None):
-    """GR/binning.cu:398-440 -> (left_up i32[V,2,N], right_down i32[V,2,N], allocate_size i32[V,N])."""
+def get_allocate_size(ndc, view_space_z, inv_cov2d, opacity, height, width, tile_h, tile_w, valid_length=None,
+                      exact_tile_bound=True):
+    """GR/binning.cu:398-440 -> (left_up i32[V,2,N], right_down i32[V,2,N], allocate_size i32[V,N]).
+
+    exact_tile_bound=False: the reference's last tile row / column, floor((bbox_max + T - 1) / T), which drops a tile the
+    ellipse reaches by less than a pixel (DESIGN.md section 7, D14); True: floor((bbox_max + T) / T)."""
     dt = ndc.dtype; V = ndc.shape[0]; N = ndc.shape[2]
     lu = np.zeros((V, 2, N), np.int32); rd = np.zeros((V, 2, N), np.int32); al = np.zeros((V, N), np.int32)
     _call("orc_get_allocate_size", dt, _c(ndc), _c(view_space_z, dt), _c(inv_cov2d, dt), _c(opacity, dt),
-          V, N, _valid(valid_length, N), int(height), int(width), int(tile_h), int(tile_w), lu, rd, al)
+          V, N, _valid(valid_length, N), int(height), int(width), int(tile_h), int(tile_w), int(bool(exact_tile_bound)), lu, rd, al)
     return lu, rd, al
 
 
-def create_table(ndc, inv_cov2d, opacity, offset, depth_sorted_pointid, allocate, height, width, tile_h, tile_w):
-    """GR/binning.cu:123-226 with the table size given explicitly -> (sorted_tileId, sorted_pointId) i32[V,allocate]."""
+def create_table(ndc, inv_cov2d, opacity, offset, depth_sorted_pointid, allocate, height, width, tile_h, tile_w,
+                 exact_tile_bound=True):
+    """GR/binning.cu:123-226 with the table size given explicitly -> (sorted_tileId, sorted_pointId) i32[V,allocate].
+    exact_tile_bound: as in get_allocate_size; the offsets must come from counts made with the same rule."""
     dt = ndc.dtype; V = ndc.shape[0]; N = ndc.shape[2]
     cap = int(allocate)
     keys = np.zeros((V, cap), np.int32); vals = np.zeros((V, cap), np.int32)
     _call("orc_create_table", dt, _c(ndc), _c(inv_cov2d, dt), _c(opacity, dt), _c(offset, np.int32),
-          _c(depth_sorted_pointid, np.int64), V, N, cap, int(height), int(width), int(tile_h), int(tile_w), keys, vals)
+          _c(depth_sorted_pointid, np.int64), V, N, cap, int(height), int(width), int(tile_h), int(tile_w),
+          int(bool(exact_tile_bound)), keys, vals)
     return keys, vals
 
 
@@ -338,15 +345,18 @@ def adamUpdate(param, grad, exp_avg, exp_avg_sq, visible_index, valid_length, lr
 # ---------------------------------------------------------------------------------------------
 
 def binning(ndc, view_depth, inv_cov2d, opacity, valid_length, img_hw, tile_hw, fix_last=True):
-    """wrapper.py:718-763: count -> stable depth sort -> inclusive scan -> emit -> tile sort -> ranges."""
+    """wrapper.py:718-763: count -> stable depth sort -> inclusive scan -> emit -> tile sort -> ranges.
+    fix_last=False reproduces the reference's tables: the last populated tile's range left open (SURVEY Q3) and the
+    reference's tile rectangle (exact_tile_bound=False, DESIGN.md section 7, D14), as litegs_fused.CONFIG["fix_last_tile"]."""
+    exact_tile_bound = bool(fix_last)
     H, W = img_hw; th, tw = tile_hw
     gy = (H + th - 1) // th; gx = (W + tw - 1) // tw
-    _, _, alloc = get_allocate_size(ndc, view_depth, inv_cov2d, opacity, H, W, th, tw, valid_length)
+    _, _, alloc = get_allocate_size(ndc, view_depth, inv_cov2d, opacity, H, W, th, tw, valid_length, exact_tile_bound)
     order = np.argsort(view_depth, axis=-1, kind="stable").astype(np.int64)
     sorted_alloc = np.take_along_axis(alloc, order, axis=-1)
     prefix = np.cumsum(sorted_alloc, axis=-1, dtype=np.int64).astype(np.int32)
     total = max(int(prefix[:, -1].max()), 1)
-    keys, vals = create_table(ndc, inv_cov2d, opacity, prefix, order, total, H, W, th, tw)
+    keys, vals = create_table(ndc, inv_cov2d, opacity, prefix, order, total, H, W, th, tw, exact_tile_bound)
     ranges = tileRange(keys, gx * gy, fix_last=fix_last)
     return ranges, vals, (alloc != 0), keys
 

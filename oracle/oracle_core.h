@@ -502,9 +502,12 @@ typedef struct {
 
 /* visibility + bounding box + tile rectangle: GR/binning.cu:309-355 (== :46-89).
  * 2*log(255 o) is evaluated in double and rounded to REAL so that the CPU and GPU (which does the
- * same) make bit-identical tile decisions; the reference's own value comes from fast-math __logf. */
+ * same) make bit-identical tile decisions; the reference's own value comes from fast-math __logf.
+ * exact_bound=1: the rectangle ends after the tile holding bbox_max, floor((bbox_max + T) / T);
+ * 0: the reference's floor((bbox_max + T - 1) / T), which drops tile k when the ellipse reaches
+ * pixel centre kT with bbox_max < kT + 1 (DESIGN.md section 7, D14). */
 static inline void SUF(splat_setup)(REAL ndcx, REAL ndcy, REAL viewz, REAL A, REAL B, REAL Cc, REAL o,
-                                    int H, int W, int TH, int TW, int gx, int gy, SUF(splat_geom)* g)
+                                    int H, int W, int TH, int TW, int gx, int gy, int exact_bound, SUF(splat_geom)* g)
 {
     g->A = A; g->B = B; g->C = Cc;
     g->disc = B * B - A * Cc;
@@ -531,8 +534,10 @@ static inline void SUF(splat_setup)(REAL ndcx, REAL ndcy, REAL viewz, REAL A, RE
     SUF(ellipse_isect)(A, B, Cc, g->inv_A, g->inv_C, g->disc, t, g->px, g->py, 0, g->argmax[1], &lo, &hi); g->bbox_max[1] = hi;
     g->rect_min[0] = SUF(imax)(0, SUF(imin)(gx, SUF(f2i_rz)(g->bbox_min[0] / TW)));
     g->rect_min[1] = SUF(imax)(0, SUF(imin)(gy, SUF(f2i_rz)(g->bbox_min[1] / TH)));
-    g->rect_max[0] = SUF(imax)(0, SUF(imin)(gx, SUF(f2i_rz)((g->bbox_max[0] + TW - 1) / TW)));
-    g->rect_max[1] = SUF(imax)(0, SUF(imin)(gy, SUF(f2i_rz)((g->bbox_max[1] + TH - 1) / TH)));
+    REAL ex = g->bbox_max[0] + TW, ey = g->bbox_max[1] + TH;
+    if (!exact_bound) { ex = ex - 1; ey = ey - 1; }
+    g->rect_max[0] = SUF(imax)(0, SUF(imin)(gx, SUF(f2i_rz)(ex / TW)));
+    g->rect_max[1] = SUF(imax)(0, SUF(imin)(gy, SUF(f2i_rz)(ey / TH)));
 }
 
 /* Attribution: the overlap walk restated below is speedy-splat's "AccuTile" procedure (https://github.com/j-alex-hanson/
@@ -593,7 +598,7 @@ static inline int SUF(process_tiles)(const SUF(splat_geom)* g, int TH, int TW, i
 /* GR/binning.cu:289-385 : per-splat pixel bbox + tile count.  [V,*,N]; entries >= valid untouched
  * (the caller pre-zeroes `alloc`, as the reference does with torch::zeros). */
 void SUF(orc_get_allocate_size)(const REAL* ndc, const REAL* viewz, const REAL* inv_cov, const REAL* opac,
-                               int V, int N, int valid, int H, int W, int TH, int TW,
+                               int V, int N, int valid, int H, int W, int TH, int TW, int exact_bound,
                                int32_t* left_up, int32_t* right_down, int32_t* alloc)
 {
     int gx = (W + TW - 1) / TW, gy = (H + TH - 1) / TH;
@@ -603,7 +608,7 @@ void SUF(orc_get_allocate_size)(const REAL* ndc, const REAL* viewz, const REAL* 
             SUF(splat_geom) g;
             size_t o4 = (size_t)b * 4 * N + i;
             SUF(splat_setup)(ndc[o4], ndc[o4 + N], viewz[(size_t)b * N + i], inv_cov[o4], inv_cov[o4 + N],
-                             inv_cov[o4 + 3 * (size_t)N], opac[i], H, W, TH, TW, gx, gy, &g);
+                             inv_cov[o4 + 3 * (size_t)N], opac[i], H, W, TH, TW, gx, gy, exact_bound, &g);
             size_t o2 = (size_t)b * 2 * N + i;
             if (g.visible) {
                 left_up[o2] = SUF(f2i_rz)(CEIL(g.bbox_min[0])); left_up[o2 + N] = SUF(f2i_rz)(CEIL(g.bbox_min[1]));
@@ -622,7 +627,7 @@ void SUF(orc_get_allocate_size)(const REAL* ndc, const REAL* viewz, const REAL* 
  * never written keep key 0 and sort to the front (SURVEY Q2).  keys_out/vals_out [V,cap]. */
 void SUF(orc_create_table)(const REAL* ndc, const REAL* inv_cov, const REAL* opac, const int32_t* offset,
                           const int64_t* sorted_id, int V, int N, int cap, int H, int W, int TH, int TW,
-                          int32_t* keys_out, int32_t* vals_out)
+                          int exact_bound, int32_t* keys_out, int32_t* vals_out)
 {
     int gx = (W + TW - 1) / TW, gy = (H + TH - 1) / TH;
     int ntile = gx * gy + 1;
@@ -642,7 +647,7 @@ void SUF(orc_create_table)(const REAL* ndc, const REAL* inv_cov, const REAL* opa
                 size_t o4 = (size_t)b * 4 * N + i;
                 /* the emit kernel skips the visibility test: it trusts asz>0 (GR/binning.cu:63) */
                 SUF(splat_setup)(ndc[o4], ndc[o4 + N], (REAL)1.0, inv_cov[o4], inv_cov[o4 + N],
-                                 inv_cov[o4 + 3 * (size_t)N], opac[i], H, W, TH, TW, gx, gy, &g);
+                                 inv_cov[o4 + 3 * (size_t)N], opac[i], H, W, TH, TW, gx, gy, exact_bound, &g);
                 if (g.visible) SUF(process_tiles)(&g, TH, TW, gx, i, off, cap, keys, vals);
             }
         }

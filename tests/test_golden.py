@@ -33,7 +33,8 @@ def run_oracle(name):
     out["bw_T_q"], out["bw_T_s"] = oracle.createTransformMatrix_backward(sl(up["g_T"]), rot, scale)
     out["bw_mvp"] = oracle.mvp_transform_backward(sl(up["g_ndc"]), sl(up["g_view"]), cam["view"], cam["proj"], inter["view_pos"])
     vz = inter["view_pos"][:, 2]
-    lu, rd, alloc = oracle.get_allocate_size(inter["ndc"], vz, inv, opacity, hw[0], hw[1], *tile)
+    # the reference's tile rectangle (DESIGN.md section 7, D14) and last-tile range (Q3), so that its tables compare
+    lu, rd, alloc = oracle.get_allocate_size(inter["ndc"], vz, inv, opacity, hw[0], hw[1], *tile, exact_tile_bound=False)
     out["alloc"] = alloc; out["left_up"] = lu; out["right_down"] = rd
     ranges, vals, _, keys = oracle.binning(inter["ndc"], vz, inv, opacity, None, hw, tile, fix_last=False)
     out["table_keys"] = keys; out["table_vals"] = vals; out["tile_range"] = ranges
@@ -53,7 +54,9 @@ def run_oracle(name):
 
 
 @pytest.mark.parametrize("name", list(CASES))
-def test_oracle_matches_reference_golden(name):
+def test_oracle_with_reference_rules_matches_reference_golden(name):
+    """The oracle with the reference's binning rules (exact_tile_bound=False, fix_last=False) against the reference's own
+    outputs; the oracle's defaults are the corrected rules (DESIGN.md section 7, D2 and D14)."""
     path = os.path.join(GOLD, f"{name}.npz")
     ref = dict(np.load(path))
     got = run_oracle(name)
