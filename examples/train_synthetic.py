@@ -73,7 +73,9 @@ def _train(n_gaussians, hw, n_views, iters, seed, device, log, perturb, antialia
         if rank == 0 and (it % 50 == 0 or it == iters - 1):
             log(f"iter {it:4d}  loss {float(history[-1]):.5f}")
     torch.cuda.synchronize(dev)
-    render.check_views()                                    # GPU-driven sizing: no view of the run outgrew its workspace
+    # GPU-driven sizing: each render_views call read the flags of the earlier batches that had landed; this reads the rest, so
+    # together they say that no view of the run outgrew its workspace
+    render.check_views()
     history = [float(h) for h in history]
     if rank == 0:
         dt = time.perf_counter() - t0

@@ -12,6 +12,7 @@ GR/binning.cu:137-163, hidden behind last epoch's feedback values when available
 """
 from __future__ import annotations
 
+import collections
 import ctypes
 import os
 from dataclasses import dataclass
@@ -414,9 +415,9 @@ class ViewWorkspace:
                  _query_bytes("lgs_scan_gathered_workspace_bytes", _round_up(N, 1 << 16)),
                  _query_bytes(f"lgs_sort_pairs_{'u16' if self.u16 else 'u32'}_workspace_bytes", _round_up(D, 1 << 18)))
         self.ws, self.ws_bytes = e(nb, _U8), nb
-        self.sticky = torch.zeros(4, dtype=_I32, device=dev)      # |flags, max pairs, max depth bits, views since the last check
-        self.sticky_host = torch.zeros(4, dtype=_I32).pin_memory()
-        self.sticky_event = None
+        self.sticky = torch.zeros(4, dtype=_I32, device=dev)      # |flags, max pairs, max depth bits, views since the last post
+        self._posted = collections.deque()    # (event, pinned i32[4]) of every post_flags() not yet read by check(), oldest first
+        self._free_host = []                  # pinned i32[4] buffers whose result has been read
         self._graphs = {}               # ("fwd"|"bwd", pointer signature) -> torch.cuda.CUDAGraph
         self._eager_runs = {}           # same key -> eager runs so far (the first run of a signature is never captured)
         self.views_done = 0
@@ -571,24 +572,34 @@ class ViewWorkspace:
 
     # -- feedback --------------------------------------------------------------------------------------------------
     def post_flags(self):
-        """Enqueue (on the current stream) the copy of the sticky overflow word to pinned memory and reset it on the device."""
-        self.sticky_host.copy_(self.sticky, non_blocking=True)
+        """Enqueue (on the current stream) the copy of the sticky overflow word to a pinned buffer of its own and reset the word on
+        the device.  The result stays queued until check() reads it: a post whose copy has not landed when the next one is made
+        is never dropped or overwritten."""
+        host = self._free_host.pop() if self._free_host else torch.zeros(4, dtype=_I32).pin_memory()
+        host.copy_(self.sticky, non_blocking=True)
         self.sticky.zero_()
-        self.sticky_event = torch.cuda.Event()
-        self.sticky_event.record(torch.cuda.current_stream(self.dev))
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(self.dev))
+        self._posted.append((ev, host))
 
     def check(self, wait: bool = False):
-        """Result of the last post_flags(): None if it has not landed yet (and wait is False); otherwise a dict, or
-        CapacityExceeded if a view since the previous check overflowed a prediction (its lists were truncated)."""
-        ev = self.sticky_event
-        if ev is None:
+        """Fold the results of every post_flags() not yet read, oldest first, that have landed (with wait, all of them: waits
+        for their copies).  None if there is none; otherwise a dict over the folded posts (max pairs and depth bits of a view, the
+        number of views), or CapacityExceeded if a view of any of them overflowed a prediction (its lists were truncated).
+        Posts that have not landed stay queued for a later check."""
+        flags, pairs, bits, views, read = 0, 0, 0, 0, 0
+        while self._posted:
+            ev, host = self._posted[0]
+            if not ev.query():
+                if not wait:
+                    break
+                ev.synchronize()
+            self._posted.popleft()
+            f, p, b, v = (int(x) for x in host)
+            self._free_host.append(host)
+            flags, pairs, bits, views, read = flags | f, max(pairs, p), max(bits, b), views + v, read + 1
+        if not read:
             return None
-        if not ev.query():
-            if not wait:
-                return None
-            ev.synchronize()
-        self.sticky_event = None
-        flags, pairs, bits, views = (int(x) for x in self.sticky_host)
         if flags:
             raise CapacityExceeded(pairs=pairs, pair_capacity=self.cap, depth_bits=bits, planned_depth_bits=self.planned_bits)
         return {"max_pairs": pairs, "max_depth_bits": bits, "views": views}

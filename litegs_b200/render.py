@@ -459,8 +459,8 @@ class _ViewSlots:
             self.ws.append(pipeline.ViewWorkspace(self.params_like, self.hw, self.tile, self.cap, self.bits))
 
     def check(self):
-        """Overflow flags of the previous batch (if they have landed): on overflow drop the workspaces -- the next batch measures
-        again -- and tell the caller to redo the step."""
+        """Overflow flags of the earlier batches that have landed (the others stay queued for the next check): on overflow drop the
+        workspaces -- the next batch measures again -- and tell the caller to redo the step."""
         try:
             for w in self.ws:
                 w.check(wait=False)
@@ -483,8 +483,9 @@ def _view_slots(params, hw, tile, n_slots, antialiased=False, filtered=False):
 
 
 def check_views(wait: bool = True):
-    """Explicit form of the lazy overflow check of render_views' GPU-driven path: (after a synchronisation) raises
-    pipeline.CapacityExceeded if a view of the last batch overflowed its workspace -- redo that step."""
+    """Explicit form of the lazy overflow check of render_views' GPU-driven path: raises pipeline.CapacityExceeded if a view of
+    any batch whose flags were not read yet overflowed its workspace -- redo that step.  wait: wait for the flags of every batch
+    enqueued so far (else only those that have landed are read; the rest stay queued)."""
     for ent in _slot_cache.values():
         if ent.ws is not None:
             try:

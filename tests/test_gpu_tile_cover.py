@@ -25,9 +25,8 @@ import torch
 
 import oracle
 from litegs_b200 import fused, pipeline
-from tests import camera_oracle as co
 from tests import tile_cover_oracle as tc
-from tests.util import tile_segments
+from tests.util import axis_camera, oracle_render_lists, screen_affine, tile_segments
 
 pytestmark = pytest.mark.gpu
 TILES = [(8, 16), (12, 16), (16, 16), (8, 8)]
@@ -115,26 +114,6 @@ def test_level_a_tables_cover_their_pixels(cuda, tile):
 # fused path: 3D Gaussians whose records land on the constructed conditions
 # ---------------------------------------------------------------------------------------------------
 
-def camera(hw):
-    H, W = hw
-    recp = 1.0 / math.tan(math.radians(30.0))
-    view, proj, _, planes = co.create_viewproj_forward(np.array([[1.0, 0, 0, 0, 0, 0, 0]]), np.array([recp]), H, W, 0.01, 100.0)
-    return dict(view=view.astype(np.float32), proj=proj.astype(np.float32), frustumplane=planes.astype(np.float32))
-
-
-def screen_affine(cam, hw, Z):
-    """(ax, bx, ay, by) with px = ax X + bx, py = ay Y + by at depth Z (fp64 from the camera matrices)."""
-    H, W = hw
-    M = cam["view"][0].astype(np.float64) @ cam["proj"][0].astype(np.float64)
-
-    def pix(X, Y):
-        h = np.stack([X, Y, Z, np.ones_like(Z)], -1) @ M
-        return (h[..., 0] / h[..., 3] + 1) * 0.5 * W - 0.5, (h[..., 1] / h[..., 3] + 1) * 0.5 * H - 0.5
-    x0, y0 = pix(np.zeros_like(Z), np.zeros_like(Z))
-    x1, y1 = pix(np.ones_like(Z), np.ones_like(Z))
-    return x1 - x0, x0, y1 - y0, y0
-
-
 def gaussians_for(cases, cam, hw, S):
     """One chunk of S Gaussians (the cases first, then invisible padding) at depths increasing with the index, shaped so that
     their projected conic is the case's: scales from the eigenvalues of the 2D covariance less the 0.3 px^2 low-pass,
@@ -163,7 +142,7 @@ def gaussians_for(cases, cam, hw, S):
 def land(cuda, cases, hw, tile, passes=4):
     """Gaussians for `cases`, moved on screen until each grazing / off-screen case's record reaches its target extent and the
     others their target centre.  -> (params, aabb, cam, n) with the Gaussians' final positions."""
-    cam = camera(hw)
+    cam = axis_camera(hw)
     n = len(cases)
     S = 32 * (-(-n // 32))
     P, (ax, ay) = gaussians_for(cases, cam, hw, S)
@@ -319,24 +298,16 @@ def end_to_end(img, st, rec, n, hw, tile):
     th, tw = tile
     gx, gy = -(-W // tw), -(-H // th)
     ntile = gx * gy
-    packed = st.packed[0].cpu().numpy().astype(np.float64)
-    N = packed.shape[0]
+    packed = st.packed[0].cpu().numpy()
     order = np.lexsort((np.arange(n), packed[:n, 9]))           # depth, ties in record order
     pid = np.tile(order.astype(np.int32), ntile)[None]
     ranges = np.full((1, ntile + 2), -1, np.int32)
     ranges[0, 1:] = np.arange(ntile + 1) * n
-    ndc = np.zeros((1, 4, N))
-    ndc[0, 0] = (packed[:, 0] + 0.5) / W * 2 - 1                   # the oracle maps ndc back to exactly the record's px, py
-    ndc[0, 1] = (packed[:, 1] + 0.5) / H * 2 - 1
-    inv = np.zeros((1, 2, 2, N))
-    inv[0, 0, 0], inv[0, 0, 1], inv[0, 1, 0], inv[0, 1, 1] = packed[:, 2], packed[:, 3], packed[:, 3], packed[:, 4]
-    col = np.ascontiguousarray(packed[:, 6:9].T[None])
-    op = packed[:, 5][None]
-    oimg, oT, _, _, _, frag = oracle.rasterize_forward(pid, ranges, ndc, inv, col, op, None, H, W, th, tw, fragile_eps=2e-6)
-    mask = q14_mask(rec, n, hw) | frag[0, :H, :W]
+    oimg, oT, frag = oracle_render_lists(packed, pid, ranges, hw, tile)
+    mask = q14_mask(rec, n, hw) | frag[:H, :W]
     assert mask.mean() < 0.03, mask.mean()
     got = img[0, :, :H, :W].cpu().numpy().astype(np.float64)
-    err = np.abs(got - oimg[0, :, :H, :W])[:, ~mask]
-    terr = np.abs(st.T[0, 0, :H, :W].cpu().numpy() - oT[0, 0, :H, :W])[~mask]
+    err = np.abs(got - oimg[:, :H, :W])[:, ~mask]
+    terr = np.abs(st.T[0, 0, :H, :W].cpu().numpy() - oT[:H, :W])[~mask]
     print(f"end to end {tile}: max |img - oracle| {err.max():.2e}, |T - oracle| {terr.max():.2e}, masked {mask.mean():.4f}")
-    assert err.max() < 1e-4 and terr.max() < 1e-4, (err.max(), terr.max(), np.argwhere(np.abs(got - oimg[0, :, :H, :W]).max(0) * ~mask > 1e-4)[:5])
+    assert err.max() < 1e-4 and terr.max() < 1e-4, (err.max(), terr.max(), np.argwhere(np.abs(got - oimg[:, :H, :W]).max(0) * ~mask > 1e-4)[:5])

@@ -167,6 +167,50 @@ def differing_tiles(ranges_a, pid_a, ranges_b, pid_b):
     return np.array(bad, np.int64), npairs
 
 
+def axis_camera(hw, t=(0.0, 0.0, 0.0)):
+    """A 60-degree camera with identity rotation and view-space position = world position + t (fp32 numpy dict).  With t = 0 the
+    view-space z of a point is its world z exactly."""
+    H, W = hw
+    recp = 1.0 / math.tan(math.radians(30.0))
+    view, proj, _, planes = co.create_viewproj_forward(np.array([[1.0, 0, 0, 0, *t]]), np.array([recp]), H, W, 0.01, 100.0)
+    return dict(view=view.astype(np.float32), proj=proj.astype(np.float32), frustumplane=planes.astype(np.float32))
+
+
+def screen_affine(cam, hw, Z):
+    """(ax, bx, ay, by) with px = ax X + bx, py = ay Y + by at depth Z (fp64 from the camera matrices)."""
+    H, W = hw
+    M = cam["view"][0].astype(np.float64) @ cam["proj"][0].astype(np.float64)
+
+    def pix(X, Y):
+        h = np.stack([X, Y, Z, np.ones_like(Z)], -1) @ M
+        return (h[..., 0] / h[..., 3] + 1) * 0.5 * W - 0.5, (h[..., 1] / h[..., 3] + 1) * 0.5 * H - 0.5
+    x0, y0 = pix(np.zeros_like(Z), np.zeros_like(Z))
+    x1, y1 = pix(np.ones_like(Z), np.ones_like(Z))
+    return x1 - x0, x0, y1 - y0, y0
+
+
+def oracle_render_lists(packed, pid, ranges, hw, tile):
+    """fp64 oracle raster of fused records packed f32[N,12] (px, py, A, B, C, o, r, g, b, ...) over the given tile lists
+    (sorted_pid i32[1,L], ranges i32[1,tiles+2]) -> (img [3,Hp,Wp], T [Hp,Wp], fragile [Hp,Wp]), all f64 / bool."""
+    H, W = hw
+    th, tw = tile
+    packed = np.asarray(packed, np.float64)
+    N = packed.shape[0]
+    ndc = np.zeros((1, 4, N))
+    ndc[0, 0] = (packed[:, 0] + 0.5) / W * 2 - 1                   # the oracle maps ndc back to exactly the record's px, py
+    ndc[0, 1] = (packed[:, 1] + 0.5) / H * 2 - 1
+    inv = np.zeros((1, 2, 2, N))
+    inv[0, 0, 0], inv[0, 0, 1], inv[0, 1, 0], inv[0, 1, 1] = packed[:, 2], packed[:, 3], packed[:, 3], packed[:, 4]
+    col = np.ascontiguousarray(packed[:, 6:9].T[None])
+    op = packed[:, 5][None]
+    pid = np.ascontiguousarray(pid, np.int32).reshape(1, -1)
+    if pid.shape[1] == 0:
+        pid = np.zeros((1, 1), np.int32)
+    oimg, oT, _, _, _, frag = oracle.rasterize_forward(pid, np.asarray(ranges, np.int32), ndc, inv, col, op, None, H, W, th, tw,
+                                                       fragile_eps=2e-6)
+    return oimg[0], oT[0, 0], frag[0]
+
+
 def rel_err(a, b):
     """max |a-b| / max(1, |b|) -- the Tier-1 metric of SURVEY 8c."""
     a = np.asarray(a, np.float64); b = np.asarray(b, np.float64)
