@@ -690,8 +690,9 @@ __global__ void project_backward_kernel(
 #pragma unroll
             for (int k = 0; k < 4; k++) o_q[k] = __fadd_rn(o_q[k], t.rn * (dqn[k] - dotn * t.qn[k]));   // no contraction into o_q
         }
-        const float sig = 1.0f - 1.0f / (1.0f + expf(o_raw));
-        o_op = d_o * (true_sigmoid ? sig * (1.0f - sig) : sig);
+        // 1 - sig is u itself: forming it from the rounded sig cancels for saturated logits
+        const float u = 1.0f / (1.0f + expf(o_raw)), sig = 1.0f - u;
+        o_op = d_o * (true_sigmoid ? sig * u : sig);
         // MVP backward (GR/transform.cu:517-558) with d_ndc.z = d_ndc.w = 0 and no view-space gradient
         const float* P = proj; const float* Vm = view;
         const float n0 = t.h[0] * t.iw, n1 = t.h[1] * t.iw;

@@ -205,8 +205,8 @@ __global__ void activate_backward_kernel(
     float dot = g[0] * o[0] + g[1] * o[1] + g[2] * o[2] + g[3] * o[3];
 #pragma unroll
     for (int k = 0; k < 4; k++) g_rot[k * AS + dst] = rn * (g[k] - dot * o[k]);
-    float sig = 1.0f - 1.0f / (1.0f + expf(opac[src]));
-    g_opac[dst] = g_aopac[dst] * (true_sigmoid ? sig * (1.0f - sig) : sig);
+    const float u = 1.0f / (1.0f + expf(opac[src])), sig = 1.0f - u;     // 1 - sig = u, not formed from the rounded sig
+    g_opac[dst] = g_aopac[dst] * (true_sigmoid ? sig * u : sig);
 
     float p[3] = { pos[src], pos[CS + src], pos[2 * CS + src] };
     constexpr int K = (DEG + 1) * (DEG + 1);

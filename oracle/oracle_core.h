@@ -221,8 +221,8 @@ void SUF(orc_activate_backward)(int deg, const int64_t* chunk_ids, int nvis, con
             REAL dot = g[0] * o[0] + g[1] * o[1] + g[2] * o[2] + g[3] * o[3];
             for (int k = 0; k < 4; k++) g_rot[k * AS + dst + s] = rn * (g[k] - dot * o[k]);
             REAL x = opac[src + s];
-            REAL sig = (REAL)1.0 - (REAL)1.0 / ((REAL)1.0 + EXP(x));
-            REAL fac = true_sigmoid ? sig * ((REAL)1.0 - sig) : sig;
+            REAL u = (REAL)1.0 / ((REAL)1.0 + EXP(x)), sig = (REAL)1.0 - u;   /* 1 - sig = u, not formed from the rounded sig */
+            REAL fac = true_sigmoid ? sig * u : sig;
             g_opac[dst + s] = g_aopac[dst + s] * fac;
             REAL p[3] = { pos[0 * CS + src + s], pos[1 * CS + src + s], pos[2 * CS + src + s] };
             for (int v = 0; v < V; v++) {
