@@ -689,13 +689,24 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_kernel(
 //    independent and interleaved;
 //  * no branch around the pixel body: a pixel the splat does not reach (alpha below 1/256, or the pixel had already
 //    stopped before this list position) gets its Gaussian weight G forced to 0, which makes every term of the chain an
-//    exact no-op (a = 0, 1/(1-a) = 1, T and S unchanged, all gradient terms +0);
+//    exact no-op (a = 0, 1/(1-a) = 1, T and S unchanged, all gradient terms +0); the warp votes right after the contribution
+//    test and drops the rest of the step when no pixel of the tile takes the splat;
+//  * "still active at position k" (k < last_contributor) is tested per position only in the chunks of 32 positions where some
+//    pixel of the tile stops; in every other chunk each pixel's answer is fixed, and it is folded into the pixel's alpha threshold;
+//  * each lane sums its pixels' gradient terms in one running chain per value, so they are parked without a pair-half add, and the
+//    lane that reduces a parked row keeps that splat's id in a register;
 //  * d opacity = sum(G dalpha) = sum(dpw) / o, so the ninth reduced value is the s0 moment itself;
 //  * the transposed row sums of the flush add the LDS.128 halves pairwise.
 // STAT adds the densification error term in one of two forms (err_mode): 1 = the reference's lane-running recurrence
 // (GR/raster.cu:779-784: after each executed pixel PAIR the lane's running sum of G dalpha over its even rows and over its
 // odd rows is squared and added), 0 = sum over pixels of (G dalpha)^2.
 __device__ __forceinline__ float2 bc2(float a) { return make_float2(a, a); }
+// Running per-lane sums over a lane's pixels in pixel order, one rounding per term; `first` (the lane's first pair) initialises them.
+__device__ __forceinline__ void acc_sum(float& s, float2 a, bool first) { s = __fadd_rn(first ? a.x : __fadd_rn(s, a.x), a.y); }
+__device__ __forceinline__ void acc_dot(float& s, float2 a, float2 b, bool first)
+{
+    s = __fmaf_rn(a.y, b.y, first ? __fmul_rn(a.x, b.x) : __fmaf_rn(a.x, b.x, s));
+}
 
 // DET (deterministic mode, lgs_set_deterministic): the per-(tile, splat) sums -- themselves computed in a fixed order inside the
 // warp -- are accumulated as FIXED-POINT integers with integer atomics, which are associative: the result no longer depends on the
@@ -741,7 +752,6 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
     __shared__ __align__(16) float2 s_gn[NORMAL ? WARPS_PER_BLOCK : 1][NORMAL ? 3 * NP : 1][NORMAL ? 32 : 1];   // g_N per pixel pair
     __shared__ __align__(8) uint64_t s_bar[WARPS_PER_BLOCK][2];
     __shared__ __align__(16) float s_acc[WARPS_PER_BLOCK][RG * NV][LGS_ROWF];
-    __shared__ int s_pid[WARPS_PER_BLOCK][4];               // ids of the splats parked in s_acc
     const int lane = threadIdx.x, warp = threadIdx.y, b = blockIdx.y;
     const int slot = blockIdx.x * blockDim.y + warp;
     int tile_id;
@@ -799,7 +809,12 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
     kmax = __reduce_max_sync(FULL_MASK, kmax);
     if (kmax <= 0) return;
 
-    int pend = 0;                                      // splats parked in s_acc (warp-uniform); their ids are in s_pid
+    // In a flush lane r sums row r of s_acc: value fv of parked splat fsp, whose id the lane keeps in fpid (set when it is parked).
+    const int fsp = lane / NV, fv = lane - fsp * NV;
+    int fpid = 0;
+    int pend = 0;                                      // splats parked in s_acc (warp-uniform)
+    float* const acc_lane = &s_acc[warp][0][lane];
+    float* park = acc_lane;                            // this lane's column of the next parked splat's rows
     auto flush = [&]() {
         __syncwarp();
         if (lane < pend * NV) {
@@ -817,20 +832,19 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
             p0 = add2(p0, p2); p4 = add2(p4, p6);
             p0 = add2(p0, p4);
             const float sum = p0.x + p0.y;
-            const int sp = lane / NV, row = lane - sp * NV;
-            const int v = (DEPTH && row == ROW_Z) ? LGS_GRAD_DEPTH : row;         // gradient slot of the row
-            const int pid = s_pid[warp][sp];
-            if (NORMAL && row >= ROW_N) {                                            // normal rows -> the side array
-                if (DET) det_add(reinterpret_cast<unsigned long long*>(grad_normal) + 2 * ((size_t)pid * 4 + (row - ROW_N)), sum);
-                else atomicAdd(&grad_normal[(size_t)pid * 4 + (row - ROW_N)], sum);
+            const int v = (DEPTH && fv == ROW_Z) ? LGS_GRAD_DEPTH : fv;           // gradient slot of the row
+            if (NORMAL && fv >= ROW_N) {                                             // normal rows -> the side array
+                if (DET) det_add(reinterpret_cast<unsigned long long*>(grad_normal) + 2 * ((size_t)fpid * 4 + (fv - ROW_N)), sum);
+                else atomicAdd(&grad_normal[(size_t)fpid * 4 + (fv - ROW_N)], sum);
             } else if (DET) {
-                det_add(reinterpret_cast<unsigned long long*>(grad) + 2 * ((size_t)pid * LGS_GRAD_FLOATS + v), sum);
+                det_add(reinterpret_cast<unsigned long long*>(grad) + 2 * ((size_t)fpid * LGS_GRAD_FLOATS + v), sum);
             } else {
-                atomicAdd(&grad[(size_t)pid * LGS_GRAD_FLOATS + v], sum);                        // RED.ADD.F32
+                atomicAdd(&grad[(size_t)fpid * LGS_GRAD_FLOATS + v], sum);                       // RED.ADD.F32
             }
         }
         __syncwarp();
         pend = 0;
+        park = acc_lane;
     };
     Stager<false> st;
     st.init(&s_rec[warp][0][0], &s_bar[warp][0], lane);
@@ -852,7 +866,12 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
         st.template wait<true, DEPTH>(v & 1, more);
         const SplatRec* chunk = &s_rec[warp][v & 1][0];
         const int nk = min(32, kmax - c * 32);
-        for (int kk = nk - 1; kk >= 0; kk--) {
+        // thr[j]: the contribution threshold of pixel j in a chunk that holds no pixel's last position -- A_MIN_S where the pixel is
+        // active throughout, NaN (no G passes) where it stopped before the chunk -- so that such chunks skip the k < nl[j] test.
+        float thr[PPT];
+        // list position c*32 + kk; CHECKED tests k < nl[j] per pixel, otherwise thr[j] carries that test
+        auto step = [&](int kk, auto checked) {
+            constexpr bool CHECKED = decltype(checked)::value;
             const int k = c * 32 + kk;
             const float4 q0 = *reinterpret_cast<const float4*>(&chunk[kk].px);   // px py a2 b2   (pre-scaled by Stager::wait<true>)
             const float4 q1 = *reinterpret_cast<const float4*>(&chunk[kk].C);    // c2 o r g
@@ -862,30 +881,46 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
             const float a2 = q0.z, b2 = q0.w, c2 = q1.x;
             const float base = a2 * dx * dx, lin = b2 * dx;
             const float2 os2 = bc2(q2.y), o2 = bc2(q1.y), c22 = bc2(c2), lin2 = bc2(lin), base2 = bc2(base);
-            const float2 cr2 = bc2(q1.z), cg2 = bc2(q1.w), cb2 = bc2(cb), dy02 = bc2(dy0);
+            const float2 cr2 = bc2(q1.z), cg2 = bc2(q1.w), cb2 = bc2(cb);
             const float2 z2 = bc2(DEPTH ? chunk[kk].pad0 : 0.0f);            // view-space z (staged by prescale<DEPTH>)
             const float4 nk4 = NORMAL ? s_nrm[warp][v & 1][kk] : make_float4(0.f, 0.f, 0.f, 0.f);   // n of this splat
             const float2 n02 = bc2(nk4.x), n12 = bc2(nk4.y), n22 = bc2(nk4.z);
-            float2 s0, s1, s2, dr, dg, db, dzs;         // per-(tile, splat) sums: the first pixel pair initialises them
-            float2 dn0, dn1, dn2;
+            float s0, s1, s2, dr, dg, db, dzs;          // per-(tile, splat) sums over the lane's pixels in order (acc_sum, acc_dot)
+            float dn0, dn1, dn2;
             float esq = 0.f, runx = 0.f, runy = 0.f;
+            float2 dyp[NP], Gp[NP];
+            bool okp[NP];
             bool any = false;
 #pragma unroll
             for (int p = 0; p < NP; p++) {
-                const float2 dy = add2(dy02, make_float2(-(float)(2 * p), -(float)(2 * p + 1)));
+                const float2 dy = make_float2(dy0 - (float)(2 * p), dy0 - (float)(2 * p + 1));
                 const float2 pw = fma2(dy, fma2(c22, dy, lin2), base2);      // same two roundings as the forward's fmaf chain
                 float2 G = make_float2(fast_ex2(pw.x), fast_ex2(pw.y));
                 // contribution test = the forward's expression bit for bit (os * G >= A_MIN_S), and the pixel must still have
                 // been active at list position k
                 const float2 tt = mul2(os2, G);
-                const bool ok0 = (tt.x >= A_MIN_S) && (k < nl[2 * p]);
-                const bool ok1 = (tt.y >= A_MIN_S) && (k < nl[2 * p + 1]);
+                bool ok0, ok1;
+                if (CHECKED) {
+                    ok0 = (tt.x >= A_MIN_S) && (k < nl[2 * p]);
+                    ok1 = (tt.y >= A_MIN_S) && (k < nl[2 * p + 1]);
+                } else {
+                    ok0 = tt.x >= thr[2 * p];
+                    ok1 = tt.y >= thr[2 * p + 1];
+                }
                 any |= ok0 | ok1;
                 G.x = ok0 ? G.x : 0.0f;
                 G.y = ok1 ? G.y : 0.0f;
+                dyp[p] = dy; Gp[p] = G; okp[p] = ok0 | ok1;
+            }
+            // No pixel of the tile takes this splat: with G = 0 everywhere the rest of the chain is an exact no-op (rc = 1, T and S
+            // unchanged, every gradient term 0), so the position is done.
+            if (!__any_sync(FULL_MASK, any)) return;
+#pragma unroll
+            for (int p = 0; p < NP; p++) {
+                const float2 dy = dyp[p], G = Gp[p];
                 const float2 at = mul2(o2, G);
                 const float2 a = make_float2(fminf(at.x, ALPHA_MAX), fminf(at.y, ALPHA_MAX));
-                const float2 om = fma2(a, bc2(-1.0f), bc2(1.0f));                  // 1 - a
+                const float2 om = make_float2(__fsub_rn(1.0f, a.x), __fsub_rn(1.0f, a.y));
                 const float2 rc = make_float2(fast_rcp(om.x), fast_rcp(om.y));
                 const float2 Tn = mul2(T[p], rc);                                  // transmittance in front of this splat
                 T[p] = Tn;                                                               // (rc = 1 exactly where G was zeroed)
@@ -903,23 +938,16 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
                 S[p] = fma2(a, diff, S[p]);
                 const float2 dpw = mul2(at, da);      // passes through the 255/256 clamp (GR/raster.cu:776-778)
                 const float2 td = mul2(dpw, dy);
-                if (p == 0) {
-                    dr = mul2(w, g0[p]); dg = mul2(w, g1[p]); db = mul2(w, g2[p]);
-                    if (DEPTH) dzs = mul2(w, gz[p]);
-                    if (NORMAL) { dn0 = mul2(w, u0); dn1 = mul2(w, u1); dn2 = mul2(w, u2); }
-                    s0 = dpw; s1 = td; s2 = mul2(td, dy);
-                } else {
-                    dr = fma2(w, g0[p], dr); dg = fma2(w, g1[p], dg); db = fma2(w, g2[p], db);
-                    if (DEPTH) dzs = fma2(w, gz[p], dzs);
-                    if (NORMAL) { dn0 = fma2(w, u0, dn0); dn1 = fma2(w, u1, dn1); dn2 = fma2(w, u2, dn2); }
-                    s0 = add2(s0, dpw);
-                    s1 = add2(s1, td);
-                    s2 = fma2(td, dy, s2);
-                }
+                acc_dot(dr, w, g0[p], p == 0); acc_dot(dg, w, g1[p], p == 0); acc_dot(db, w, g2[p], p == 0);
+                if (DEPTH) acc_dot(dzs, w, gz[p], p == 0);
+                if (NORMAL) { acc_dot(dn0, w, u0, p == 0); acc_dot(dn1, w, u1, p == 0); acc_dot(dn2, w, u2, p == 0); }
+                acc_sum(s0, dpw, p == 0);
+                acc_sum(s1, td, p == 0);
+                acc_dot(s2, td, dy, p == 0);
                 if (STAT) {
                     const float2 go = mul2(G, da);
                     if (err_mode == 1) {
-                        if (__any_sync(FULL_MASK, ok0 | ok1)) {      // the reference skips a pair no lane of the warp reaches
+                        if (__any_sync(FULL_MASK, okp[p])) {         // the reference skips a pair no lane of the warp reaches
                             runx += go.x; runy += go.y;
                             esq = fmaf(runx, runx, fmaf(runy, runy, esq));
                         }
@@ -928,31 +956,42 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) raster_backward_v2_kerne
                     }
                 }
             }
-            if (__any_sync(FULL_MASK, any)) {
+            {
                 // raw moments (LGS_GRAD_* slots, common.cuh): the conic factors are applied once per splat by the consumer
-                const float m0 = s0.x + s0.y, m1 = s1.x + s1.y, m2 = s2.x + s2.y;
-                const float u0 = dx * m0;
-                if (lane == kk) s_pid[warp][pend] = id_this;
-                float* row = &s_acc[warp][pend * NV][lane];
+                const float u0 = dx * s0;
+                const int pid = __shfl_sync(FULL_MASK, id_this, kk);
+                if (fsp == pend) fpid = pid;
+                float* const row = park;
                 row[0 * LGS_ROWF] = u0;                    // sum dx s0
-                row[1 * LGS_ROWF] = m1;                    // sum s1
+                row[1 * LGS_ROWF] = s1;                    // sum s1
                 row[2 * LGS_ROWF] = dx * u0;               // sum dx^2 s0
-                row[3 * LGS_ROWF] = dx * m1;               // sum dx s1
-                row[4 * LGS_ROWF] = m2;                    // sum s2
-                row[5 * LGS_ROWF] = dr.x + dr.y;
-                row[6 * LGS_ROWF] = dg.x + dg.y;
-                row[7 * LGS_ROWF] = db.x + db.y;
-                row[8 * LGS_ROWF] = m0;                    // sum s0
+                row[3 * LGS_ROWF] = dx * s1;               // sum dx s1
+                row[4 * LGS_ROWF] = s2;                    // sum s2
+                row[5 * LGS_ROWF] = dr;
+                row[6 * LGS_ROWF] = dg;
+                row[7 * LGS_ROWF] = db;
+                row[8 * LGS_ROWF] = s0;                    // sum s0
                 if (STAT) row[9 * LGS_ROWF] = esq;
-                if (DEPTH) row[ROW_Z * LGS_ROWF] = dzs.x + dzs.y;        // sum w g_z -> slot LGS_GRAD_DEPTH
+                if (DEPTH) row[ROW_Z * LGS_ROWF] = dzs;                  // sum w g_z -> slot LGS_GRAD_DEPTH
                 if (NORMAL) {                                            // sum w g_N -> grad_normal
-                    row[ROW_N * LGS_ROWF] = dn0.x + dn0.y;
-                    row[(ROW_N + 1) * LGS_ROWF] = dn1.x + dn1.y;
-                    row[(ROW_N + 2) * LGS_ROWF] = dn2.x + dn2.y;
+                    row[ROW_N * LGS_ROWF] = dn0;
+                    row[(ROW_N + 1) * LGS_ROWF] = dn1;
+                    row[(ROW_N + 2) * LGS_ROWF] = dn2;
                 }
                 pend++;
+                park += NV * LGS_ROWF;
                 if (pend == RG) flush();
             }
+        };
+        bool edge = false;                             // a pixel of the lane stops inside this chunk: c*32 < nl[j] < c*32 + nk
+#pragma unroll
+        for (int j = 0; j < PPT; j++) edge |= (nl[j] > c * 32) && (nl[j] < c * 32 + nk);
+        if (__any_sync(FULL_MASK, edge)) {
+            for (int kk = nk - 1; kk >= 0; kk--) step(kk, std::true_type{});
+        } else {
+#pragma unroll
+            for (int j = 0; j < PPT; j++) thr[j] = (nl[j] > c * 32) ? A_MIN_S : __int_as_float(0x7fc00000);
+            for (int kk = nk - 1; kk >= 0; kk--) step(kk, std::false_type{});
         }
         __syncwarp();
     }
