@@ -35,15 +35,11 @@ SIGNATURES = {
     "lgs_create_table": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _Z, _P],
     "lgs_set_exact_tile_bound": [_I],
     "lgs_tile_range": [_P, _I, _I, _I, _I, _P, _P],
-    "lgs_tile_range_u16": [_P, _I, _I, _I, _I, _P, _P],
     "lgs_sort_pairs_u16_workspace_bytes": [_I, ctypes.POINTER(_Z)],
     "lgs_sort_pairs_u16": [_P, _P, _P, _P, _I, _I, _I, _P, _Z, _P],
-    "lgs_emit_pairs_u16": [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P],
     "lgs_sort_pairs_u32_workspace_bytes": [_I, ctypes.POINTER(_Z)],
     "lgs_sort_pairs_u32": [_P, _P, _P, _P, _I, _I, _I, _P, _Z, _P],
-    "lgs_sort_pairs_u32_rebased": [_P, _P, _P, _P, _I, ctypes.c_uint, _I, _P, _Z, _P],
     "lgs_scan_gathered_workspace_bytes": [_I, ctypes.POINTER(_Z)],
-    "lgs_scan_gathered": [_P, _P, _I, _P, _P, _Z, _P],
     "lgs_view_params": [_P, _I, _I, _I, _P, _P, _P],
     "lgs_sort_pairs_u32_dev": [_P, _P, _P, _P, _I, _P, _P, _I, _P, _Z, _P],
     "lgs_sort_pairs_u16_dev": [_P, _P, _P, _P, _I, _P, _I, _I, _P, _Z, _P],
@@ -69,7 +65,6 @@ SIGNATURES = {
     "lgs_set_deterministic": [_I],
     "lgs_project_forward": [_I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _I, _P,
                             _P],
-    "lgs_emit_pairs": [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P],
     "lgs_project_backward": [_I, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _I,
                              _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _P, _I, _I, _P, _P],
     "lgs_create_viewproj_forward": [_P, _P, _I, _I, _I, _F, _F, _P, _P, _P, _P, _P],

@@ -9,7 +9,6 @@
 #include <cub/device/device_scan.cuh>
 #include <cub/iterator/transform_input_iterator.cuh>
 #include <cub/iterator/counting_input_iterator.cuh>
-#include <cstdlib>
 #include "common.cuh"
 #include "splat_geom.cuh"
 
@@ -155,51 +154,9 @@ __global__ void fill_int_kernel(int* __restrict__ p, int v, size_t n)
     if (i < n) p[i] = v;
 }
 
-// KeyT = int (op-level table) or unsigned short (fused pipeline when tiles+1 < 65536).  Each thread owns VEC consecutive
-// keys, fetched with one vector load, plus the first key of the next group.
-template <typename KeyT, int VEC>
-__global__ void __launch_bounds__(256) tile_range_kernel(const KeyT* __restrict__ keys, int L, int max_tile, int fix_last,
-                                                         int* __restrict__ range)
-{
-    const int b = blockIdx.y;
-    const KeyT* k = keys + (size_t)b * L;
-    int* r = range + (size_t)b * (max_tile + 2);
-    const int j0 = (blockIdx.x * blockDim.x + threadIdx.x) * VEC;
-    if (j0 >= L) return;
-    int key[VEC + 1];
-    if (VEC > 1 && j0 + VEC <= L) {
-        struct __align__(sizeof(KeyT) * VEC) Pack { KeyT v[VEC]; };
-        Pack pk = *reinterpret_cast<const Pack*>(k + j0);
-#pragma unroll
-        for (int i = 0; i < VEC; i++) key[i] = (int)pk.v[i];
-    } else {
-#pragma unroll
-        for (int i = 0; i < VEC; i++) key[i] = (j0 + i < L) ? (int)k[j0 + i] : -1;
-    }
-    key[VEC] = (j0 + VEC < L) ? (int)k[j0 + VEC] : -1;
-    if (j0 == 0) r[key[0]] = 0;
-#pragma unroll
-    for (int i = 0; i < VEC; i++) {
-        const int j = j0 + i;
-        if (j >= L) break;
-        const int cur = key[i];
-        if (j == L - 1) {
-            r[max_tile + 1] = L;
-            if (fix_last && cur + 1 <= max_tile + 1) r[cur + 1] = L;
-        } else {
-            const int nxt = key[i + 1];
-            if (cur != nxt) {
-                if (cur + 1 < nxt) r[cur + 1] = j + 1;
-                r[nxt] = j + 1;
-            }
-        }
-    }
-}
-
-// The same table by search: entry t only depends on where key t would be inserted in the sorted list, so one warp per
-// tile does one lower_bound instead of the whole list being streamed once -- 16k warps x 5 probe rounds instead of 22 MB at
-// 1080p.  Bit-identical to tile_range_kernel (kept above as the reference
-// form and for the description of the rules):
+// The table by search: entry t only depends on where key t would be inserted in the sorted list, so one warp per tile does
+// one lower_bound instead of the whole list being streamed once -- 16k warps x 5 probe rounds instead of 22 MB at 1080p.
+// KeyT = int (op-level table) or unsigned short (fused pipeline when tiles+1 < 65536).  The rules:
 //   populated t                      -> first index of t
 //   empty t right after a populated  -> that tile's end (its successor's start); for the LAST populated tile only if fix_last
 //   t = max_tile + 1                 -> L
@@ -251,20 +208,6 @@ static int tile_range_launch(const KeyT* keys, int V, int L, int max_tile, int f
         LGS_CHECK_LAUNCH("fill_int_kernel");
         return LGS_OK;
     }
-    static const bool scan_form = getenv("LGS_TILE_RANGE") != nullptr && getenv("LGS_TILE_RANGE")[0] == 's';   // A/B: "scan"
-    if (scan_form) {
-        size_t n = (size_t)V * (max_tile + 2);
-        fill_int_kernel<<<lgs_cdiv((long long)n, 256), 256, 0, st>>>(range, -1, n);
-        LGS_CHECK_LAUNCH("fill_int_kernel");
-        constexpr int VEC = 16 / sizeof(KeyT);             // one 16-byte load per thread
-        const bool aligned = (((uintptr_t)keys) % 16 == 0) && (V == 1 || ((size_t)L * sizeof(KeyT)) % 16 == 0);
-        if (aligned)
-            tile_range_kernel<KeyT, VEC><<<dim3(lgs_cdiv(lgs_cdiv(L, VEC), 256), V), 256, 0, st>>>(keys, L, max_tile, fix_last, range);
-        else
-            tile_range_kernel<KeyT, 1><<<dim3(lgs_cdiv(L, 256), V), 256, 0, st>>>(keys, L, max_tile, fix_last, range);
-        LGS_CHECK_LAUNCH("tile_range_kernel");
-        return LGS_OK;
-    }
     tile_range_bsearch_kernel<KeyT><<<dim3(lgs_cdiv(max_tile + 2, 8), V), 256, 0, st>>>(keys, L, max_tile, fix_last, range, nullptr);
     LGS_CHECK_LAUNCH("tile_range_bsearch_kernel");
     return LGS_OK;
@@ -275,14 +218,6 @@ extern "C" int lgs_tile_range(const int* table_tile_id, int V, int table_length,
 {
     LGS_REQUIRE(V >= 1 && table_length >= 0 && max_tile_id >= 0, "tileRange: bad sizes V=%d L=%d max_tile=%d", V, table_length, max_tile_id);
     return tile_range_launch<int>(table_tile_id, V, table_length, max_tile_id, fix_last, tile_range, (cudaStream_t)stream);
-}
-
-extern "C" int lgs_tile_range_u16(const unsigned short* table_tile_id, int V, int table_length, int max_tile_id, int fix_last,
-                                  int* tile_range, void* stream)
-{
-    LGS_REQUIRE(V >= 1 && table_length >= 0 && max_tile_id >= 0 && max_tile_id < 65535, "tileRange(u16): bad sizes V=%d L=%d max_tile=%d", V,
-                table_length, max_tile_id);
-    return tile_range_launch<unsigned short>(table_tile_id, V, table_length, max_tile_id, fix_last, tile_range, (cudaStream_t)stream);
 }
 
 // device-side length forms (GPU-driven sizing: `capacity` bounds the launch, *length_dev is the live length)
@@ -325,38 +260,23 @@ extern "C" int lgs_scan_gathered_workspace_bytes(int n, size_t* bytes)
     return LGS_OK;
 }
 
-// out[j] = sum_{k<=j} counts[order[k]]   (inclusive, int32)
-static int scan_gathered(const int* counts, const unsigned* order, int n, const int* n_dev, int* out, void* workspace,
-                         size_t workspace_bytes, void* stream);
-
-extern "C" int lgs_scan_gathered(const int* counts, const unsigned* order, int n, int* out, void* workspace, size_t workspace_bytes,
-                                 void* stream)
-{
-    return scan_gathered(counts, order, n, nullptr, out, workspace, workspace_bytes, stream);
-}
-
-// capacity items are scanned; items at or past *n_dev contribute 0 (their `order` entries are never read)
+// out[j] = sum_{k<=j} counts[order[k]]   (inclusive, int32) over `capacity` items; items at or past *n_dev contribute 0
+// (their `order` entries are never read)
 extern "C" int lgs_scan_gathered_dev(const int* counts, const unsigned* order, int capacity, const int* n_dev, int* out, void* workspace,
                                      size_t workspace_bytes, void* stream)
 {
     LGS_REQUIRE(n_dev != nullptr, "scan_gathered_dev: n_dev is NULL");
-    return scan_gathered(counts, order, capacity, n_dev, out, workspace, workspace_bytes, stream);
-}
-
-static int scan_gathered(const int* counts, const unsigned* order, int n, const int* n_dev, int* out, void* workspace,
-                         size_t workspace_bytes, void* stream)
-{
-    if (n <= 0) return LGS_OK;
+    if (capacity <= 0) return LGS_OK;
     cub::CountingInputIterator<int> cnt(0);
     GatherCount op{ counts, order, n_dev };
     cub::TransformInputIterator<int, GatherCount, cub::CountingInputIterator<int>> it(cnt, op);
     size_t need = 0;
-    cub::DeviceScan::InclusiveSum(nullptr, need, it, out, n);
+    cub::DeviceScan::InclusiveSum(nullptr, need, it, out, capacity);
     void* ws = (void*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
     if (workspace == nullptr || workspace_bytes < need + 256) {
         lgs_set_error("scan_gathered: workspace of %zu bytes needed, %zu given", need + 256, workspace_bytes);
         return LGS_ERR_WORKSPACE;
     }
-    LGS_CUDA(cub::DeviceScan::InclusiveSum(ws, need, it, out, n, (cudaStream_t)stream));
+    LGS_CUDA(cub::DeviceScan::InclusiveSum(ws, need, it, out, capacity, (cudaStream_t)stream));
     return LGS_OK;
 }

@@ -404,43 +404,9 @@ __global__ void __launch_bounds__(LGS_EMIT_WARPS * 32) emit_pairs_rec_kernel(con
     }
 }
 
-extern "C" int lgs_emit_pairs(const float* packed_params, const int* offset, const unsigned* order, int n, int cap, int img_h,
-                              int img_w, int tile_h, int tile_w, int* keys, int* vals, void* stream)
-{
-    LGS_REQUIRE(lgs_tile_ok(tile_h, tile_w), "emit_pairs: tile %dx%d not one of 8x16, 12x16, 16x16, 8x8", tile_h, tile_w);
-    if (n <= 0 || cap <= 0) return LGS_OK;
-    int gx = (img_w + tile_w - 1) / tile_w, gy = (img_h + tile_h - 1) / tile_h;
-    cudaStream_t st = (cudaStream_t)stream;
-    lgs_with_tile(tile_h, tile_w, [&](auto th, auto tw) {
-        emit_pairs_rec_kernel<th, tw, int><<<lgs_cdiv(n, LGS_EMIT_WARPS * 32), LGS_EMIT_WARPS * 32, 0, st>>>(
-            (const SplatRec*)packed_params, offset, order, n, cap, img_h, img_w, gx, gy, keys, vals, nullptr, nullptr);
-        return LGS_OK;
-    });
-    LGS_CHECK_LAUNCH("emit_pairs_rec_kernel");
-    return LGS_OK;
-}
-
-// same with 16-bit tile keys (requires tiles + 1 < 65536)
-extern "C" int lgs_emit_pairs_u16(const float* packed_params, const int* offset, const unsigned* order, int n, int cap, int img_h,
-                                  int img_w, int tile_h, int tile_w, unsigned short* keys, int* vals, void* stream)
-{
-    LGS_REQUIRE(lgs_tile_ok(tile_h, tile_w), "emit_pairs_u16: tile %dx%d not one of 8x16, 12x16, 16x16, 8x8", tile_h, tile_w);
-    if (n <= 0 || cap <= 0) return LGS_OK;
-    int gx = (img_w + tile_w - 1) / tile_w, gy = (img_h + tile_h - 1) / tile_h;
-    LGS_REQUIRE(gx * gy + 1 < 65536, "emit_pairs_u16: %d tiles do not fit 16-bit keys", gx * gy);
-    cudaStream_t st = (cudaStream_t)stream;
-    lgs_with_tile(tile_h, tile_w, [&](auto th, auto tw) {
-        emit_pairs_rec_kernel<th, tw, unsigned short><<<lgs_cdiv(n, LGS_EMIT_WARPS * 32), LGS_EMIT_WARPS * 32, 0, st>>>(
-            (const SplatRec*)packed_params, offset, order, n, cap, img_h, img_w, gx, gy, keys, vals, nullptr, nullptr);
-        return LGS_OK;
-    });
-    LGS_CHECK_LAUNCH("emit_pairs_rec_kernel<u16>");
-    return LGS_OK;
-}
-
-// GPU-driven forms: n_capacity bounds the launch, *n_dev is the live splat count; runs that would cross `cap` are dropped (and
-// flagged by lgs_view_params) and *valid_pairs (nullable; normally &params[1]) is lowered to the length of the list that WAS
-// written, so that nothing downstream reads an unwritten slot.  key_bits = 16 or 32.
+// n_capacity bounds the launch, *n_dev is the live splat count; runs that would cross `cap` are dropped (and flagged by
+// lgs_view_params) and *valid_pairs (nullable; normally &params[1]) is lowered to the length of the list that WAS written, so
+// that nothing downstream reads an unwritten slot.  key_bits = 16 (requires tiles + 1 < 65536) or 32.
 extern "C" int lgs_emit_pairs_dev(const float* packed_params, const int* offset, const unsigned* order, int n_capacity, const int* n_dev,
                                   int cap, int img_h, int img_w, int tile_h, int tile_w, int key_bits, void* keys, int* vals,
                                   int* valid_pairs, void* stream)

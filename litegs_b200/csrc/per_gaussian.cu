@@ -21,7 +21,7 @@ void lgs_set_error(const char* fmt, ...)
     va_end(ap);
 }
 extern "C" const char* lgs_last_error(void) { return g_err; }
-extern "C" int lgs_abi_version(void) { return 3; }
+extern "C" int lgs_abi_version(void) { return 4; }
 
 #define VALID_GUARD(idx, n)                                                \
     if ((idx) >= (n) || (valid_length != nullptr && (idx) >= valid_length[0])) return;

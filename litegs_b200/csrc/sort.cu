@@ -41,10 +41,10 @@ int sort_impl()
 // Automatic choice when nothing is forced: the own passes up to 7-bit digits (1080p: 14 tile bits = 2 x 7), cub's onesweep when
 // the tile ids need 8-bit digits on more than 8 M pairs (4K: 16 bits, 71.7 M pairs) -- profiles/microbench/dev_count_bench.py
 // times both.
-int sort_impl_for(int n, int bits, unsigned bias)
+int sort_impl_for(int n, int bits)
 {
     int impl = sort_impl();
-    if (!g_sort_forced && impl == 1 && bias == 0u && bits > 14 && n > (8 << 20)) impl = 0;
+    if (!g_sort_forced && impl == 1 && bits > 14 && n > (8 << 20)) impl = 0;
     return impl;
 }
 
@@ -546,16 +546,15 @@ size_t sort_workspace_bytes(int n, int max_bits)
 
 template <typename KeyT>
 int sort_pairs(const char* who, const KeyT* keys_in, KeyT* keys_out, const unsigned* vals_in, unsigned* vals_out, int n, int begin_bit,
-               int end_bit, unsigned bias, void* workspace, size_t workspace_bytes, void* stream)
+               int end_bit, void* workspace, size_t workspace_bytes, void* stream)
 {
     if (n <= 0) return LGS_OK;
     LGS_REQUIRE(begin_bit >= 0 && end_bit >= begin_bit && end_bit <= (int)(8 * sizeof(KeyT)), "%s: bad bit range [%d, %d)", who, begin_bit,
                 end_bit);
     char* ws = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
     size_t need;
-    const int impl = sort_impl_for(n, end_bit - begin_bit, bias);
+    const int impl = sort_impl_for(n, end_bit - begin_bit);
     if (impl == 0) {
-        if (bias != 0u) { begin_bit = 0; end_bit = 8 * (int)sizeof(KeyT); }   // cub cannot rebase: all bits of the raw keys, same order
         need = 0;
         cub::DeviceRadixSort::SortPairs<KeyT, unsigned>(nullptr, need, nullptr, nullptr, nullptr, nullptr, n, begin_bit, end_bit);
     } else {
@@ -570,7 +569,7 @@ int sort_pairs(const char* who, const KeyT* keys_in, KeyT* keys_out, const unsig
                                                                  (cudaStream_t)stream));
         return LGS_OK;
     }
-    return rs_sort<KeyT>(keys_in, keys_out, vals_in, vals_out, n, begin_bit, end_bit, bias, ws, (cudaStream_t)stream);
+    return rs_sort<KeyT>(keys_in, keys_out, vals_in, vals_out, n, begin_bit, end_bit, 0u, ws, (cudaStream_t)stream);
 }
 
 }  // namespace
@@ -601,18 +600,8 @@ extern "C" int lgs_sort_pairs_u32_workspace_bytes(int n, size_t* bytes)
 extern "C" int lgs_sort_pairs_u32(const unsigned* keys_in, unsigned* keys_out, const unsigned* vals_in, unsigned* vals_out, int n,
                                   int begin_bit, int end_bit, void* workspace, size_t workspace_bytes, void* stream)
 {
-    return sort_pairs<unsigned>("sort_pairs_u32", keys_in, keys_out, vals_in, vals_out, n, begin_bit, end_bit, 0u, workspace,
-                                workspace_bytes, stream);
-}
-
-// Order by (key - bias) on the bits [0, end_bit): for keys known to lie in [bias, bias + 2^end_bit) this is the order of the
-// full keys at fewer passes (view-space z in [1.3, 4.7) spans 31 bits of float pattern but only 24 bits of range).  Keys
-// outside that interval land in unspecified places.
-extern "C" int lgs_sort_pairs_u32_rebased(const unsigned* keys_in, unsigned* keys_out, const unsigned* vals_in, unsigned* vals_out, int n,
-                                          unsigned bias, int end_bit, void* workspace, size_t workspace_bytes, void* stream)
-{
-    return sort_pairs<unsigned>("sort_pairs_u32_rebased", keys_in, keys_out, vals_in, vals_out, n, 0, end_bit, bias, workspace,
-                                workspace_bytes, stream);
+    return sort_pairs<unsigned>("sort_pairs_u32", keys_in, keys_out, vals_in, vals_out, n, begin_bit, end_bit, workspace, workspace_bytes,
+                                stream);
 }
 
 // 16-bit tile keys (tiles+1 < 65536, i.e. anything up to 4K at 8x16): 6 instead of 8 bytes per pair and pass
@@ -625,7 +614,7 @@ extern "C" int lgs_sort_pairs_u16_workspace_bytes(int n, size_t* bytes)
 extern "C" int lgs_sort_pairs_u16(const unsigned short* keys_in, unsigned short* keys_out, const unsigned* vals_in, unsigned* vals_out,
                                   int n, int begin_bit, int end_bit, void* workspace, size_t workspace_bytes, void* stream)
 {
-    return sort_pairs<unsigned short>("sort_pairs_u16", keys_in, keys_out, vals_in, vals_out, n, begin_bit, end_bit, 0u, workspace,
+    return sort_pairs<unsigned short>("sort_pairs_u16", keys_in, keys_out, vals_in, vals_out, n, begin_bit, end_bit, workspace,
                                       workspace_bytes, stream);
 }
 
@@ -634,6 +623,9 @@ extern "C" int lgs_sort_pairs_u16(const unsigned short* keys_in, unsigned short*
 // for the rebased depth sort, the bias from *bias_dev -- no read-back, so a whole view can be enqueued (or captured in a
 // CUDA graph) without a host synchronisation (SURVEY 7 "GPU-driven sizing"; the reference hides its two read-backs behind last
 // epoch's feedback values instead, GR/compact.cu:527-549, GR/binning.cu:137-163).  Own radix sort only.
+// The depth sort orders by (key - *bias_dev) on the bits [0, end_bit): for keys known to lie in [bias, bias + 2^end_bit) this is
+// the order of the full keys at fewer passes (view-space z in [1.3, 4.7) spans 31 bits of float pattern but only 24 bits of
+// range).  Keys outside that interval land in unspecified places.
 extern "C" int lgs_sort_pairs_u32_dev(const unsigned* keys_in, unsigned* keys_out, const unsigned* vals_in, unsigned* vals_out,
                                       int capacity, const int* n_dev, const unsigned* bias_dev, int end_bit, void* workspace,
                                       size_t workspace_bytes, void* stream)

@@ -336,6 +336,7 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
         if stat:
             _feed_statistics(state, stats, pg_, (th, tw))
         losses.append(loss.detach())
+        return state
 
     def one_autograd(i, wait_ev):
         cam = camera_fn(i)
@@ -386,11 +387,8 @@ def render_views(n_views: int, camera_fn, loss_fn, cluster_origin, cluster_exten
         losses.append(loss.detach())
 
     def one_probe(i, wait_ev):
-        n0 = len(pipeline.LAST_VIEW_SIZES)
-        one_direct(i, wait_ev)
-        for pairs, bits in pipeline.LAST_VIEW_SIZES[n0:]:
-            probe["pairs"] = max(probe["pairs"], pairs); probe["bits"] = max(probe["bits"], bits)
-        del pipeline.LAST_VIEW_SIZES[:]
+        state = one_direct(i, wait_ev)
+        probe["pairs"] = max(probe["pairs"], state.n_pairs); probe["bits"] = max(probe["bits"], state.depth_bits)
 
     use_ws = slots is not None and slots.ws is not None
     if use_ws:

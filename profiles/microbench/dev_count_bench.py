@@ -1,5 +1,6 @@
-"""Cost of the GPU-driven (device-side count) entry points against the host-count ones on the C2 sizes:
-tile sort of D = 10.9 M (u16 key, i32 value) pairs on 14 bits, depth sort of 1 M u32 keys on 24 bits, gathered scan of 1 M."""
+"""Cost of the device-side count entry points on the C2 sizes: the tile sort of D = 10.9 M (u16 key, i32 value) pairs on 14 bits
+against its host-count form, the depth sort of 1 M u32 keys on 24 bits and the gathered scan of 1 M (these two have the
+device-count form only); and the host-count tile sort at the C4 size."""
 import ctypes
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
@@ -45,18 +46,16 @@ _lib.call("lgs_sort_pairs_u32_workspace_bytes", N, ctypes.byref(nb))
 ws = torch.empty(nb.value, dtype=torch.uint8, device=dev)
 ndev = torch.tensor([984_960], dtype=torch.int32, device=dev)
 bias = torch.zeros(1, dtype=torch.int32, device=dev)
-t_host = timeit(lambda: _lib.call("lgs_sort_pairs_u32_rebased", P(k32), P(ko), P(v32), P(vo), 984_960, 0, 24, P(ws), ctypes.c_size_t(nb.value), st()))
 t_dev = timeit(lambda: _lib.call("lgs_sort_pairs_u32_dev", P(k32), P(ko), P(v32), P(vo), N, P(ndev), P(bias), 24, P(ws), ctypes.c_size_t(nb.value), st()))
-print(f"depth sort N=984960 (capacity {N}): host count {t_host:.1f} us, device count {t_dev:.1f} us")
+print(f"depth sort N=984960 (capacity {N}): device count {t_dev:.1f} us")
 cnt = torch.randint(0, 20, (N,), device=dev, dtype=torch.int32)
 out = torch.empty(N, dtype=torch.int32, device=dev)
 nb2 = ctypes.c_size_t(0)
 _lib.call("lgs_scan_gathered_workspace_bytes", N, ctypes.byref(nb2))
 ws2 = torch.empty(nb2.value, dtype=torch.uint8, device=dev)
 order = torch.randperm(N, device=dev).to(torch.int32)
-t_host = timeit(lambda: _lib.call("lgs_scan_gathered", P(cnt), P(order), 984_960, P(out), P(ws2), ctypes.c_size_t(nb2.value), st()))
 t_dev = timeit(lambda: _lib.call("lgs_scan_gathered_dev", P(cnt), P(order), N, P(ndev), P(out), P(ws2), ctypes.c_size_t(nb2.value), st()))
-print(f"gathered scan: host count {t_host:.1f} us, device count {t_dev:.1f} us")
+print(f"gathered scan: device count {t_dev:.1f} us")
 
 # C4-sized tile sort (71.7 M pairs, 16 bits)
 D4 = 71_700_532

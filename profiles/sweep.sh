@@ -2,7 +2,7 @@
 # A/B sweeps on the C2 workload; prints views/s and per-stage ms/view.  Usage: bash profiles/sweep.sh [tiles|switches|streams]
 # (scratch output goes to $SWEEP_DIR, default a fresh temporary directory)
 # Switches (all default to the faster setting; each keeps the other implementation selectable for cross-checks):
-#   LGS_SORT=lgs|cub            own radix sort | cub::DeviceRadixSort          LGS_TILE_RANGE=search|scan   lower_bound per tile | streaming
+#   LGS_SORT=lgs|cub            own radix sort | cub::DeviceRadixSort
 #   LGS_STAGING=cpasync|bulk    3 x cp.async | cp.async.bulk + mbarrier         LGS_BWD_REDUCE=smem|butterfly  backward warp reduction
 #   LGS_VIEWS_AUTOGRAD=0|1      render_views direct | through the autograd Function     LGS_WPB=4|2|1  tiles per CTA
 SWEEP_DIR=${SWEEP_DIR:-$(mktemp -d)}
@@ -24,7 +24,6 @@ elif [ "$what" = streams ]; then
 else
   EXTRA="" run "defaults" LGS_WPB=4
   EXTRA="" run "LGS_SORT=cub" LGS_SORT=cub
-  EXTRA="" run "LGS_TILE_RANGE=scan" LGS_TILE_RANGE=scan
   EXTRA="" run "LGS_STAGING=bulk" LGS_STAGING=bulk
   EXTRA="" run "LGS_BWD_REDUCE=butterfly" LGS_BWD_REDUCE=butterfly
   EXTRA="" run "LGS_VIEWS_AUTOGRAD=1" LGS_VIEWS_AUTOGRAD=1

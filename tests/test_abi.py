@@ -22,7 +22,7 @@ def _header_decls():
     return out
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_every_declared_symbol_of_abi_4():
     from litegs_b200 import _lib, build
     build.build()
     lib = ctypes.CDLL(_lib.LIB_PATH)
@@ -34,7 +34,7 @@ def test_library_exports_every_declared_symbol():
     for name, n in decls.items():
         if name in _lib.SIGNATURES:
             assert len(_lib.SIGNATURES[name]) == n, name
-    assert lib.lgs_abi_version() == 3
+    assert lib.lgs_abi_version() == 4
 
 
 def test_library_contains_sm90a_code_and_bulk_copy():

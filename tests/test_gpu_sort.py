@@ -95,10 +95,13 @@ def test_sort_pairs_matches_stable_sort(cuda, impl, dtype, n, begin, end, kind):
     assert torch.equal(ko, ek)
 
 
+@pytest.mark.parametrize("junk", [0, 40_000], ids=["capacity_is_count", "junk_past_count"])
 @pytest.mark.parametrize("impl", list(IMPLS))
-def test_rebased_depth_sort_orders_keys_inside_the_range(cuda, impl):
-    """lgs_sort_pairs_u32_rebased: keys inside [bias, bias + 2^bits) come out in full-key stable order; the keys outside
-    (culled splats, all ones) may land anywhere but must all still be present."""
+def test_device_count_depth_sort_orders_keys_inside_the_range(cuda, impl, junk):
+    """lgs_sort_pairs_u32_dev, the depth sort of both view paths: keys inside [*bias_dev, *bias_dev + 2^bits) come out in full-key
+    stable order; the keys outside (culled splats, all ones) may land anywhere but must all still be present.  The launch covers
+    the live count plus `junk` unsorted slots past *n_dev (the synchronising path launches exactly the count, the workspace a
+    capacity); forcing cub (LGS_SORT) does not reach this sort: it is the own radix sort in every setting."""
     g = torch.Generator(device="cpu").manual_seed(7)
     n = 700_001
     z = torch.rand(n, generator=g) * 3.4 + 1.3                       # crosses the 2.0 and 4.0 exponent boundaries
@@ -108,22 +111,26 @@ def test_rebased_depth_sort_orders_keys_inside_the_range(cuda, impl):
     kmin, kmax = int(k[inside].min()), int(k[inside].max())
     bits = max(1, (kmax - kmin).bit_length())
     assert bits <= 24 < (kmin ^ kmax).bit_length()
-    keys = torch.where(k >= (1 << 31), k - (1 << 32), k).to(torch.int32).to(cuda)
-    vals = torch.arange(n, dtype=torch.int32, device=cuda)
+    tail = torch.randint(0, 1 << 31, (junk,), generator=g, dtype=torch.int64)
+    keys = torch.cat([torch.where(k >= (1 << 31), k - (1 << 32), k), tail]).to(torch.int32).to(cuda)
+    vals = torch.cat([torch.arange(n), tail]).to(torch.int32).to(cuda)
+    cap = n + junk
     nb = ctypes.c_size_t(0)
-    _lib.call("lgs_sort_pairs_u32_workspace_bytes", n, ctypes.byref(nb))
+    _lib.call("lgs_sort_pairs_u32_workspace_bytes", cap, ctypes.byref(nb))
     ws = torch.empty(nb.value, dtype=torch.uint8, device=cuda)
     ko, vo = torch.empty_like(keys), torch.empty_like(vals)
+    n_dev = torch.tensor([n], dtype=torch.int32, device=cuda)
+    bias_dev = torch.tensor([kmin], dtype=torch.int32, device=cuda)          # positive float bits: below 2^31
+    ptr = lambda t: ctypes.c_void_p(t.data_ptr())
     _force(impl)
     try:
-        _lib.call("lgs_sort_pairs_u32_rebased", ctypes.c_void_p(keys.data_ptr()), ctypes.c_void_p(ko.data_ptr()),
-                  ctypes.c_void_p(vals.data_ptr()), ctypes.c_void_p(vo.data_ptr()), n, kmin, bits, ctypes.c_void_p(ws.data_ptr()),
+        _lib.call("lgs_sort_pairs_u32_dev", ptr(keys), ptr(ko), ptr(vals), ptr(vo), cap, ptr(n_dev), ptr(bias_dev), bits, ptr(ws),
                   ctypes.c_size_t(nb.value), None)
     finally:
         _unforce()
     torch.cuda.synchronize()
-    vo_c, ko_c = vo.cpu().long(), ko.cpu()
-    assert torch.equal(torch.sort(vo_c).values, torch.arange(n))      # a permutation
+    vo_c, ko_c = vo[:n].cpu().long(), ko[:n].cpu()
+    assert torch.equal(torch.sort(vo_c).values, torch.arange(n))      # a permutation of the live slots
     assert torch.equal(ko_c.long() & 0xFFFFFFFF, k[vo_c])              # keys travel with their payload
     got = vo_c[inside[vo_c]]                                           # order of the keys that matter
     want = torch.sort(torch.where(inside, k, torch.full_like(k, 1 << 40)), stable=True).indices[: int(inside.sum())]

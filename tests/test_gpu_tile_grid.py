@@ -193,8 +193,8 @@ def _key_list(rng, max_tile, first, last):
 
 
 def _tile_range(cuda, keys, max_tile, fix_last, u16, dev_form):
-    """One call of lgs_tile_range / _u16 / _dev / _u16_dev on `keys`; the _dev forms get a larger capacity whose tail holds
-    garbage (unsorted keys) that a kernel reading past *length_dev would pick up."""
+    """One call of lgs_tile_range / _dev / _u16_dev on `keys`; the _dev forms get a larger capacity whose tail holds garbage
+    (unsorted keys) that a kernel reading past *length_dev would pick up."""
     L = keys.shape[0]
     buf = keys
     if dev_form:
@@ -213,9 +213,13 @@ def _tile_range(cuda, keys, max_tile, fix_last, u16, dev_form):
     return out.cpu().numpy()
 
 
-@pytest.mark.parametrize("dev_form", [False, True], ids=["host_length", "device_length"])
-@pytest.mark.parametrize("u16,max_tile", [(True, 64_800), (True, 65_534), (False, 64_800), (False, 65_534), (False, 65_535),
-                                          (False, 129_600)])
+# the 16-bit keys have the device-length form only
+RANGE_CASES = [(u16, max_tile, dev_form) for dev_form in (False, True) for u16, max_tile in
+               [(True, 64_800), (True, 65_534), (False, 64_800), (False, 65_534), (False, 65_535), (False, 129_600)] if dev_form or not u16]
+
+
+@pytest.mark.parametrize("u16,max_tile,dev_form", RANGE_CASES,
+                         ids=[f"{u}-{m}-{'device_length' if d else 'host_length'}" for u, m, d in RANGE_CASES])
 def test_tile_range_matches_oracle(cuda, u16, max_tile, dev_form):
     rng = np.random.default_rng(max_tile + 7 * u16)
     for first in (0, 1):
@@ -233,30 +237,26 @@ def test_tile_range_matches_oracle(cuda, u16, max_tile, dev_form):
             assert np.array_equal(got, oracle.tileRange(keys[None], max_tile, fix_last=bool(fix_last))), (key, fix_last)
 
 
-def test_16bit_key_guards(cuda):
-    """65,535 tiles do not fit the 16-bit keys (tiles + 1 < 65536): the 16-bit entry points refuse them, 65,534 tiles pass."""
+def test_16bit_key_guards_of_the_device_forms(cuda):
+    """65,535 tiles do not fit the 16-bit keys (tiles + 1 < 65536): the 16-bit forms refuse them, 65,534 tiles pass."""
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
     i32 = lambda *v: torch.tensor(v, dtype=torch.int32, device=cuda)
     keys, vals, ranges = i32(0, 0), i32(0, 0), torch.empty(65_537, dtype=torch.int32, device=cuda)
     packed = torch.zeros((1, 1, 12), dtype=torch.float32, device=cuda)
     offsets, order, n_dev = i32(0), i32(0), i32(1)           # one splat that owns no pair: emission has nothing to write
     for max_tile, ok in ((65_534, True), (65_535, False)):
-        for fn, args in (("lgs_tile_range_u16", (keys.data_ptr(), 1, 1, max_tile, 1, ranges.data_ptr(), st)),
-                         ("lgs_tile_range_u16_dev", (keys.data_ptr(), 1, n_dev.data_ptr(), max_tile, 1, ranges.data_ptr(), st))):
-            if ok:
-                _lib.call(fn, *args)
-            else:
-                with pytest.raises(_lib.LiteGSB200Error):
-                    _lib.call(fn, *args)
+        args = (keys.data_ptr(), 1, n_dev.data_ptr(), max_tile, 1, ranges.data_ptr(), st)
+        if ok:
+            _lib.call("lgs_tile_range_u16_dev", *args)
+        else:
+            with pytest.raises(_lib.LiteGSB200Error):
+                _lib.call("lgs_tile_range_u16_dev", *args)
     for (H, W), ok in (((2410, 3470), True), ((2050, 4075), False)):          # 65,534 and 65,535 tiles of 8x16
-        calls = (("lgs_emit_pairs_u16", (packed.data_ptr(), offsets.data_ptr(), order.data_ptr(), 1, 1, H, W, 8, 16, keys.data_ptr(),
-                                         vals.data_ptr(), st)),
-                 ("lgs_emit_pairs_dev", (packed.data_ptr(), offsets.data_ptr(), order.data_ptr(), 1, n_dev.data_ptr(), 1, H, W, 8, 16, 16,
-                                         keys.data_ptr(), vals.data_ptr(), None, st)))
-        for fn, args in calls:
-            if ok:
-                _lib.call(fn, *args)
-            else:
-                with pytest.raises(_lib.LiteGSB200Error):
-                    _lib.call(fn, *args)
+        args = (packed.data_ptr(), offsets.data_ptr(), order.data_ptr(), 1, n_dev.data_ptr(), 1, H, W, 8, 16, 16, keys.data_ptr(),
+                vals.data_ptr(), None, st)
+        if ok:
+            _lib.call("lgs_emit_pairs_dev", *args)
+        else:
+            with pytest.raises(_lib.LiteGSB200Error):
+                _lib.call("lgs_emit_pairs_dev", *args)
     torch.cuda.synchronize()

@@ -10,7 +10,8 @@ References:
 Cases: zero, one and capacity +- 1 pairs; depth-key ranges of 2^k - 1 and 2^k; a run that straddles the capacity, runs longer than
 the 512-pair emit window, junk past the live count; scenes seen from an identity-rotation camera, so that view-space z is world
 z and the test picks the depth-key bits; a graph captured with one visible-chunk count and replayed with others; a padded image
-at 12x16 tiles and 65,536 8x8 tiles (32-bit tile keys); and overflow flags that land after the next batch was enqueued."""
+at 12x16 tiles and 65,536 8x8 tiles (32-bit tile keys); the last populated tile closed on both paths with Level A's
+CONFIG["fix_last_tile"] off; and overflow flags that land after the next batch was enqueued."""
 import ctypes
 import math
 
@@ -19,7 +20,7 @@ import pytest
 import torch
 
 import oracle
-from litegs_b200 import _lib, pipeline, render
+from litegs_b200 import _lib, fused, pipeline, render
 from litegs_b200.arguments import PipelineParams
 from litegs_b200.dist import GradAccumulator
 from tests import tile_cover_oracle as tc
@@ -426,6 +427,23 @@ def test_small_views_match_the_synchronising_path(cuda, deterministic, case):
     ws.post_flags()
     r = ws.check(wait=True)
     assert r == {"max_pairs": D, "max_depth_bits": 1, "views": 4 * len(cams) + (nvis == 0)}
+
+
+def test_both_paths_close_the_last_tile_with_fix_last_tile_off(cuda, deterministic, monkeypatch):
+    """CONFIG["fix_last_tile"] = False selects the reference's open last tile for Level A (tileRange) only: on a view whose last
+    populated tile is not the grid's last, both fused paths still close it and the workspace equals S bit for bit."""
+    monkeypatch.setitem(fused.CONFIG, "fix_last_tile", False)
+    hw, tile = (64, 96), (16, 16)
+    P, aabb, cams = edge_scenes(hw)["one splat"]
+    P, A, cams = to_dev(cuda, P, aabb, cams)
+    d_img = torch.from_numpy(np.random.default_rng(5).normal(size=(1, 3, *hw)).astype(np.float32)).to(cuda)
+    img, st, acc_s = sync_view(P, A, cams[0], hw, tile, d_img)
+    D, r = st.n_pairs, st.ranges[0].cpu().numpy()
+    ntile = r.shape[0] - 2
+    top = int(np.flatnonzero((r[:ntile + 1] >= 0) & (r[:ntile + 1] < D)).max())      # highest populated (tile + 1) key
+    assert 0 < D and top < ntile and r[top + 1] == D
+    ws = pipeline.ViewWorkspace(P, hw, tile, pair_capacity=1024, planned_depth_bits=32)
+    workspace_runs(ws, P, A, cams, d_img, lambda i, acc, rnd: assert_matches_sync(ws, img, st, acc, acc_s, rnd))
 
 
 def depth_scene(hw, bits):
