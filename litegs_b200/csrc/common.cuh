@@ -117,4 +117,18 @@ __device__ __forceinline__ void lgs_finish_raster_grad(const float4& a, const fl
     g.dC = -0.5f * c.x;
     g.dop = (o > 0.0f) ? e.x / o : 0.0f;
 }
+
+// The splat's gradient to ndc (x, y), to the 2D inverse covariance (dBh = d [0][1] = d [1][0]), to the colour and to the
+// opacity, each times the de-normaliser s of the max-normalised image gradient (wrapper.py:490-494).
+struct LgsRecordGrad { float dndcx, dndcy, dA, dBh, dC, dcol[3], dop; };
+__device__ __forceinline__ void lgs_record_grad(const float4& a, const float4& c, const float4& e, float A, float B, float C, float o,
+                                                int H, int W, float s, LgsRecordGrad& d)
+{
+    LgsRasterGrad g;
+    lgs_finish_raster_grad(a, c, e, A, B, C, o, g);
+    d.dndcx = g.dmx * 0.5f * W * s; d.dndcy = g.dmy * 0.5f * H * s;
+    d.dA = g.dA * s; d.dBh = g.dB * 0.5f * s; d.dC = g.dC * s;
+    d.dcol[0] = c.y * s; d.dcol[1] = c.z * s; d.dcol[2] = c.w * s;
+    d.dop = g.dop * s;
+}
 #endif

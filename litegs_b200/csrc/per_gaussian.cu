@@ -7,7 +7,7 @@
 // materialises the intermediates these kernels exchange through HBM.
 #include <stdarg.h>
 #include "common.cuh"
-#include "sh.cuh"
+#include "projection.cuh"
 
 // ------------------------------------------------------------------------------------------------
 // error string plumbing
@@ -132,27 +132,22 @@ __global__ void activate_forward_kernel(
     const size_t src = (size_t)chunk_ids[a] * S + s;
     float p[3] = { pos[src], pos[CS + src], pos[2 * CS + src] };
     apos[dst] = p[0]; apos[AS + dst] = p[1]; apos[2 * AS + dst] = p[2]; apos[3 * AS + dst] = 1.0f;
+    const float sr_[3] = { scale[src], scale[CS + src], scale[2 * CS + src] };
+    const float q[4] = { rot[src], rot[CS + src], rot[2 * CS + src], rot[3 * CS + src] };
+    float sa[3], qn[4];
+    lgs_activate_scale(sr_, sa);
+    lgs_normalize_quat(q, qn);
 #pragma unroll
-    for (int k = 0; k < 3; k++) ascale[k * AS + dst] = expf(scale[k * CS + src]);
-    float q0 = rot[src], q1 = rot[CS + src], q2 = rot[2 * CS + src], q3 = rot[3 * CS + src];
-    float rn = 1.0f / sqrtf(q0 * q0 + q1 * q1 + q2 * q2 + q3 * q3 + 1e-12f);
-    arot[dst] = q0 * rn; arot[AS + dst] = q1 * rn; arot[2 * AS + dst] = q2 * rn; arot[3 * AS + dst] = q3 * rn;
-    aopac[dst] = 1.0f / (1.0f + expf(-opac[src]));
+    for (int k = 0; k < 3; k++) ascale[k * AS + dst] = sa[k];
+#pragma unroll
+    for (int k = 0; k < 4; k++) arot[k * AS + dst] = qn[k];
+    aopac[dst] = lgs_sigmoid(opac[src]);
     for (int v = 0; v < V; v++) {
-        float cc[3];
-        lgs_camera_center(view + v * 16, cc);
-        float d0 = p[0] - cc[0], d1 = p[1] - cc[1], d2 = p[2] - cc[2];
-        float dn = 1.0f / sqrtf(d0 * d0 + d1 * d1 + d2 * d2 + 1e-12f);
-        float b[16];
-        lgs_sh_basis<DEG>(d0 * dn, d1 * dn, d2 * dn, b);
-        constexpr int K = (DEG + 1) * (DEG + 1);
+        float dirn[3], col[3];
+        lgs_view_dir(view + v * 16, p, dirn);
+        lgs_sh_color<DEG>(dirn[0], dirn[1], dirn[2], sh0, shr, src, CS, col);
 #pragma unroll
-        for (int c = 0; c < 3; c++) {
-            float r = b[0] * sh0[c * CS + src];
-#pragma unroll
-            for (int k = 1; k < K; k++) r += b[k] * shr[((size_t)(k - 1) * 3 + c) * CS + src];
-            color[((size_t)v * 3 + c) * AS + dst] = r + 0.5f;
-        }
+        for (int c = 0; c < 3; c++) color[((size_t)v * 3 + c) * AS + dst] = col[c];
     }
 }
 
@@ -194,19 +189,18 @@ __global__ void activate_backward_kernel(
     const size_t dst = (size_t)a * S + s, src = (size_t)chunk_ids[a] * S + s;
 #pragma unroll
     for (int k = 0; k < 3; k++) g_pos[k * AS + dst] = g_apos[k * AS + dst];
+    const float sr_[3] = { scale[src], scale[CS + src], scale[2 * CS + src] };
+    float q[4], g[4], sa[3], qn[4], dq[4];
+    lgs_activate_scale(sr_, sa);
 #pragma unroll
-    for (int k = 0; k < 3; k++) g_scale[k * AS + dst] = expf(scale[k * CS + src]) * g_ascale[k * AS + dst];
-    float q[4], g[4], o[4];
+    for (int k = 0; k < 3; k++) g_scale[k * AS + dst] = sa[k] * g_ascale[k * AS + dst];
 #pragma unroll
     for (int k = 0; k < 4; k++) { q[k] = rot[k * CS + src]; g[k] = g_arot[k * AS + dst]; }
-    float rn = 1.0f / sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] + 1e-12f);
+    const float rn = lgs_normalize_quat(q, qn);
+    lgs_quat_normalize_backward(g, qn, rn, dq);
 #pragma unroll
-    for (int k = 0; k < 4; k++) o[k] = q[k] * rn;
-    float dot = g[0] * o[0] + g[1] * o[1] + g[2] * o[2] + g[3] * o[3];
-#pragma unroll
-    for (int k = 0; k < 4; k++) g_rot[k * AS + dst] = rn * (g[k] - dot * o[k]);
-    const float u = 1.0f / (1.0f + expf(opac[src])), sig = 1.0f - u;     // 1 - sig = u, not formed from the rounded sig
-    g_opac[dst] = g_aopac[dst] * (true_sigmoid ? sig * u : sig);
+    for (int k = 0; k < 4; k++) g_rot[k * AS + dst] = dq[k];
+    g_opac[dst] = lgs_sigmoid_backward(g_aopac[dst], opac[src], true_sigmoid);
 
     float p[3] = { pos[src], pos[CS + src], pos[2 * CS + src] };
     constexpr int K = (DEG + 1) * (DEG + 1);
@@ -216,12 +210,9 @@ __global__ void activate_backward_kernel(
 #pragma unroll
         for (int k = 0; k < K; k++) acc[c][k] = 0.0f;
     for (int v = 0; v < V; v++) {
-        float cc[3];
-        lgs_camera_center(view + v * 16, cc);
-        float d0 = p[0] - cc[0], d1 = p[1] - cc[1], d2 = p[2] - cc[2];
-        float dn = 1.0f / sqrtf(d0 * d0 + d1 * d1 + d2 * d2 + 1e-12f);
-        float b[16];
-        lgs_sh_basis<DEG>(d0 * dn, d1 * dn, d2 * dn, b);
+        float dirn[3], b[16];
+        lgs_view_dir(view + v * 16, p, dirn);
+        lgs_sh_basis<DEG>(dirn[0], dirn[1], dirn[2], b);
 #pragma unroll
         for (int c = 0; c < 3; c++) {
             float gc = g_color[((size_t)v * 3 + c) * AS + dst];
@@ -279,11 +270,8 @@ __global__ void mvp_forward_kernel(const float* __restrict__ view, const float* 
     float w[4], v[4], h[4];
 #pragma unroll
     for (int k = 0; k < 4; k++) w[k] = pos[(size_t)k * N + i];
-#pragma unroll
-    for (int k = 0; k < 4; k++) v[k] = w[0] * Vm[k] + w[1] * Vm[4 + k] + w[2] * Vm[8 + k] + w[3] * Vm[12 + k];
-#pragma unroll
-    for (int k = 0; k < 4; k++) h[k] = v[0] * P[k] + v[1] * P[4 + k] + v[2] * P[8 + k] + v[3] * P[12 + k];
-    float iw = (fabsf(h[3]) > 1e-12f) ? (1.0f / h[3]) : 0.0f;
+    lgs_mvp_view(Vm, w, v);
+    float iw = lgs_mvp_clip(P, v, h);
     size_t o = (size_t)b * 4 * N + i;
 #pragma unroll
     for (int k = 0; k < 4; k++) vpos[o + (size_t)k * N] = v[k];
@@ -313,23 +301,16 @@ __global__ void mvp_backward_kernel(const float* __restrict__ g_ndc, const float
     for (int b = 0; b < V; b++) {
         const float* Vm = view + b * 16; const float* P = proj + b * 16;
         size_t o = (size_t)b * 4 * N + i;
-        float v[4], h[4], gn[4], dh[4], dv[4];
+        float v[4], h[4], gn[4], gv[4], dh[4], dv[4], dw[4];
 #pragma unroll
         for (int k = 0; k < 4; k++) v[k] = vpos[o + (size_t)k * N];
+        const float iw = lgs_mvp_clip(P, v, h);
 #pragma unroll
-        for (int k = 0; k < 4; k++) h[k] = v[0] * P[k] + v[1] * P[4 + k] + v[2] * P[8 + k] + v[3] * P[12 + k];
-        float iw = (fabsf(h[3]) > 1e-12f) ? (1.0f / h[3]) : 0.0f;
-        float n0 = h[0] * iw, n1 = h[1] * iw, n2 = h[2] * iw;
+        for (int k = 0; k < 4; k++) { gn[k] = g_ndc[o + (size_t)k * N]; gv[k] = g_view[o + (size_t)k * N]; }
+        lgs_mvp_clip_backward(P, h, iw, gn, gv, dh, dv);
+        lgs_mvp_view_backward(Vm, dv, dw);
 #pragma unroll
-        for (int k = 0; k < 4; k++) gn[k] = g_ndc[o + (size_t)k * N];
-        dh[0] = gn[0] * iw; dh[1] = gn[1] * iw; dh[2] = gn[2] * iw;
-        dh[3] = -(gn[0] * n0 + gn[1] * n1 + gn[2] * n2) * iw;
-#pragma unroll
-        for (int k = 0; k < 4; k++)
-            dv[k] = dh[0] * P[k * 4] + dh[1] * P[k * 4 + 1] + dh[2] * P[k * 4 + 2] + dh[3] * P[k * 4 + 3] + g_view[o + (size_t)k * N];
-#pragma unroll
-        for (int k = 0; k < 4; k++)
-            acc[k] += dv[0] * Vm[k * 4] + dv[1] * Vm[k * 4 + 1] + dv[2] * Vm[k * 4 + 2] + dv[3] * Vm[k * 4 + 3];
+        for (int k = 0; k < 4; k++) acc[k] += dw[k];
     }
 #pragma unroll
     for (int k = 0; k < 4; k++) g_pos[(size_t)k * N + i] = acc[k];
@@ -350,20 +331,13 @@ extern "C" int lgs_mvp_transform_backward(const float* grad_ndc_pos, const float
 // ------------------------------------------------------------------------------------------------
 // T = diag(s) R(q).                                                   replaces GR/transform.cu:92-256
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void quat_R(float r, float x, float y, float z, float* R)
-{
-    R[0] = 1 - 2 * (y * y + z * z); R[1] = 2 * (x * y + r * z);     R[2] = 2 * (x * z - r * y);
-    R[3] = 2 * (x * y - r * z);     R[4] = 1 - 2 * (x * x + z * z); R[5] = 2 * (y * z + r * x);
-    R[6] = 2 * (x * z + r * y);     R[7] = 2 * (y * z - r * x);     R[8] = 1 - 2 * (x * x + y * y);
-}
-
 __global__ void transform_forward_kernel(const float* __restrict__ quat, const float* __restrict__ scale,
                                          const int* __restrict__ valid_length, float* __restrict__ T, int N)
 {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     VALID_GUARD(i, N);
     float R[9];
-    quat_R(quat[i], quat[(size_t)N + i], quat[2 * (size_t)N + i], quat[3 * (size_t)N + i], R);
+    lgs_quat_R(quat[i], quat[(size_t)N + i], quat[2 * (size_t)N + i], quat[3 * (size_t)N + i], R);
 #pragma unroll
     for (int a = 0; a < 3; a++) {
         float s = scale[(size_t)a * N + i];
@@ -389,20 +363,15 @@ __global__ void transform_backward_kernel(const float* __restrict__ gT, const fl
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     VALID_GUARD(i, N);
     float r = quat[i], x = quat[(size_t)N + i], y = quat[2 * (size_t)N + i], z = quat[3 * (size_t)N + i];
-    float R[9], dt[9];
-    quat_R(r, x, y, z, R);
+    float R[9], dt[9], dq[4];
+    lgs_quat_R(r, x, y, z, R);
 #pragma unroll
     for (int k = 0; k < 9; k++) dt[k] = gT[(size_t)k * N + i];
 #pragma unroll
-    for (int a = 0; a < 3; a++) {
-        g_scale[(size_t)a * N + i] = R[a * 3] * dt[a * 3] + R[a * 3 + 1] * dt[a * 3 + 1] + R[a * 3 + 2] * dt[a * 3 + 2];
-        float s = scale[(size_t)a * N + i];
-        dt[a * 3] *= s; dt[a * 3 + 1] *= s; dt[a * 3 + 2] *= s;
-    }
-    g_quat[i] = 2 * z * (dt[1] - dt[3]) + 2 * y * (dt[6] - dt[2]) + 2 * x * (dt[5] - dt[7]);
-    g_quat[(size_t)N + i] = 2 * y * (dt[3] + dt[1]) + 2 * z * (dt[6] + dt[2]) + 2 * r * (dt[5] - dt[7]) - 4 * x * (dt[8] + dt[4]);
-    g_quat[2 * (size_t)N + i] = 2 * x * (dt[3] + dt[1]) + 2 * r * (dt[6] - dt[2]) + 2 * z * (dt[5] + dt[7]) - 4 * y * (dt[8] + dt[0]);
-    g_quat[3 * (size_t)N + i] = 2 * r * (dt[1] - dt[3]) + 2 * x * (dt[6] + dt[2]) + 2 * y * (dt[5] + dt[7]) - 4 * z * (dt[4] + dt[0]);
+    for (int a = 0; a < 3; a++) g_scale[(size_t)a * N + i] = lgs_scale_rot_backward(R + a * 3, scale[(size_t)a * N + i], dt + a * 3);
+    lgs_quat_R_backward(r, x, y, z, dt, dq);
+#pragma unroll
+    for (int k = 0; k < 4; k++) g_quat[(size_t)k * N + i] = dq[k];
 }
 
 extern "C" int lgs_create_transform_matrix_backward(const float* transform_grad, const float* quaternion, const float* scale,
@@ -431,16 +400,11 @@ __global__ void jacobian_kernel(const float* __restrict__ vpos, const float* __r
     bool live = !(valid_length != nullptr && i >= valid_length[0]);
     float j00 = 0.f, j11 = 0.f, j20 = 0.f, j21 = 0.f;
     if (live) {
-        float p00 = proj[b * 16], p11 = proj[b * 16 + 5];
-        float fx = p00 * W * 0.5f, fy = p11 * H * 0.5f;
         size_t vo = (size_t)b * 4 * N + i;
-        float tx = vpos[vo], ty = vpos[vo + N], tz = vpos[vo + 2 * (size_t)N];
-        float lx = tz / p00 * 1.3f, ly = tz / p11 * 1.3f;
-        tx = fmaxf(fminf(tx, lx), -lx);
-        ty = fmaxf(fminf(ty, ly), -ly);
-        float rz = 1.0f / fmaxf(tz, 1e-2f);
-        float rz2 = rz * rz;
-        j00 = fx * rz; j11 = fy * rz; j20 = -fx * tx * rz2; j21 = -fy * ty * rz2;
+        const float v[3] = { vpos[vo], vpos[vo + N], vpos[vo + 2 * (size_t)N] };
+        float Jr[6];
+        lgs_ray_J(proj + b * 16, v, H, W, Jr);
+        j00 = Jr[0]; j11 = Jr[3]; j20 = Jr[4]; j21 = Jr[5];
     }
     J[o] = j00; J[o + (size_t)N] = 0.f; J[o + 2 * (size_t)N] = 0.f;
     J[o + 3 * (size_t)N] = 0.f; J[o + 4 * (size_t)N] = j11; J[o + 5 * (size_t)N] = 0.f;
@@ -461,32 +425,19 @@ extern "C" int lgs_jacobian_rayspace(const float* view_pos, const float* proj_ma
 // ------------------------------------------------------------------------------------------------
 // cov2d = (T V3 J)^T (T V3 J) + 0.3 I and its backward.              replaces GR/transform.cu:736-927
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void cov_M(const float* __restrict__ T, int N, int i, const float* __restrict__ Vm,
-                                      const float* __restrict__ Jb, float* VJ, float* M)
+// the [3,2] block of the [3,3,N] Jacobian and the [3,3,N] T of Gaussian i, then M = T.V3.J
+__device__ __forceinline__ void load_cov_M(const float* __restrict__ T, int N, int i, const float* __restrict__ Vm,
+                                           const float* __restrict__ Jb, float* VJ, float* M)
 {
-    float Jl[6];
+    float Jl[6], Tl[9];
 #pragma unroll
     for (int a = 0; a < 3; a++)
 #pragma unroll
         for (int c = 0; c < 2; c++) Jl[a * 2 + c] = Jb[((size_t)a * 3 + c) * N + i];
 #pragma unroll
-    for (int a = 0; a < 3; a++)
-#pragma unroll
-        for (int c = 0; c < 2; c++) {
-            float t = 0.f;
-#pragma unroll
-            for (int k = 0; k < 3; k++) t += Vm[a * 4 + k] * Jl[k * 2 + c];
-            VJ[a * 2 + c] = t;
-        }
-#pragma unroll
-    for (int a = 0; a < 3; a++)
-#pragma unroll
-        for (int c = 0; c < 2; c++) {
-            float t = 0.f;
-#pragma unroll
-            for (int k = 0; k < 3; k++) t += T[((size_t)a * 3 + k) * N + i] * VJ[k * 2 + c];
-            M[a * 2 + c] = t;
-        }
+    for (int k = 0; k < 9; k++) Tl[k] = T[(size_t)k * N + i];
+    const float one[3] = { 1.0f, 1.0f, 1.0f };
+    lgs_cov_M(Vm, Jl, Tl, one, VJ, M);
 }
 
 __global__ void cov2d_forward_kernel(const float* __restrict__ J, const float* __restrict__ view, const float* __restrict__ T,
@@ -494,11 +445,9 @@ __global__ void cov2d_forward_kernel(const float* __restrict__ J, const float* _
 {
     int i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
     VALID_GUARD(i, N);
-    float VJ[6], M[6];
-    cov_M(T, N, i, view + b * 16, J + (size_t)b * 9 * N, VJ, M);
-    float c00 = M[0] * M[0] + M[2] * M[2] + M[4] * M[4] + 0.3f;
-    float c01 = M[0] * M[1] + M[2] * M[3] + M[4] * M[5];
-    float c11 = M[1] * M[1] + M[3] * M[3] + M[5] * M[5] + 0.3f;
+    float VJ[6], M[6], c00, c01, c11;
+    load_cov_M(T, N, i, view + b * 16, J + (size_t)b * 9 * N, VJ, M);
+    lgs_cov2d(M, c00, c01, c11);
     size_t o = (size_t)b * 4 * N + i;
     cov[o] = c00; cov[o + N] = c01; cov[o + 2 * (size_t)N] = c01; cov[o + 3 * (size_t)N] = c11;
 }
@@ -525,18 +474,13 @@ __global__ void cov2d_backward_kernel(const float* __restrict__ g_cov, const flo
     for (int k = 0; k < 9; k++) acc[k] = 0.f;
     if (!(valid_length != nullptr && i >= valid_length[0])) {
         for (int b = 0; b < V; b++) {
-            float VJ[6], M[6], G[4], dM[6];
-            cov_M(T, N, i, view + b * 16, J + (size_t)b * 9 * N, VJ, M);
+            float VJ[6], M[6], G[4], dM[6], dT[9];
+            load_cov_M(T, N, i, view + b * 16, J + (size_t)b * 9 * N, VJ, M);
 #pragma unroll
             for (int k = 0; k < 4; k++) G[k] = g_cov[((size_t)b * 4 + k) * N + i];
+            lgs_cov2d_backward(M, VJ, G, dM, dT);
 #pragma unroll
-            for (int a = 0; a < 3; a++)
-#pragma unroll
-                for (int c = 0; c < 2; c++) dM[a * 2 + c] = 2.f * (M[a * 2] * G[c] + M[a * 2 + 1] * G[2 + c]);
-#pragma unroll
-            for (int a = 0; a < 3; a++)
-#pragma unroll
-                for (int k = 0; k < 3; k++) acc[a * 3 + k] += dM[a * 2] * VJ[k * 2] + dM[a * 2 + 1] * VJ[k * 2 + 1];
+            for (int k = 0; k < 9; k++) acc[k] += dT[k];
         }
     }
 #pragma unroll
@@ -565,9 +509,6 @@ __global__ void eigh_inv_forward_kernel(const float* __restrict__ in, const int*
     VALID_GUARD(i, N);
     size_t o = (size_t)b * 4 * N + i;
     float m00 = in[o], m01 = in[o + N], m10 = in[o + 2 * (size_t)N], m11 = in[o + 3 * (size_t)N];
-    float det = m00 * m11 - m01 * m10;
-    float det1 = (m00 - m01) * (m11 - m01) + m01 * (m00 + m11 - 2 * m01);
-    det = (fabsf(det) < fabsf(1e-5f * m01 * m10)) ? det1 : det;
     float t0 = m00 + m11;
     float t1 = sqrtf((m00 - m11) * (m00 - m11) + 4 * m01 * m01);
     t1 = fmaxf(t1, 1e-9f);
@@ -579,9 +520,10 @@ __global__ void eigh_inv_forward_kernel(const float* __restrict__ in, const int*
     else { v00 = m11 - e0; v01 = -m01; v10 = m01; v11 = e1 - m00; }
     float l0 = 1.0f / sqrtf(v00 * v00 + v01 * v01), l1 = 1.0f / sqrtf(v10 * v10 + v11 * v11);
     vec[o] = v00 * l0; vec[o + N] = v10 * l1; vec[o + 2 * (size_t)N] = v01 * l0; vec[o + 3 * (size_t)N] = v11 * l1;
-    det = (fabsf(det) < 1e-9f) ? 1e-9f : det;
-    float dr = 1.0f / det;
-    inv[o] = m11 * dr; inv[o + N] = -m01 * dr; inv[o + 2 * (size_t)N] = -m10 * dr; inv[o + 3 * (size_t)N] = m00 * dr;
+    float iv[4];
+    lgs_inv2x2(m00, m01, m10, m11, iv);
+#pragma unroll
+    for (int k = 0; k < 4; k++) inv[o + (size_t)k * N] = iv[k];
 }
 
 extern "C" int lgs_eigh_and_inv_2x2_forward(const float* input, const int* valid_length, int V, int N, float* val, float* vec,
@@ -600,15 +542,12 @@ __global__ void inv2x2_backward_kernel(const float* __restrict__ inv, const floa
     int i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
     VALID_GUARD(i, N);
     size_t o = (size_t)b * 4 * N + i;
-    float A[4], G[4], t[4];
+    float A[4], G[4], d[4];
 #pragma unroll
     for (int k = 0; k < 4; k++) { A[k] = inv[o + (size_t)k * N]; G[k] = g_inv[o + (size_t)k * N]; }
-    t[0] = A[0] * G[0] + A[1] * G[2]; t[1] = A[0] * G[1] + A[1] * G[3];
-    t[2] = A[2] * G[0] + A[3] * G[2]; t[3] = A[2] * G[1] + A[3] * G[3];
-    g_in[o] = -(t[0] * A[0] + t[1] * A[2]);
-    g_in[o + N] = -(t[0] * A[1] + t[1] * A[3]);
-    g_in[o + 2 * (size_t)N] = -(t[2] * A[0] + t[3] * A[2]);
-    g_in[o + 3 * (size_t)N] = -(t[2] * A[1] + t[3] * A[3]);
+    lgs_inv2x2_backward(A, G, d);
+#pragma unroll
+    for (int k = 0; k < 4; k++) g_in[o + (size_t)k * N] = d[k];
 }
 
 extern "C" int lgs_inv_2x2_backward(const float* inv_matrix, const float* grad_inv, const int* valid_length, int V, int N,
@@ -630,17 +569,11 @@ __global__ void sh2rgb_forward_kernel(const float* __restrict__ sh0, const float
 {
     int i = blockIdx.x * blockDim.x + threadIdx.x, v = blockIdx.y;
     if (i >= N) return;
-    constexpr int K = (DEG + 1) * (DEG + 1);
-    float b[16];
+    float col[3];
     size_t od = (size_t)v * 3 * N + i;
-    lgs_sh_basis<DEG>(dirs[od], dirs[od + N], dirs[od + 2 * (size_t)N], b);
+    lgs_sh_color<DEG>(dirs[od], dirs[od + N], dirs[od + 2 * (size_t)N], sh0, shr, i, N, col);
 #pragma unroll
-    for (int c = 0; c < 3; c++) {
-        float r = b[0] * sh0[(size_t)c * N + i];
-#pragma unroll
-        for (int k = 1; k < K; k++) r += b[k] * shr[((size_t)(k - 1) * 3 + c) * N + i];
-        rgb[od + (size_t)c * N] = r + 0.5f;
-    }
+    for (int c = 0; c < 3; c++) rgb[od + (size_t)c * N] = col[c];
 }
 
 extern "C" int lgs_sh2rgb_forward(int degree, const float* sh_base, const float* sh_rest, const float* dirs, int V, int N,

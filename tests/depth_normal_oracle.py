@@ -8,7 +8,7 @@ import numpy as np
 
 
 def intrinsics(proj, H, W, dt=np.float32):
-    """(fx, fy) = ((P[0][0] W) 0.5, (P[1][1] H) 0.5) in dt, as fused_J."""
+    """(fx, fy) = ((P[0][0] W) 0.5, (P[1][1] H) 0.5) in dt, as lgs_ray_J."""
     P = np.asarray(proj, np.float64).reshape(4, 4).astype(dt)
     return (P[0, 0] * dt(W)) * dt(0.5), (P[1, 1] * dt(H)) * dt(0.5)
 

@@ -3,7 +3,7 @@
 The mode (DESIGN.md section 1, "Exact gradient mode") adds two terms to the position gradient and to the camera gradient that
 the default convention drops:
 
-- through the ray-space Jacobian J (``fused_J`` in fused.cu, ``jacobianRayspace`` of the oracle): dM = 2 M G with G the whole
+- through the ray-space Jacobian J (``lgs_ray_J`` in projection.cuh, ``jacobianRayspace`` of the oracle): dM = 2 M G with G the whole
   d cov2d (the antialiased term included), dVJ = T^T dM, dJ[k][c] = sum_a V3[a][k] dVJ[a][c], and ``J_backward`` takes dJ00,
   dJ11, dJ20, dJ21 back to the view-space position and to P00, P11, one clamp branch at a time;
 - through the SH view direction: with d = p - cc, n = 1 / sqrt(|d|^2 + 1e-12) and u = d n, g_u = sum_k w_k d b_k / du with
@@ -22,7 +22,7 @@ SH_C3 = (-0.5900435899266435, 2.890611442640554, -0.4570457994644658, 0.37317633
 
 
 def fused_J(v, p00, p11, H, W):
-    """(J00, J11, J20, J21) of fused_J for view-space positions v [3,N] (tx, ty, tz)."""
+    """(J00, J11, J20, J21) of lgs_ray_J for view-space positions v [3,N] (tx, ty, tz)."""
     tx, ty, tz = v
     fx, fy = p00 * W * 0.5, p11 * H * 0.5
     lx, ly = tz / p00 * 1.3, tz / p11 * 1.3
@@ -51,7 +51,7 @@ def _axis_backward(p, n, t, tz, rz, rz2, dJd, dJ2):
 
 
 def J_backward(v, p00, p11, H, W, dJ00, dJ11, dJ20, dJ21):
-    """Back-propagation through fused_J as written -> (dv [3,N], d p00 [N], d p11 [N]).  Each clamp passes the gradient to the
+    """Back-propagation through lgs_ray_J as written -> (dv [3,N], d p00 [N], d p11 [N]).  Each clamp passes the gradient to the
     operand it returned, the position at a tie; below the 0.01 depth floor rz is constant."""
     tx, ty, tz = v
     rz = 1.0 / np.maximum(tz, 1e-2)

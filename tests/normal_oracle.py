@@ -13,7 +13,7 @@ import oracle
 
 
 def quat_R(qn):
-    """Rotation matrix rows [9,N] of unit quaternions qn [4,N] (r, x, y, z), laid out as fused_quat_R."""
+    """Rotation matrix rows [9,N] of unit quaternions qn [4,N] (r, x, y, z), laid out as lgs_quat_R."""
     r, x, y, z = qn
     return np.stack([1 - 2 * (y * y + z * z), 2 * (x * y + r * z), 2 * (x * z - r * y),
                      2 * (x * y - r * z), 1 - 2 * (x * x + z * z), 2 * (y * z + r * x),

@@ -44,7 +44,7 @@ def sh_basis(deg, d):
 
 
 def _clamp_pos(t, l, pred=None):
-    """max(min(t, l), -l) as fused_J writes it: the gradient goes to the operand returned, at a tie to t.  pred: the two decisions
+    """max(min(t, l), -l) as lgs_ray_J writes it: the gradient goes to the operand returned, at a tie to t.  pred: the two decisions
     (t > l, min(t, l) < -l) to take instead of comparing here."""
     up = t > l if pred is None else pred[0]
     m = torch.where(up, l, t)
@@ -52,7 +52,7 @@ def _clamp_pos(t, l, pred=None):
 
 
 def clamp_decisions_fp32(v, P):
-    """fused_J's clamp decisions [4,N] made in fp32, with the limit l = (tz / p) * 1.3 rounded as the kernel rounds it, from the
+    """lgs_ray_J's clamp decisions [4,N] made in fp32, with the limit l = (tz / p) * 1.3 rounded as the kernel rounds it, from the
     fp32-rounded view position (exactly the kernel's under an axis camera, whose view position is the world position)."""
     f = lambda a: np.asarray(a, np.float64).astype(np.float32)
     tz = f(v[2])
@@ -64,7 +64,7 @@ def clamp_decisions_fp32(v, P):
 
 
 def camera_J(v, P, hw, pred=None):
-    """J [N,3,2] of view positions v [4,N] under P [N,4,4] (fused_J); pred: clamp decisions [4,N] (clamp_decisions_fp32) or None."""
+    """J [N,3,2] of view positions v [4,N] under P [N,4,4] (lgs_ray_J); pred: clamp decisions [4,N] (clamp_decisions_fp32) or None."""
     H, W = hw
     p00, p11 = P[:, 0, 0], P[:, 1, 1]
     fx, fy = p00 * W * 0.5, p11 * H * 0.5
@@ -306,7 +306,7 @@ def constructed_cases():
     ax = cams["axis"]
     out = {}
     rq = lambda n: rng.normal(size=(n, 4))
-    # J clamp: view-space x/z and y/z just inside, exactly at (in fp32, as fused_J forms the limit) and beyond 1.3/P00 (1.3/P11), on
+    # J clamp: view-space x/z and y/z just inside, exactly at (in fp32, as lgs_ray_J forms the limit) and beyond 1.3/P00 (1.3/P11), on
     # both sides of both axes; the splats are large enough to reach the image
     xyz, s = [], []
     z = np.float32(2.0)
