@@ -492,3 +492,53 @@ def fragile(ref, view, *, exact=False, aa=False):
             l = np.abs(v[2] / p * 1.3)
             out |= np.abs(np.abs(t) - l) <= 4 * u * l
     return out
+
+
+def _quat_R_abs(qn):
+    """The absolute terms of each entry of quat_R [N,3,3] at unit quaternions qn [4,N]: |1| of a diagonal entry is replaced by
+    |R_aa| (1 - 2 (y^2 + z^2) rounds to a few ulps of its result plus 2 (y^2 + z^2)), 2 (|xy| + |rz|) off the diagonal."""
+    r, x, y, z = qn.abs()
+    R = quat_R(qn).abs()
+    d = [2 * (y * y + z * z), 2 * (x * x + z * z), 2 * (x * x + y * y)]
+    off = lambda a, b, c, e: 2 * (a * b + c * e)
+    return torch.stack([torch.stack([R[:, 0, 0] + d[0], off(x, y, r, z), off(x, z, r, y)], -1),
+                        torch.stack([off(x, y, r, z), R[:, 1, 1] + d[1], off(y, z, r, x)], -1),
+                        torch.stack([off(x, z, r, y), off(y, z, r, x), R[:, 2, 2] + d[2]], -1)], 1)
+
+
+def conversion_magnitude(params, view, proj, hw, m, *, filt=None):
+    """The error the kernel's fp32 conic carries into its record gradient where the off-diagonal of the 2D covariance is below its
+    own rounding, through the position and the camera -> dict(xyz [3,N], cam_each [N,2,4,4], where [N] bool).
+
+    The kernel turns the raw moments into the position's record gradient with its own conic: g_px = -(A m0 + B m1), g_py =
+    -(B m0 + C m1) (lgs_record_grad).  Its covariance c = M^T M + 0.3 I sums products of M = diag(s) R (V3 J).  Each rotation
+    entry is a few fp32 roundings of its absolute terms (_quat_R_abs): 1 - 2 (y^2 + z^2) is a few ulps of 1 off even where it is
+    nearly 0.  So M[a][c] is off by dM[a][c] = 2^-21 s_a sum_k Rabs[a][k] |VJ[k][c]| (8 ulps), and c_ij by
+    dc_ij = sum_a (dM[a][i] |M[a][j]| + |M[a][i]| dM[a][j]) + 2^-22 sum_a |M[a][i] M[a][j]|.  Where |c01| > dc01 this is an
+    error relative to the covariance's own terms, which 1e-6 |J|^T |g| and the conditioning term already bound.  Where |c01| <= dc01
+    (a needle along a screen axis under a rotation that rounds, whose fp64 B is about 0), B's error times the needle's m1 is far
+    above 1e-6 |J|^T |g|, which only sees the fp64 B: there this returns d inv = |inv| dc |inv|, d g_px = dA |m0| + dB |m1|,
+    d g_py = dB |m0| + dC |m1|, carried by |d px / d .| and |d py / d .|; elsewhere zero."""
+    t = lambda a: torch.as_tensor(np.asarray(a, np.float64))
+    th, Vm, P = leaves(dict(params, sh=np.asarray(params["sh"])[:1]), view, proj)
+    f = None if filt is None else t(filt)
+    rec, it = record(th, Vm, P, hw, 0, filt=f)
+    ins = [th["xyz"], Vm, P]
+    jx = torch.autograd.grad(rec[0].sum(), ins, retain_graph=True)
+    jy = torch.autograd.grad(rec[1].sum(), ins)
+    with torch.no_grad():
+        VJ, M, s = it["VJ"].abs(), it["M"].abs(), it["s"].T                     # [N,3,2], [N,3,2], [N,3]
+        dM = 2.0 ** -21 * s[:, :, None] * torch.einsum("nak,nkc->nac", _quat_R_abs(it["qn"]), VJ)
+        T = torch.einsum("nai,naj->nij", dM, M)
+        dc = T + T.transpose(1, 2) + 2.0 ** -22 * torch.einsum("nai,naj->nij", M, M)
+        where = it["c01"].abs() <= dc[:, 0, 1]
+        A, B, C = rec[2].abs(), rec[3].abs(), rec[4].abs()
+        inv = torch.stack([torch.stack([A, B], -1), torch.stack([B, C], -1)], 1)
+        dinv = (inv @ dc @ inv) * where[:, None, None]
+        mm = t(m).abs().T
+        dgx = dinv[:, 0, 0] * mm[0] + dinv[:, 0, 1] * mm[1]
+        dgy = dinv[:, 0, 1] * mm[0] + dinv[:, 1, 1] * mm[1]
+        xyz = jx[0].abs() * dgx + jy[0].abs() * dgy
+        cam = torch.stack([jx[1].abs() * dgx[:, None, None] + jy[1].abs() * dgy[:, None, None],
+                           jx[2].abs() * dgx[:, None, None] + jy[2].abs() * dgy[:, None, None]], 1)
+    return dict(xyz=xyz.numpy(), cam_each=cam.numpy(), where=where.numpy())

@@ -13,7 +13,8 @@ the record map is well conditioned; the third where the backward's terms cancel 
 axis, the long-axis scale of screen-sized needles).  The families in CONDITIONED (screen-sized needles, rho down to 1e-3, the
 rotated camera's needles) add 2^-22 (kappa_c + kappa_aa) (|J|^T |g|): the kernel evaluates the conic and the antialiasing factor in
 fp32, and entries of M^T M rounded to a few ulps move the determinants by a few ulps of kappa_c = (|c00 c11| + c01^2) / |det| and
-kappa_aa = (a00 a11 + a01^2) / det(M^T M).  Gaussians whose branch decisions are within rounding of flipping (project_grad_oracle.
+kappa_aa = (a00 a11 + a01^2) / det(M^T M).  The needles along a screen axis (CONVERSION) add to the position and camera bars
+the error the kernel's fp32 conic carries into the record gradient (project_grad_oracle.conversion_magnitude).  Gaussians whose branch decisions are within rounding of flipping (project_grad_oracle.
 fragile) are masked, taken out of the camera gradient, and counted.  Then the output forms, capacity-sized launches and
 camera_grad_sum_kernel.
 """
@@ -35,10 +36,14 @@ FLAGS = ("cam", "aa", "f3d", "exact", "depth", "normal")
 MODES = ([{f: False for f in FLAGS}] + [{f: f == g for f in FLAGS} for g in FLAGS] + [{f: True for f in FLAGS}] +
          [{f: f != g for f in FLAGS} for g in FLAGS])
 CASES = pg.constructed_cases()
-# The families held to the bar on the device: all but the needles (see DESIGN.md section 2, "Projection gradient coverage").
-HELD = tuple(f for f in CASES if f != "needles_sizes")
+# The families held to the bar on the device: all of them (see DESIGN.md section 2, "Projection gradient coverage").
+HELD = tuple(CASES)
 # Families whose conic or antialiasing factor is ill-conditioned (kappa up to 1e6): their bar carries the conditioning term.
-CONDITIONED = ("det1", "antialias", "rotated_camera")
+CONDITIONED = ("det1", "needles_sizes", "antialias", "rotated_camera")
+# Families with needles along a screen axis, whose fp32 conic carries an off-diagonal error far above the fp64 one into the
+# position's record gradient: their position and camera bars carry project_grad_oracle.conversion_magnitude, which is zero
+# except where the covariance's off-diagonal is below its own fp32 rounding.
+CONVERSION = ("needles_sizes",)
 CHAIN = 2.0 ** -20                 # 16 ulps of the backward's own absolute terms (project_grad_oracle.chain_magnitude)
 
 
@@ -151,7 +156,8 @@ def _compare(kern, ref, bar, mask):
     return (float(r.max()) if r.size else 0.0), np.argwhere((err > bar) & mask)
 
 
-def _check_against_reference(sc, deg, mode, m_src, gn_src, ts, kern_out, d_cam, conditioned=False, masked_have_no_gradient=False):
+def _check_against_reference(sc, deg, mode, m_src, gn_src, ts, kern_out, d_cam, conditioned=False, masked_have_no_gradient=False,
+                             conversion=False):
     """Compare one launch with the reference -> (failures, largest err/bar, fragile Gaussians among the family's own)."""
     ref = sc.reference(deg, mode, m_src, gn_src, ts)
     K = (deg + 1) ** 2
@@ -159,6 +165,8 @@ def _check_against_reference(sc, deg, mode, m_src, gn_src, ts, kern_out, d_cam, 
     cond = 2.0 ** -22 * (kc + ka) if conditioned else np.zeros_like(kc)
     chain = pg.chain_magnitude(ref, sc.view, sc.hw, aa=mode["aa"], filt=sc.p["filt"] if mode["f3d"] else None, normal=mode["normal"],
                                exact=mode["exact"])
+    if conversion:
+        conv = pg.conversion_magnitude(sc.p, sc.view, sc.proj, sc.hw, m_src, filt=sc.p["filt"] if mode["f3d"] else None)
     fr = pg.fragile(ref, sc.view, exact=mode["exact"], aa=mode["aa"])
     mask = ~fr
     n_fragile = int(fr[:sc.N0].sum())                     # the padding repeats the family's first Gaussian
@@ -169,7 +177,11 @@ def _check_against_reference(sc, deg, mode, m_src, gn_src, ts, kern_out, d_cam, 
 
     def bar(k):
         b = 1e-4 * np.abs(ref["grads"][k]) + (1e-6 + cond) * ref["mag"][k]
-        return d(b + CHAIN * chain[k] if k in chain else b)
+        if k in chain:
+            b = b + CHAIN * chain[k]
+        if conversion and k == "xyz":
+            b = b + conv["xyz"]
+        return d(b)
     for k in ("xyz", "scale", "rot", "opacity"):
         kv = outs[k].reshape(*outs[k].shape[:-2], -1)
         w, bad = _compare(kv, d(ref["grads"][k]), bar(k), md)
@@ -187,6 +199,8 @@ def _check_against_reference(sc, deg, mode, m_src, gn_src, ts, kern_out, d_cam, 
         got = d_cam
         cref = (ref["cam_each"] * keep).sum(0)
         cbar = 1e-4 * np.abs(cref) + ((1e-6 + cond)[:, None, None, None] * ref["mag_cam_each"] * keep).sum(0)
+        if conversion:
+            cbar = cbar + (conv["cam_each"] * keep).sum(0)
         w, bad = _compare(got.reshape(-1), cref.reshape(-1), cbar.reshape(-1), np.ones(32, bool))
         worst = max(worst, w)
         if len(bad):
@@ -198,7 +212,7 @@ def _check_against_reference(sc, deg, mode, m_src, gn_src, ts, kern_out, d_cam, 
 def test_family_matches_fp64_reference(cuda, family):
     """Every mode pair at SH degrees 0 and 3 and both opacity conventions: each component of each Gaussian within the bar."""
     sc = Scene(cuda, CASES[family])
-    conditioned = family in CONDITIONED
+    conditioned, conversion = family in CONDITIONED, family in CONVERSION
     rng = np.random.default_rng(zlib.crc32(family.encode()))
     N = sc.N
     m_src, gn_src = _record_grad(N, rng, depth_only=(1,), normal_only=(2,), zero=(3,))
@@ -208,13 +222,14 @@ def test_family_matches_fp64_reference(cuda, family):
         for mi, mode in enumerate(MODES):
             for ts in (0, 1):
                 kern, d_cam, _ = sc.launch(deg, mode, m_dst, gn_dst, ts=ts)
-                f, w, nf, fr = _check_against_reference(sc, deg, mode, m_src, gn_src, ts, kern, d_cam, conditioned)
+                f, w, nf, fr = _check_against_reference(sc, deg, mode, m_src, gn_src, ts, kern, d_cam, conditioned,
+                                                        conversion=conversion)
                 if d_cam is not None and fr.any():
                     # the camera gradient without the masked Gaussians: their record gradient zeroed
                     m2, g2 = m_src.copy(), gn_src.copy()
                     m2[fr], g2[fr] = 0.0, 0.0
                     kern2, d_cam2, _ = sc.launch(deg, mode, sc.src_order(m2.T).T.copy(), sc.src_order(g2.T).T.copy(), ts=ts)
-                    f2, w2, _, _ = _check_against_reference(sc, deg, mode, m2, g2, ts, kern2, d_cam2, conditioned, True)
+                    f2, w2, _, _ = _check_against_reference(sc, deg, mode, m2, g2, ts, kern2, d_cam2, conditioned, True, conversion)
                     f += [x for x in f2 if x[0] == "cam"]
                     w = max(w, w2)
                 worst, nfrag = max(worst, w), max(nfrag, nf)

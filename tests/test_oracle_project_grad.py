@@ -124,3 +124,57 @@ def test_opacity_logit_factor():
     assert np.all(np.abs(new - want) <= 4 * 2.0 ** -24 * want * (1 + np.exp(-x)))    # below 0, sig = 1 - u has ulps of u / sig
     assert np.abs(old[-1] - want[-1]) > 1e-2 * want[-1]
     assert np.array_equal(pg.sigmoid_factor(x, False).numpy(), torch.sigmoid(torch.as_tensor(x)).numpy())
+
+
+def _conic_fp32(p, view, proj, hw):
+    """The conic (A, B, C) [3,N] in fp32 numpy by the kernel's formulas (lgs_normalize_quat, lgs_quat_R, lgs_ray_J, lgs_cov_M,
+    lgs_cov2d, lgs_inv2x2), for Gaussians in front of an axis camera, whose view position is the world position."""
+    f = np.float32
+    H, W = hw
+    q = np.asarray(p["rot"], f)
+    rn = f(1) / np.sqrt((q * q).sum(0) + f(1e-12))
+    r, x, y, z = q * rn
+    R = np.stack([np.stack([1 - 2 * (y * y + z * z), 2 * (x * y + r * z), 2 * (x * z - r * y)]),
+                  np.stack([2 * (x * y - r * z), 1 - 2 * (x * x + z * z), 2 * (y * z + r * x)]),
+                  np.stack([2 * (x * z + r * y), 2 * (y * z - r * x), 1 - 2 * (x * x + y * y)])]).astype(f)     # [3,3,N]
+    s = np.exp(np.asarray(p["scale"], f))
+    tx, ty, tz = np.asarray(p["xyz"], f)
+    P = np.asarray(proj, f)
+    fx, fy = P[0, 0] * f(W) * f(0.5), P[1, 1] * f(H) * f(0.5)
+    rz = f(1) / np.maximum(tz, f(1e-2))
+    z0 = np.zeros_like(tz)
+    J = np.stack([np.stack([fx * rz, z0]), np.stack([z0, fy * rz]), np.stack([-fx * tx * rz * rz, -fy * ty * rz * rz])])   # [3,2,N]
+    V3 = np.asarray(view, f)[:3, :3]
+    VJ = np.einsum("ak,kcn->acn", V3, J).astype(f)
+    M = np.einsum("akn,kcn->acn", (R * s[:, None, :]).astype(f), VJ).astype(f)
+    c00 = (M[0, 0] * M[0, 0] + M[1, 0] * M[1, 0] + M[2, 0] * M[2, 0]) + f(0.3)
+    c01 = M[0, 0] * M[0, 1] + M[1, 0] * M[1, 1] + M[2, 0] * M[2, 1]
+    c11 = (M[0, 1] * M[0, 1] + M[1, 1] * M[1, 1] + M[2, 1] * M[2, 1]) + f(0.3)
+    dr = f(1) / (c00 * c11 - c01 * c01)
+    return np.stack([c11 * dr, -c01 * dr, c00 * dr]).astype(np.float64)
+
+
+def test_conversion_magnitude_bounds_the_fp32_conic():
+    """conversion_magnitude on the needles: zero wherever c01 is above its own rounding, and for the 0-degree needles, whose
+    rotation (1, 0, 0, 0) is exact; non-zero for the needles along the screen's y axis; and above the position error that an fp32
+    conic by the kernel's formulas carries through lgs_record_grad's conversion."""
+    case = pg.constructed_cases()["needles_sizes"]
+    p, (view, proj), hw = case["params"], case["cam"], case["hw"]
+    N = p["xyz"].shape[1]
+    m = np.random.default_rng(0).normal(size=(N, 12))
+    out = pg.conversion_magnitude(p, view, proj, hw, m)
+    ang = [0, 10, 30, 45, 60, 90, 135]
+    along_y = [i for i in range(14) if ang[i % 7] == 90]
+    assert np.array_equal(np.flatnonzero(out["where"]), along_y)
+    assert np.all(out["xyz"][:, [0, 7]] == 0.0) and np.all(out["cam_each"][[0, 7]] == 0.0)
+    assert np.all(out["xyz"][:2, along_y] > 0.0)
+    th, Vm, P = pg.leaves(dict(p, sh=p["sh"][:1]), view, proj)
+    rec, _ = pg.record(th, Vm, P, hw, 0)
+    jx, = torch.autograd.grad(rec[0].sum(), th["xyz"], retain_graph=True)
+    jy, = torch.autograd.grad(rec[1].sum(), th["xyz"])
+    d = np.abs(_conic_fp32(p, view, proj, hw) - rec[2:5].detach().numpy())
+    dgx = d[0] * np.abs(m[:, 0]) + d[1] * np.abs(m[:, 1])
+    dgy = d[1] * np.abs(m[:, 0]) + d[2] * np.abs(m[:, 1])
+    err = jx.abs().numpy() * dgx + jy.abs().numpy() * dgy
+    assert np.all(err[:, along_y] <= out["xyz"][:, along_y]), (err[:, along_y], out["xyz"][:, along_y])
+    assert np.all(err[:, along_y].max(1)[:2] > 0.05 * out["xyz"][:2, along_y].max(1))     # the bound is not vacuous
