@@ -7,6 +7,7 @@
     python examples/train_colmap.py --make /tmp/synth_depth --depth-weight 0.1     # also supervise the expected depth
     python examples/train_colmap.py --make /tmp/synth_normal --normal-weight 0.1   # also supervise the rendered normals
     python examples/train_colmap.py --data /path/to/colmap --depth-normal-weight 0.1   # self-supervised depth-normal consistency
+    python examples/train_colmap.py --data /path/to/colmap --depth-normal-weight 0.1 --mesh mesh.ply   # ... and write a mesh
 
 Reads ``sparse/0/{cameras,images,points3D}.bin`` and ``images/*`` (litegs_b200.colmap; same files and conventions as the
 reference's ``litegs/io_manager/colmap.py`` + ``litegs/data.py``), initialises Gaussians from the SfM points the way
@@ -21,6 +22,9 @@ pixels, with N from the normal mode (DESIGN.md section 1, "Normals"); it compose
 With ``--depth-normal-weight W`` the loss gains W * mean(1 - n_d . N / |N|), n_d the normal of the surface the rendered expected
 depth unprojects to (litegs_b200.geometry, DESIGN.md section 1, "Depth-normal consistency"): it turns depth and normals on and
 needs no ``depths/`` or ``normals/`` directory, so it trains the geometry of a real capture; it composes with every option above.
+With ``--mesh PATH`` the trained model's expected depth from every training camera (the refined poses with ``--refine-poses``, the
+3D filter with ``--filter-3d``) is fused into a TSDF volume over the Gaussian centres and written as a coloured triangle mesh
+(litegs_b200.mesh, DESIGN.md section 1, "Mesh extraction").
 """
 import argparse
 import os
@@ -31,7 +35,7 @@ import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from litegs_b200 import colmap, dist as lgs_dist, geometry, optimizer, render, scene, ssim  # noqa: E402
+from litegs_b200 import colmap, dist as lgs_dist, geometry, mesh as lgs_mesh, optimizer, ply, render, scene, ssim  # noqa: E402
 from litegs_b200.arguments import PipelineParams  # noqa: E402
 from litegs_b200.dist import PARAM_ORDER  # noqa: E402
 
@@ -167,9 +171,11 @@ def depth_normal_angle(depth, trans, normal, proj):
 
 
 def train(root, iters=300, views_per_step=8, log=print, refine_poses=False, antialiased=False, filter_3d=False, exact_grad=False,
-          depth_weight=0.0, metrics=None, normal_weight=0.0, depth_normal_weight=0.0):
+          depth_weight=0.0, metrics=None, normal_weight=0.0, depth_normal_weight=0.0, mesh=None, mesh_resolution=256):
     """Returns (loss history, PSNR).  depth_weight > 0 adds the expected-depth term (the dataset must have depths/), normal_weight
     > 0 the normal term (the dataset must have normals/), depth_normal_weight > 0 the depth-normal consistency term (no targets).
+    mesh (a PLY path, optional): at the end, the mesh fused from all training cameras in a volume of mesh_resolution lattice
+    points along the longest axis of the Gaussian centres' box.
     metrics (a dict, optional) receives "ed_error": mean |ED - target| over the known pixels of 8 training views, when the dataset
     has depths, "normal_angle": their mean angle in degrees between N / |N| and the target, when it has normals, and
     "depth_normal_angle": the mean angle in degrees between N / |N| and n_d where both are defined, with depth_normal_weight > 0."""
@@ -180,7 +186,7 @@ def train(root, iters=300, views_per_step=8, log=print, refine_poses=False, anti
     fused.CONFIG["true_sigmoid_grad"] = True               # our own loops train with the true sigmoid derivative (SURVEY Q15)
     try:
         return _train(root, iters, views_per_step, log, refine_poses, antialiased, filter_3d, exact_grad, depth_weight, metrics,
-                      normal_weight, depth_normal_weight)
+                      normal_weight, depth_normal_weight, mesh, mesh_resolution)
     finally:
         fused.CONFIG["true_sigmoid_grad"] = keep
 
@@ -218,7 +224,7 @@ class _Poses:
 
 
 def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=False, filter_3d=False, exact_grad=False,
-           depth_weight=0.0, metrics=None, normal_weight=0.0, depth_normal_weight=0.0):
+           depth_weight=0.0, metrics=None, normal_weight=0.0, depth_normal_weight=0.0, mesh=None, mesh_resolution=256):
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", 0)))
     torch.cuda.set_device(dev)
     frames, xyz, rgb = load_dataset(root, dev=dev)
@@ -330,6 +336,16 @@ def _train(root, iters, views_per_step, log, refine_poses=False, antialiased=Fal
     if poses:
         moved = (poses.extr.detach() - extr0).abs()
         log(f"poses refined: mean |change| of the quaternions {float(moved[:, :4].mean()):.2e}, of the translations {float(moved[:, 4:].mean()):.2e}")
+    if mesh:
+        all_cams = poses.cameras(list(range(len(frames)))) if poses else [f[0] for f in frames]
+        vol = lgs_mesh.bounding_volume(P["xyz"], resolution=mesh_resolution)
+        A = list(scene.cluster_aabb_torch(P["xyz"], P["scale"], P["rot"], filter_3d=filt))
+        lgs_mesh.mesh_from_views(dict(P, cluster_origin=A[0], cluster_extend=A[1]), all_cams, (H, W),
+                                 PipelineParams(tile_size=(8, 16), antialiased=antialiased), vol, filter_3d=filt)
+        v, f, c = vol.extract()
+        ply.save_mesh_ply(mesh, v, f, c)
+        log(f"mesh fused from {len(all_cams)} training views in a {'x'.join(map(str, vol.dims))} volume: {len(v)} vertices, "
+            f"{len(f)} faces -> {mesh}")
     return hist, psnr
 
 
@@ -352,6 +368,8 @@ if __name__ == "__main__":
     ap.add_argument("--depth-normal-weight", type=float, default=0.0,
                     help="weight of the mean (1 - cos) term between N / |N| and the normal of the rendered expected depth (needs no "
                          "targets)")
+    ap.add_argument("--mesh", default=None, metavar="PATH", help="after training, write the mesh fused from the training views (PLY)")
+    ap.add_argument("--mesh-resolution", type=int, default=256, help="lattice points along the longest axis of the --mesh volume")
     ap.add_argument("--pose-noise", type=float, nargs=2, default=None, metavar=("DEG", "FRAC"),
                     help="with --make: perturb the written poses by DEG degrees and FRAC of the camera distance")
     a = ap.parse_args()
@@ -362,5 +380,5 @@ if __name__ == "__main__":
         ap.error("give --data or --make")
     h, _ = train(root, a.iters, refine_poses=a.refine_poses, antialiased=a.antialiased, filter_3d=a.filter_3d,
                  exact_grad=a.exact_grad, depth_weight=a.depth_weight, normal_weight=a.normal_weight,
-                 depth_normal_weight=a.depth_normal_weight)
+                 depth_normal_weight=a.depth_normal_weight, mesh=a.mesh, mesh_resolution=a.mesh_resolution)
     assert h[-1] < h[0]

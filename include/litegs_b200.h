@@ -438,6 +438,44 @@ int lgs_depth_normal(const float* depth, int depth_row_stride, const float* tran
                      int normal_row_stride, int normal_channel_stride, const float* proj, int H, int W, float alpha_min, float grad_scale,
                      float* n_d, float* d_depth, float* d_trans, float* d_normal, float* block_sums, void* stream);
 
+/* ---- mesh extraction (ours) ------------------------------------------------------------------------------------------ */
+
+/* TSDF fusion of a batch of V rendered views, ours (DESIGN.md section 1, "Mesh extraction").  The volume is a lattice of
+ * nx x ny x nz points, x fastest (fewer than 2^31 in all); point (i, j, k) sits at (ox, oy, oz) + (i, j, k) voxel_size.
+ *   tsdf, weight: f32[nz,ny,nx] on the device, read and written in place (a new volume holds 1 and 0);
+ *   color: f32[3,nz,ny,nx] (a new volume holds 0), or NULL for a volume without colour;
+ *   sdf_trunc: the truncation distance (> 0, world units);
+ *   depth, trans: f32[V,1,H,W], the depth mode's accumulated depth D and the transmittance T, contiguous;
+ *   rgb: f32[V,3,H,W], the rendered images, contiguous; NULL exactly when color is NULL;
+ *   view, proj: f32[V,4,4] on the device (row-vector convention); view in full, proj[0][0] and proj[1][1] are read;
+ *   alpha_min in [0, 1): pixels with 1 - T <= alpha_min are skipped; depth_far: expected depths beyond it are skipped (+inf: none).
+ * Per lattice point and view, in view order: z = (p~ V)[2] > 0.01, pixel (floor(u), floor(v)) of u = (x / z) fx + W/2,
+ * v = (y / z) fy + H/2 inside the image, alpha = 1 - T > alpha_min, ED = D / alpha <= depth_far, sdf = ED - z >= -sdf_trunc;
+ * then t = min(1, sdf / sdf_trunc), weight w -> w + 1, tsdf -> (tsdf w + t) / (w + 1), color -> (color w + clamp(rgb / alpha,
+ * 0, 1)) / (w + 1).  Exact fp32 order in DESIGN.md; no atomics (bit-reproducible, a batch gives the bits of its views one by
+ * one), no host synchronisation. */
+int lgs_tsdf_integrate(float* tsdf, float* weight, float* color, int nx, int ny, int nz, float ox, float oy, float oz, float voxel_size,
+                       float sdf_trunc, const float* depth, const float* trans, const float* rgb, const float* view, const float* proj,
+                       int V, int H, int W, float alpha_min, float depth_far, void* stream);
+/* Marching tetrahedra on the Freudenthal subdivision of the lattice's cells, first stage: per lattice point a (all outputs
+ * u8[nz,ny,nx] on the device)
+ *   vmask: bit d set when edge a -> a + d (d = x, y, z, x+y, x+z, y+z, x+y+z) belongs to a valid cell (all 8 corners with
+ *          weight >= weight_min) and its ends differ in tsdf < 0, i.e. carries a vertex;
+ *   vcount: the number of such edges (<= 7);
+ *   fcount: the number of triangles of the cell whose lower corner is a (<= 12; 0 for an invalid or missing cell).
+ * The caller scans vcount and fcount into int64 inclusive prefix sums for lgs_mesh_emit. */
+int lgs_mesh_count(const float* tsdf, const float* weight, int nx, int ny, int nz, float weight_min, unsigned char* vmask,
+                   unsigned char* vcount, unsigned char* fcount, void* stream);
+/* Second stage: the mesh in canonical order.  tsdf, color (nullable) as for lgs_tsdf_integrate; vmask, fcount from
+ * lgs_mesh_count; vert_end, face_end: i64[nz,ny,nx] inclusive prefix sums of vcount and fcount; n_vertices, n_faces: their
+ * totals, each below 2^31 (refused otherwise).  Outputs on the device:
+ *   vertices f32[n_vertices,3], ordered by (lattice point, edge direction), at p_a + (t_a / (t_a - t_b)) (p_b - p_a);
+ *   faces i32[n_faces,3], ordered by (cell, tetrahedron 0..5, triangle 0..1), wound with the right-hand normal toward tsdf >= 0;
+ *   vcolors u8[n_vertices,3] (NULL exactly when color is NULL): the same interpolation of the colour, times 255, rounded. */
+int lgs_mesh_emit(const float* tsdf, const float* color, int nx, int ny, int nz, float ox, float oy, float oz, float voxel_size,
+                  const unsigned char* vmask, const unsigned char* fcount, const long long* vert_end, const long long* face_end,
+                  long long n_vertices, long long n_faces, float* vertices, int* faces, unsigned char* vcolors, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -84,6 +84,9 @@ SIGNATURES = {
     "lgs_ssim_backward": [_P, _P, _P, _F, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P, _P],
     "lgs_depth_normal_num_block_sums": [_I, _I, ctypes.POINTER(_I)],
     "lgs_depth_normal": [_P, _I, _P, _I, _P, _I, _I, _P, _I, _I, _F, _F, _P, _P, _P, _P, _P, _P],
+    "lgs_tsdf_integrate": [_P, _P, _P, _I, _I, _I, _F, _F, _F, _F, _F, _P, _P, _P, _P, _P, _I, _I, _I, _F, _F, _P],
+    "lgs_mesh_count": [_P, _P, _I, _I, _I, _F, _P, _P, _P, _P],
+    "lgs_mesh_emit": [_P, _P, _I, _I, _I, _F, _F, _F, _F, _P, _P, _P, _P, ctypes.c_longlong, ctypes.c_longlong, _P, _P, _P, _P],
 }
 NO_STATUS = {"lgs_last_error": ctypes.c_char_p, "lgs_abi_version": ctypes.c_int}
 

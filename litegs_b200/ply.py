@@ -9,6 +9,8 @@ stored raw.  ``save_ply`` / ``load_ply`` keep the reference's signatures (``[C, 
 ``params_from_ply`` / ``params_to_ply`` convert to and from this package's clustered parameter dict.  Checkpoints trained with
 Mip-Splatting's 3D smoothing filter carry it as one more float property, ``filter_3D``, after ``rot_3``; it is written when given
 and read (by name) into the dict's ``"filter_3D"`` entry when the file has it.
+``save_mesh_ply`` / ``load_mesh_ply`` write and read triangle meshes (litegs_b200.mesh's output) in the binary layout MeshLab,
+Open3D and Blender read.
 """
 from __future__ import annotations
 
@@ -122,6 +124,85 @@ def params_from_ply(path: str, sh_degree: int = 3, chunk: int = 128, morton: boo
     out["cluster_origin"], out["cluster_extend"] = scene.cluster_aabb(out["xyz"], out["scale"], out["rot"])
     out["n_points"] = n
     return out
+
+
+def _numpy(a, dtype, name: str, cols: int = 3):
+    a = a.detach().cpu().numpy() if hasattr(a, "detach") else np.asarray(a)
+    if a.ndim != 2 or a.shape[1] != cols:
+        raise ValueError(f"{name} must be [N,{cols}], got {list(a.shape)}")
+    return np.ascontiguousarray(a, dtype)
+
+
+def save_mesh_ply(path: str, vertices, faces, colors=None) -> None:
+    """A triangle mesh as the binary little-endian PLY that MeshLab, Open3D and Blender read: element vertex (float x y z and,
+    with colours, uchar red green blue), element face (list uchar int vertex_indices).  vertices f32[M,3], faces i32[F,3],
+    colors u8[M,3] or None; numpy arrays or tensors of any device."""
+    v = _numpy(vertices, "<f4", "vertices")
+    f = _numpy(faces, "<i4", "faces")
+    fields = [("x", "<f4"), ("y", "<f4"), ("z", "<f4")]
+    if colors is not None:
+        c = _numpy(colors, "u1", "colors")
+        if c.shape[0] != v.shape[0]:
+            raise ValueError(f"colors has {c.shape[0]} rows, vertices {v.shape[0]}")
+        fields += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
+    vt = np.empty(v.shape[0], np.dtype(fields))
+    vt["x"], vt["y"], vt["z"] = v[:, 0], v[:, 1], v[:, 2]
+    if colors is not None:
+        vt["red"], vt["green"], vt["blue"] = c[:, 0], c[:, 1], c[:, 2]
+    ft = np.empty(f.shape[0], np.dtype([("n", "u1"), ("i", "<i4", (3,))]))
+    ft["n"], ft["i"] = 3, f
+    header = ("ply\nformat binary_little_endian 1.0\n" + f"element vertex {v.shape[0]}\n" + "".join(f"property float {a}\n" for a in "xyz")
+              + ("".join(f"property uchar {a}\n" for a in ("red", "green", "blue")) if colors is not None else "")
+              + f"element face {f.shape[0]}\nproperty list uchar int vertex_indices\nend_header\n")
+    d = os.path.dirname(path)
+    if d:
+        os.makedirs(d, exist_ok=True)
+    with open(path, "wb") as fh:
+        fh.write(header.encode("ascii"))
+        fh.write(vt.tobytes())
+        fh.write(ft.tobytes())
+
+
+def load_mesh_ply(path: str):
+    """save_mesh_ply's layout back -> (vertices f32[M,3], faces i32[F,3], colors u8[M,3] or None), numpy.  Other layouts (ASCII,
+    other vertex properties, polygons that are not triangles) are refused."""
+    with open(path, "rb") as fh:
+        if fh.readline().strip() != b"ply":
+            raise ValueError(f"{path}: not a PLY file")
+        lines = []
+        while True:
+            line = fh.readline()
+            if not line:
+                raise ValueError(f"{path}: header without end_header")
+            tok = line.decode("ascii", "replace").split()
+            if tok == ["end_header"]:
+                break
+            if tok and tok[0] != "comment":
+                lines.append(tok)
+        body = fh.read()
+    if ["format", "binary_little_endian", "1.0"] not in lines:
+        raise ValueError(f"{path}: only binary_little_endian 1.0 meshes are read")
+    els, cur = {}, None
+    for tok in lines:
+        if tok[0] == "element":
+            cur = els[tok[1]] = (int(tok[2]), [])
+        elif tok[0] == "property" and cur is not None:
+            cur[1].append(tuple(tok[1:]))
+    xyz = [("float", a) for a in "xyz"]
+    rgb = [("uchar", a) for a in ("red", "green", "blue")]
+    if set(els) != {"vertex", "face"} or els["vertex"][1] not in (xyz, xyz + rgb) or els["face"][1] != [("list", "uchar", "int", "vertex_indices")]:
+        raise ValueError(f"{path}: not a triangle mesh in save_mesh_ply's layout")
+    has_rgb = els["vertex"][1] == xyz + rgb
+    M, F = els["vertex"][0], els["face"][0]
+    vdt = np.dtype([("p", "<f4", (3,))] + ([("c", "u1", (3,))] if has_rgb else []))
+    fdt = np.dtype([("n", "u1"), ("i", "<i4", (3,))])
+    if len(body) < M * vdt.itemsize + F * fdt.itemsize:
+        raise ValueError(f"{path}: truncated")
+    vt = np.frombuffer(body, vdt, count=M)
+    ft = np.frombuffer(body, fdt, count=F, offset=M * vdt.itemsize)
+    if F and not (ft["n"] == 3).all():
+        raise ValueError(f"{path}: faces that are not triangles")
+    return (np.ascontiguousarray(vt["p"]), np.ascontiguousarray(ft["i"]), np.ascontiguousarray(vt["c"]) if has_rgb else None)
 
 
 def params_to_ply(path: str, params: dict, n_points: int | None = None) -> None:
